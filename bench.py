@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py -- throughput of the ZipNN hot path (compress + decompress) on B200.
+"""bench.py -- throughput of the ZipNN hot path (compress + decompress) on H100.
 
 Contract (see the task statement):  python bench.py --gpus N --steps K --warmup W [--impl reference]
 prints ONE JSON line on rank 0.
@@ -11,8 +11,8 @@ prints ONE JSON line on rank 0.
   e2e       the same metric through the host-buffer API (pinned host tensors; H2D and D2H
             inside the timed region).
   roofline  for the dominant kernel of the step, timed with CUDA events on its own stream.
-  cpu_baseline / --impl reference : the reference's own C path (oracle/_ref, compiled from
-            /root/reference) or, if that binary is absent, the oracle port, on the host cores.
+  cpu_baseline / --impl reference : the reference's own C path (oracle/_ref, compiled from the
+            reference's sources) or, if that binary is absent, the oracle port, on the host cores.
 """
 import argparse
 import json
@@ -42,6 +42,8 @@ def parse():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-sharded", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (the stream and the decompressed tensor) as .npy files")
     return ap.parse_args()
 
 
@@ -53,7 +55,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 class ClockSampler:
@@ -103,6 +105,33 @@ class ClockSampler:
         busy = sorted(sm)[len(sm) // 2:]  # upper half = samples under load
         return {"sm_mhz": sorted(busy)[len(busy) // 2], "sm_max_mhz": max(mx), "power_w_max": max(pw),
                 "samples": len(sm), "reasons": sorted(reasons)}
+
+
+def dump_outputs(out_dir, stream, tensor, suffix=""):
+    """Write the stream and the decompressed tensor of one step as .npy files (45 MiB at most): stream_length,
+    stream_head (the first MiB: header, type bytes, size table), and stream_sample / decompressed_sample, the
+    values at sorted positions drawn from a fixed seed (every value when the array is smaller than the sample).
+    Two builds run with the same arguments can so be compared file by file."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.default_rng(20240601)
+    flat = tensor.reshape(-1)
+
+    def sample(x, m):
+        if x.numel() <= m:
+            return x
+        idx = np.unique(rng.integers(0, x.numel(), m))
+        return x[torch.from_numpy(idx).to(x.device)]
+
+    arrays = {
+        "stream_length": np.array([stream.numel()], dtype=np.float64),
+        "stream_head": stream[: 1 << 20].float().cpu().numpy(),
+        "stream_sample": sample(stream, 4 << 20).float().cpu().numpy(),
+        "decompressed_sample": sample(flat, 6 << 20).float().cpu().numpy(),
+    }
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}{suffix}.npy"), a)
 
 
 def make_tensor(nbytes, dtype, device, seed):
@@ -281,7 +310,7 @@ def run_reference(args, rank, world):
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": round(1e3 * sample / (v * 1e9), 3),
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8", "data": "synthetic",
         "config": {"workload": workload_text(args.dtype, full),
-                   "l2": "inputs are far larger than the 126 MB L2 (no flush needed)", "sharding": "one tensor shard per GPU, no data-path collective"},
+                   "l2": "inputs are far larger than the 50 MB L2 (no flush needed)", "sharding": "one tensor shard per GPU, no data-path collective"},
         "timing": "host wall clock; the reference C path (zipnn_core.zipnn_core + combine_dtype) called directly, input clone outside the timed region, leaked result buffers freed by the harness between steps",
         "compress_gbs": round(sum(x[2] for x in vals) / len(vals), 4), "decompress_gbs": round(sum(x[3] for x in vals) / len(vals), 4),
         "ratio": round(vals[0][4], 6),
@@ -433,7 +462,9 @@ def run_ours(args, rank, local_rank, world):
         return s, d
 
     # ---- warm-up + exactness check (outside the timed region)
+    s = d = None
     for _ in range(max(args.warmup, 1)):
+        del s, d                   # the previous step's outputs go before the next step allocates its own
         s, d = step()
     assert torch.equal(d.view(torch.uint8), t.view(torch.uint8)), "round trip is not exact"
     stream_bytes = s.numel()
@@ -455,10 +486,14 @@ def run_ours(args, rank, local_rank, world):
         ev[2 * i + 1].record()
         d = ZipNN(input_format="torch").decompress(s)
         ev[2 * i + 2].record()
-        del s, d
+        if i + 1 < args.steps:
+            del s, d
     torch.cuda.synchronize()
     barrier()
     clk = clocks.stop() if rank == 0 else None
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, s, d, f"_rank{rank}" if world > 1 else "")
+    del s, d
     launches = _native.launch_count() - launches0
     ktimes = _native.timing_collect()
     _native.timing_enable(False)
@@ -610,16 +645,6 @@ def run_ours(args, rank, local_rank, world):
                    "algo_gbs": round(algo[k] / (v[0] * 1e-3) / 1e9, 1) if k in algo and v[0] > 0 else None,
                    "roofline_frac": round(algo[k] / (v[0] * 1e-3) / 1e9 / peak, 4) if k in algo and v[0] > 0 else None}
                for k, v in per_launch.items()}
-    # DRAM bytes per launch of the dominant kernel: recorded from one `ncu --set full` capture of the same
-    # workload (never measured under this run: ncu serialises and replays kernels); null when the
-    # workload differs from the recorded one.
-    traffic, traffic_src = None, None
-    try:
-        rec = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "traffic.json"))).get(dom)
-        if rec and rec.get("n_bytes") == N and dtype == torch.bfloat16:
-            traffic, traffic_src = rec["traffic_bytes_per_launch"], rec["source"]
-    except Exception:
-        pass
     # The north-star kernel (BASELINE.json: decompress) is no longer the longest one: its roofline next to `roofline`,
     # which stays the dominant kernel of the step as the contract says.
     north_star = None
@@ -627,11 +652,9 @@ def run_ours(args, rank, local_rank, world):
         ns = "k_huf_decode_fused"
         if ns in per_launch and per_launch[ns][0] > 0:
             ns_ms = per_launch[ns][0]
-            ns_rec = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "traffic.json"))).get(ns) or {}
-            ns_traffic = ns_rec.get("traffic_bytes_per_launch") if (ns_rec.get("n_bytes") == N and dtype == torch.bfloat16) else None
             north_star = {"kernel": ns, "bound": "hbm", "achieved": round(algo[ns] / (ns_ms * 1e-3) / 1e9, 1), "peak": peak, "unit": "GB/s",
                           "frac": round(algo[ns] / (ns_ms * 1e-3) / 1e9 / peak, 4), "ms_per_launch": round(ns_ms, 4),
-                          "algorithmic_bytes_per_launch": algo[ns], "traffic": ns_traffic}
+                          "algorithmic_bytes_per_launch": algo[ns]}
     except Exception:
         north_star = None
     line = {
@@ -639,14 +662,14 @@ def run_ours(args, rank, local_rank, world):
         "ms_per_step": round(step_ms, 3), "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "u8", "data": "synthetic",
         "config": {"workload": workload_text(args.dtype, nbytes),
-                   "l2": "inputs are far larger than the 126 MB L2 (no flush needed)", "sharding": "one tensor shard per GPU, no data-path collective"},
+                   "l2": "inputs are far larger than the 50 MB L2 (no flush needed)", "sharding": "one tensor shard per GPU, no data-path collective"},
         "compress_gbs": round(world * N / (tc_ms * 1e-3) / 1e9, 2), "decompress_gbs": round(world * N / (td_ms * 1e-3) / 1e9, 2),
         "ratio": round(Cb / N, 6),
         "path_roofline": {"compress_frac": round((N + Cb) / (tc_ms * 1e-3) / 1e9 / peak, 4),
                           "decompress_frac": round((N + Cb) / (td_ms * 1e-3) / 1e9 / peak, 4),
                           "note": "(N + C) / t / peak: SURVEY.md section 8d definition for the whole direction"},
         "roofline": {"bound": "hbm", "kernel": dom, "achieved": round(achieved, 1), "peak": peak, "unit": "GB/s",
-                     "frac": round(achieved / peak, 4), "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                     "frac": round(achieved / peak, 4), "peak_source": peak_src,
                      "algorithmic_bytes_per_launch": algo.get(dom, N), "ms_per_launch": round(dom_ms, 4)},
         "kernels": kernels,
         "north_star_kernel": north_star,

@@ -1,5 +1,5 @@
 /*
- * zipnn_b200.h -- C ABI of the B200-native ZipNN encode/decode path.
+ * zipnn_b200.h -- C ABI of the H100-native ZipNN encode/decode path.
  *
  * This is the drop-in boundary for the reference's native extension `zipnn_core`
  * (reference csrc/zipnn_core_module.c:9-23).  Entry points map one to one:

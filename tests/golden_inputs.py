@@ -4,8 +4,13 @@ Inputs are regenerated from a seed rather than committed; each manifest record
 carries the input sha256 so a test can tell "generator drifted" (skip) from
 "codec wrong" (fail).
 """
+import json
+import os
+
 import numpy as np
 import torch
+
+REF_CHECKS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_checks.json")
 
 _TORCH_DT = {
     "bfloat16": torch.bfloat16, "float16": torch.float16, "float32": torch.float32,
@@ -55,3 +60,10 @@ def raw_bytes(data) -> bytes:
     if data.numel() == 0:
         return b""
     return data.contiguous().reshape(-1).view(torch.uint8).numpy().tobytes()
+
+
+def load_ref_checks() -> dict:
+    """What the compiled reference returned on the seeded cases of test_oracle.py and
+    test_stream_windows.py (written by make_golden_ref_checks.py)."""
+    with open(REF_CHECKS) as f:
+        return json.load(f)

@@ -1,12 +1,13 @@
-"""The oracle (our C restatement) against the reference: committed golden streams, and the
-compiled reference itself when oracle/_ref is present.  CPU only."""
+"""The oracle (our C restatement) against the reference: committed golden streams, and what the
+compiled reference returned on seeded blocks and streams (tests/golden/ref_checks.json, written by
+tests/make_golden_ref_checks.py).  CPU only."""
 import hashlib
 
 import numpy as np
 import pytest
 
 from conftest import golden_stream, load_manifest
-from golden_inputs import make_input, raw_bytes
+from golden_inputs import load_ref_checks, make_input, raw_bytes
 from oracle import oracle as O
 from zipnn_b200 import ZipNN
 
@@ -38,10 +39,10 @@ def test_port_reproduces_reference_stream(rec):
     assert back.tobytes() == raw
 
 
-def test_port_matches_compiled_reference_blocks():
-    if O.ref_cdll() is None:
-        pytest.skip("oracle/_ref not built (needs /root/reference)")
+def block_inputs():
+    """-> [(src, dst capacity)]: the seeded HUF blocks compared with the reference's HUF_compress."""
     rng = np.random.default_rng(3)
+    cases = []
     for it in range(300):
         size = int(rng.choice([12, 13, 64, 257, 1500, 4096, 65536, 131072, int(rng.integers(1, 131073))]))
         kind = it % 5
@@ -57,15 +58,14 @@ def test_port_matches_compiled_reference_blocks():
             src = np.full(size, 7, dtype=np.uint8)
         else:
             src = np.minimum(rng.geometric(rng.uniform(0.02, 0.9), size), 255).astype(np.uint8)
-        cap = 256 * 1024 if it % 2 else 128 * 1024
-        assert O.huf_compress(src, cap) == O.ref_huf_compress(src, cap)
+        cases.append((src, 256 * 1024 if it % 2 else 128 * 1024))
+    return cases
 
 
-def test_port_matches_compiled_reference_streams():
-    ref = O.ref_core()
-    if ref is None:
-        pytest.skip("oracle/_ref not built (needs /root/reference)")
+def stream_inputs():
+    """-> [(header, data, G, bits, bytes_mode, chunk)]: the seeded streams compared with the reference's zipnn_core."""
     rng = np.random.default_rng(11)
+    cases = []
     for it in range(40):
         G = [1, 2, 4][it % 3]
         bits = (it // 3) % 2
@@ -80,7 +80,29 @@ def test_port_matches_compiled_reference_streams():
             data = np.ascontiguousarray((x.view(np.uint32) >> 16).astype(np.uint16).view(np.uint8)[:n])
         h = bytearray(32)
         h[0:2] = b"ZN"
-        r = bytes(ref.zipnn_core(bytes(h), bytearray(data.tobytes()), G, bits, bm, 0, chunk, 0.95, 10, 4))
+        cases.append((h, data, G, bits, bm, chunk))
+    return cases
+
+
+def test_port_matches_compiled_reference_blocks():
+    """HUF_compress of the port == the reference's: return code and output bytes."""
+    want = load_ref_checks()["huf_blocks"]
+    cases = block_inputs()
+    assert len(cases) == len(want)
+    for (src, cap), w in zip(cases, want):
+        assert sha(src) == w["input_sha256"], "the seeded input generator drifted"
+        r, out = O.huf_compress(src, cap)
+        assert (int(r), sha(out)) == (w["ret"], w["out_sha256"])
+
+
+def test_port_matches_compiled_reference_streams():
+    """zipnn_core of the port == the reference's stream, and the port decodes it back to the input
+    (the reference's combine_dtype did too when the golden data was written)."""
+    want = load_ref_checks()["streams"]
+    cases = stream_inputs()
+    assert len(cases) == len(want)
+    for (h, data, G, bits, bm, chunk), w in zip(cases, want):
+        assert sha(data) == w["input_sha256"], "the seeded input generator drifted"
         o = O.zipnn_compress(h, data, G, bits, bm, chunk, 0.95, threads=2).tobytes()
-        assert r == o
-        assert bytes(ref.combine_dtype(o[32:], G, bits, bm, chunk, n, 2)) == data.tobytes()
+        assert (len(o), sha(o)) == (w["stream_len"], w["stream_sha256"])
+        assert O.zipnn_decompress(np.frombuffer(o[32:], dtype=np.uint8), G, bits, bm, chunk, data.size, threads=2).tobytes() == data.tobytes()

@@ -5,9 +5,12 @@ alone; port vs the compiled reference).  GPU part: streams far larger than anyth
 oracle run could cover in seconds -- 9 GiB bf16 (the group-0 size table passes 2^32 at chunk 32768)
 and 6 GiB fp32 (groups 2 and 3 start beyond 2^32) -- compared with the oracle on windows that
 include the chunks around every 2^32 crossing (u64 size table, csrc/zipnn_core.c:145-153)."""
+import hashlib
+
 import numpy as np
 import pytest
 
+from golden_inputs import load_ref_checks
 from oracle import oracle as O
 from tools.stream_windows import StreamTables, check_stream_windows, compare_window
 
@@ -16,6 +19,10 @@ def _hdr():
     h = bytearray(32)
     h[0:2] = b"ZN"
     return h
+
+
+def sha(b):
+    return hashlib.sha256(bytes(b)).hexdigest()
 
 
 def _gauss_bytes(rng, n, esz):
@@ -50,19 +57,26 @@ def test_windows_of_an_oracle_stream_match_the_chunks_compressed_alone(G, bits, 
         check_stream_windows(bad, 32, G, K, chunk, n, lambda a, b: data[a:b], [(3, 7)], comp)
 
 
-def test_windows_against_the_compiled_reference():
-    ref = O.ref_core()
-    if ref is None:
-        pytest.skip("oracle/_ref not built (needs /root/reference)")
+def window_input():
+    """-> (data, chunk, G, K, windows): the stream whose windows are compared with the reference's."""
     rng = np.random.default_rng(8)
     chunk, G, K = 262144, 2, 9
-    n = K * chunk
-    data = _gauss_bytes(rng, n, 2)
+    return _gauss_bytes(rng, K * chunk, 2), chunk, G, K, [(0, 3), (4, 9)]
+
+
+def test_windows_against_the_compiled_reference():
+    """Each window of the port's whole stream matches the port's stream of the window's chunks alone, and that
+    one is the reference's zipnn_core stream for the same bytes (sha256 in tests/golden/ref_checks.json)."""
+    want = load_ref_checks()["windows"]
+    data, chunk, G, K, wins = window_input()
     whole = O.zipnn_compress(_hdr(), data, G, 1, 10, chunk, 0.95, threads=4)
     tab = StreamTables(whole, 32, G, K)
-    for c0, c1 in [(0, 3), (4, 9)]:
-        r = np.frombuffer(bytes(ref.zipnn_core(bytes(_hdr()), bytearray(data[c0 * chunk: c1 * chunk].tobytes()), G, 1, 10, 0, chunk, 0.95, 10, 4)),
-                          dtype=np.uint8)
+    assert len(wins) == len(want)
+    for (c0, c1), w in zip(wins, want):
+        part = data[c0 * chunk: c1 * chunk]
+        assert [c0, c1, sha(part)] == [w["c0"], w["c1"], w["input_sha256"]]
+        r = O.zipnn_compress(_hdr(), part, G, 1, 10, chunk, 0.95, threads=4)
+        assert (r.size, sha(r)) == (w["stream_len"], w["stream_sha256"])
         assert compare_window(tab, c0, c1, r, 32) > 0
 
 

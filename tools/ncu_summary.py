@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""Summarise an .ncu-rep (ncu --set full) into the few numbers DESIGN.md and bench.py quote.
-usage: python tools/ncu_summary.py gpurun_out/x.ncu-rep > profiles/x.summary.txt"""
+"""Summarise an .ncu-rep (ncu --set full) into a few numbers: DRAM traffic, issue activity, stall reasons.
+usage: python tools/ncu_summary.py x.ncu-rep > x.summary.txt"""
 import csv
 import io
 import subprocess

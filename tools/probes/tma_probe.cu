@@ -1,5 +1,5 @@
-// tma_probe.cu -- validates the TMA descriptor shapes the decode kernel relies on (run on the B200 box).
-//   nvcc -O2 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o tma_probe tma_probe.cu && ./tma_probe
+// tma_probe.cu -- validates the TMA descriptor shapes the decode kernel relies on (run on an H100).
+//   nvcc -O2 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tma_probe tma_probe.cu && ./tma_probe
 // 1. a byte tensor {seg + 16, rows} with row stride seg (rows overlap by 16 bytes): does cuTensorMapEncodeTiled accept it?
 // 2. 2-D box loads at an arbitrary byte x coordinate (the unaligned raw plane inside a stream), SWIZZLE_32B / 64B / NONE
 // 3. 2-D box store {128, 32} with SWIZZLE_128B from a [32][128] stage

@@ -1,4 +1,4 @@
-"""zipnn_b200 -- the ZipNN encode/decode hot path on B200 (sm_100a).
+"""zipnn_b200 -- the ZipNN encode/decode hot path on H100 (sm_90a).
 
 Drop-in for the reference package surface that sits on the hot path
 (reference zipnn/__init__.py:1):  `ZipNN`, `zipnn_safetensors`, `zipnn_hf` (the transformers

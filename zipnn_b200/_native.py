@@ -14,7 +14,7 @@ import threading
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(CSRC, "libzipnn_b200.so")
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-diag-suppress", "128", "-Xcompiler", "-fPIC", "-shared"]
 
 OK, E_ARG, E_CAPACITY, E_CORRUPT, E_CUDA, E_UNSUPPORTED = 0, 1, 2, 3, 4, 5
@@ -41,7 +41,7 @@ def sources():
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/zipnn_b200.cu for sm_100a into csrc/libzipnn_b200.so (no GPU needed)."""
+    """Compile csrc/zipnn_b200.cu for sm_90a into csrc/libzipnn_b200.so (no GPU needed)."""
     newest = max(os.path.getmtime(p) for p in sources())
     if not force and os.path.exists(LIB_PATH) and os.path.getmtime(LIB_PATH) >= newest:
         return LIB_PATH

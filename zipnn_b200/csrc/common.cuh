@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for the zipnn_b200 kernels (sm_100a).
+// common.cuh -- shared device helpers for the zipnn_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -32,7 +32,7 @@
 #endif
 #define ZB_SIDE_SLOTS 4  // 16-byte cp.async slots per lane and side plane of the fused kernel.  2 would do (block k+3 is
                          // requested two iterations before it is read) and saves 1 KiB per plane, but a cp.async into a slot
-                         // that an LDS read an instant earlier is slow on B200: 9.65 ms instead of 8.52 (profiles/r2_decode_probe.txt)
+                         // that an LDS read an instant earlier is slow
 #endif
 
 namespace zb {
@@ -255,7 +255,7 @@ __global__ void k_batch_errors(BatchCfg B) {
 // filled with cp.async (16-byte, L2-only) two iterations ahead of use.  Registers never
 // wait on a global load: a per-lane "prefetch into a register" does not work on a GPU,
 // because lanes refill at different symbols while the scoreboard is per warp, so every
-// refill ends up waiting for some other lane's load (measured: 234 clk/symbol).
+// refill ends up waiting for some other lane's load.
 // The refill itself is branch-free: every second symbol all lanes execute the same
 // select/shift/LDS sequence, whether or not their window needed a word.
 // ====================================================================================
@@ -811,7 +811,7 @@ __global__ void __launch_bounds__(32) k_huf_decode_planar(DecodeCfg cfg) {
 // of elements.
 //
 // Persistent: the grid is (SM count x resident warps per SM) one-warp CTAs and CTA i takes
-// the chunk groups i, i + grid, ...  A bitstream is serial, so a group costs the same ~2 ms
+// the chunk groups i, i + grid, ...  A bitstream is serial, so a group costs the same time
 // however the launch is shaped; with one CTA per group the last, partial wave lands on a
 // few SMs that run it at full-wave speed while the rest idle.  A static round-robin leaves
 // every SM the same share of the remainder.
@@ -863,7 +863,7 @@ __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bu
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // Shared memory of one warp (dynamic; offsets from the 1 KiB aligned base, A = its shared address).  The number of
-// resident warps is what the kernel's speed follows (DESIGN.md 3.1: 8 warps/SM 12.0 ms ... 15 warps 8.4 ms), and
+// resident warps is what the kernel's speed follows (DESIGN.md 3.1), and
 // shared memory is what limits it, so nothing here is slack:
 //   PB = 5 (bf16 / fp32 exponent planes):
 //     cols  [32][32] u16   2 KiB   private 5-bit columns; must start on a 2 KiB boundary of the shared
@@ -918,7 +918,7 @@ __device__ __forceinline__ FusedSmem fused_smem_carve(unsigned char* raw) {
   S.base_s = (uint32_t)__cvta_generic_to_shared(raw);
   // Opaque from here on: ptxas otherwise treats every address derived from it as "window base + constant"
   // and REBUILDS the base (S2R SR_CgaCtaId, MOV, LEA) at each use -- three extra instructions per symbol
-  // in front of the predicated tail lookup (measured: +13 % instructions, 8.7 -> 10.4 ms).
+  // in front of the predicated tail lookup.
   asm volatile("" : "+r"(S.base_s));
   uint32_t at;
   if (PB == 0) {
@@ -1330,8 +1330,8 @@ __global__ void __launch_bounds__(32, G == 4 ? 12 : ZB_FUSED_MIN_BLOCKS) k_huf_d
                 emit_elements<G>(pl, rot_mask, stage, lane, (tr * kTI + ki) * G);
               }
             }
-            // (a bulk tensor store of the 32 rows instead of these 8 x (LDS.128 + STG.128) was measured here too:
-            //  7.35 ms against 7.35 -- the fence and the wait for the store's reads cost what the LSU work saves)
+            // (a bulk tensor store of the 32 rows instead of these 8 x (LDS.128 + STG.128) is ZIPNN_B200_TMA=1: the fence
+            //  and the wait for the store's reads cost what the LSU work saves)
             __syncwarp();
             if (chunk_256k) {
 #pragma unroll

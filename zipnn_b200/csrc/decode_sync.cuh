@@ -1,7 +1,7 @@
 // decode_sync.cuh -- intra-stream parallel Huffman decode for small and medium tensors.
 //
 // k_huf_decode_fused gives every huff0 bitstream ONE thread (huf_decompress.c:203-260 is a serial
-// loop: symbol i+1 starts where symbol i ends), so a decode takes ~2 ms whether the tensor has 4
+// loop: symbol i+1 starts where symbol i ends), so a decode takes the same time whether the tensor has 4
 // chunks or 20 000.  Huffman codes self-synchronise: a decoder started at a wrong bit position
 // falls into step with the true parse after a few symbols.  This kernel uses that (Klein & Wiseman;
 // Weissenberger & Schmidt for GPUs), with the reference's stream format untouched:
@@ -25,7 +25,7 @@
 //      the general regroup (several coded groups, ragged tail), copies the quarter plane to the
 //      chunk's workspace plane.
 // About 2.6 decode passes instead of 1, but over 256 threads per bitstream instead of 1: a 1 MiB
-// tensor is 16 CTAs x tens of microseconds instead of 16 threads x 1.5 ms.  The bitstream is copied into shared
+// tensor is 16 CTAs of short passes instead of 16 threads that each walk a whole bitstream.  The bitstream is copied into shared
 // memory once and every pass reads it there; one full 2^11-entry table per CTA (built by 256 threads, from the
 // weights k_parse_tables extracted once per item), so no two-level lookup.
 #pragma once

@@ -58,7 +58,6 @@ __device__ __forceinline__ uint32_t rot_byte_at(const uint8_t* __restrict__ in_c
 // =====================================================================================
 // Columns per bin.  32 = one per lane: no two lanes of a warp ever meet in a bank (1 wavefront per
 // atomic instead of 2), at 32 KiB of counters per plane; fp32 has four planes and keeps 16.
-// Measured on 16 GiB bf16: 16 columns 5.84 ms, 32 columns 5.07 ms, + two quarters per fold 4.61 ms.
 template <int G>
 struct HistCfg {
   static constexpr int R = (G == 4) ? 16 : 32;
@@ -122,7 +121,7 @@ __global__ void __launch_bounds__(kEncThreads) k_encode_hist(const uint8_t* __re
                   // byte b of the word -> address of its counter in THREE instructions: extract (PRMT with zeros),
                   // bin * (R * 4) + this lane's column (one multiply-add on the FMA pipe), shared-memory reduction
                   // with the plane as an immediate offset.  (Shift, mask | column, add the array base, ATOMS took four,
-                  // and the kernel is bound by instruction issue: profiles/r2p_encode_16GiB.summary.txt)
+                  // and the kernel is bound by instruction issue)
                   const uint32_t byte = __byte_perm(w[i], 0u, 0x4440u | (uint32_t)b);
                   atomicAdd(reinterpret_cast<uint32_t*>(col_p + ((4 * i + b) % G) * (256 * R * 4) + byte * (uint32_t)(R * 4)), inc);
                 }

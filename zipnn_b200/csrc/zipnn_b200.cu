@@ -1,6 +1,6 @@
-// zipnn_b200.cu -- C ABI (include/zipnn_b200.h) over the sm_100a kernels.
+// zipnn_b200.cu -- C ABI (include/zipnn_b200.h) over the sm_90a kernels.
 //
-// Build:  nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -lineinfo \
+// Build:  nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo \
 //              -Xcompiler -fPIC -shared -o libzipnn_b200.so zipnn_b200.cu
 #include "../../include/zipnn_b200.h"
 
@@ -98,7 +98,7 @@ int sm_count_cached() {
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
       cached = n;
     else
-      return 148;
+      return 132;
   }
   return cached;
 }
@@ -135,7 +135,6 @@ bool byte_map_2d(CUtensorMap* m, const void* base, uint64_t inner, uint64_t rows
 
 struct Knobs {
   int tma = 2, grid_mode = 1, warps_per_sm = 0;  // tma: 1 = bulk-tensor stores of the output rows, 2 = bulk-tensor tiles for the side plane.
-                                                 // measured: bulk stores and a persistent grid are 3-4 % slower (profiles/r2_decode_probe.txt)
   long long sync_max = -1;  // chunks up to which k_huf_decode_sync replaces the one-thread-per-bitstream kernels (-1: default)
   size_t smem_pad = 0;
 };
@@ -178,8 +177,8 @@ inline uint64_t num_chunks(size_t n, size_t chunk) { return (n + chunk - 1) / ch
 // general chunks, e.g. fp32 tensors upcast from bf16).
 constexpr uint64_t kDefaultSlots = 64;
 constexpr uint64_t kSyncTablesMaxChunks = 16384;  // largest tensor the sync decoder can be asked to take (ZIPNN_B200_SYNC_MAX is clamped to it)
-constexpr uint64_t kSyncDefaultMaxChunks = 4096;  // measured crossover with the one-thread-per-bitstream kernels (bf16): 256 MiB 0.39 vs
-                                                  // 1.5 ms, 1 GiB 1.45 vs 1.50 ms, 4 GiB ~5.7 vs 2.1 (profiles/r2_kernel_times.jsonl)
+constexpr uint64_t kSyncDefaultMaxChunks = 3072;  // crossover with the one-thread-per-bitstream kernels for one- and two-plane types
+                                                  // (H100 SXM at 400 W: they win up to 3072 chunks and lose from 3584 on)
 struct DecWs {
   size_t items_off, mode_off, slot_off, rlist_off, olist_off, hlist_off, tables_off, fill_off, planes_off, pstride, fixed;
 };
@@ -341,8 +340,8 @@ static int fill_decode_cfg(DecodeCfg& cfg, const void* d_body, size_t body_len, 
 static uint64_t sync_max_chunks(int G) {
   const Knobs kn = knobs();
   // four-plane types: the CTA's merge phase writes twice as much per decoded symbol, the crossover is lower
-  // (fp32 1 GiB: 1.68 ms against 1.29 for the one-thread kernel, profiles/r2_sweep_1gpu.jsonl)
-  const uint64_t dflt = G == 4 ? (kSyncDefaultMaxChunks * 3) / 4 : kSyncDefaultMaxChunks;
+  // (fp32 on the same H100: between 1536 and 2048 chunks)
+  const uint64_t dflt = G == 4 ? kSyncDefaultMaxChunks / 2 : kSyncDefaultMaxChunks;
   return std::min<uint64_t>(kn.sync_max >= 0 ? (uint64_t)kn.sync_max : dflt, kSyncTablesMaxChunks);
 }
 
@@ -357,8 +356,8 @@ int zipnn_b200_decompress(const void* d_body, size_t body_len, int num_buf, int 
   const uint64_t K = num_chunks(orig, chunk);
   cudaStream_t st = (cudaStream_t)cuda_stream;
   // Small and medium tensors: one CTA per bitstream (decode_sync.cuh) instead of one thread per bitstream.
-  // The one-thread kernels take ~2.2 ms for anything up to ~20 000 chunks (a bitstream is serial); the
-  // per-bitstream CTAs cost ~K * 0.7 us: crossover near 3000 chunks (measured on B200, profiles/r2c_sweep.txt).
+  // The one-thread kernels take about the same time for anything up to ~20 000 chunks (a bitstream is serial);
+  // the per-bitstream CTAs cost time in proportion to K, so they win below the crossover.
   const bool use_sync = K <= sync_max_chunks(G);
   DecodeCfg cfg;
   {

@@ -4,7 +4,7 @@ Mirrors reference zipnn/zipnn.py:1584-1643 (`decompress_safetensors_tensor`, `Sa
 `zipnn_safetensors`), scripts/zipnn_compress_safetensors.py:37-148 and
 scripts/zipnn_decompress_safetensors.py:34-136.
 
-B200 behaviour: `SafeOpen(..., device="cuda")` reads a compressed entry as uint8 bytes,
+GPU behaviour: `SafeOpen(..., device="cuda")` reads a compressed entry as uint8 bytes,
 moves the COMPRESSED bytes to the GPU, decodes there and returns a CUDA tensor, so a
 consumer such as vLLM's weight iterator (`for name in f.keys(): f.get_tensor(name)`) pays
 the H2D copy on ~2/3 of the bytes and the decode on the GPU.  With device="cpu" the tensor

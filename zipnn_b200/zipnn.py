@@ -1,4 +1,4 @@
-"""`ZipNN` -- host-side mirror of the reference codec object, routed to the B200 kernels.
+"""`ZipNN` -- host-side mirror of the reference codec object, routed to the CUDA kernels.
 
 Same constructor, same `compress()` / `decompress()` contract and the same stream bytes as
 reference `zipnn/zipnn.py:27-1218`; the native calls `zipnn_core.zipnn_core(...)`
@@ -141,7 +141,7 @@ class ZipNN:
         if self.method not in (EnumMethod.AUTO.value, EnumMethod.HUFFMAN.value):
             # reference: these need the optional zstandard / lz4 / snappy wheels and are only
             # reachable for one-group byte_reorder modes that no float dtype selects
-            raise ImportError(f"method {EnumMethod(self.method).name} is not part of the B200 path; use AUTO or HUFFMAN")
+            raise ImportError(f"method {EnumMethod(self.method).name} is not part of the GPU path; use AUTO or HUFFMAN")
         if self.lossy_compressed_type != EnumLossy.NONE and self.input_format != EnumFormat.TORCH.value:
             raise ValueError("When use lossy compression the input have to be torch.tensor")
 
@@ -504,10 +504,10 @@ class DecodePipe:
     """Decode many host- or file-resident streams onto one GPU without a host synchronisation per
     tensor (the load path: `SafeOpen(..., device="cuda")`, SURVEY.md section 8f N1).
 
-    One bitstream of a chunk is decoded serially, so a decode takes ~1.5 ms however small the tensor
+    One bitstream of a chunk is decoded serially, so a decode takes the same time however small the tensor
     is, and a checkpoint has hundreds of tensors.  `submit*` therefore (1) parses the header on the
     host, (2) moves the body through a ring of pinned 64 MiB slabs -- filled by a few threads with
-    `preadv` straight from the file (a memory-mapped source costs a page fault per 4 KiB: 2 GB/s) --
+    `preadv` straight from the file (a memory-mapped source costs a page fault per 4 KiB) --
     (3) enqueues the H2D copies and the decode on one of a few side streams, each of which owns its
     body and workspace buffers, with the error word left on the device, and (4) makes the caller's
     current stream wait for that decode: the tensor that comes back is safe to use on the current
