@@ -111,6 +111,28 @@ int zipnn_b200_decompress_batch_workspace_size(const zipnn_b200_batch_item* item
 int zipnn_b200_decompress_batch(const zipnn_b200_batch_item* items, int n, void* d_ws, size_t ws_bytes,
                                 void* cuda_stream, int check);
 
+/* ---- slices: a box of each stream's decoded bytes (sharded loads) --------------------------
+ * Row r of the box is decoded bytes [base + r*pitch, base + r*pitch + len), r in [0, rows); d_out
+ * receives the rows*len bytes packed row after row.  A slice of a row-major tensor along dim 0 is
+ * one row; along a later dim, one row per index of the dims in front of it.
+ * Only the chunks the box touches are read and validated: a chunk outside it is never dereferenced
+ * (the totals of the size table are still checked), so a corrupt byte there goes unnoticed.  Every
+ * item is decoded by the per-bitstream-CTA kernels, all items by ONE launch of each, whatever their
+ * size; a box that covers more than 16384 chunks is split into several pieces internally.
+ * E_ARG: a box past `orig`, len > pitch with rows > 1, or a misaligned d_out.  Empty boxes (rows or
+ * len 0) are valid and do nothing.  Status: OR of the items' error words, as in the batch call. */
+typedef struct zipnn_b200_slice_item {
+  const void* d_body; size_t body_len;   /* a whole stream after the python header, or a sub-stream of
+                                            consecutive chunks with rebased size rows                  */
+  int num_buf, bits_mode, bytes_mode;
+  size_t chunk, orig;                    /* orig = decoded bytes of THIS (sub)stream                    */
+  size_t base, rows, pitch, len;         /* the box, in the decoded bytes of this (sub)stream           */
+  void* d_out;                           /* rows*len bytes, 16-byte aligned                              */
+} zipnn_b200_slice_item;
+int zipnn_b200_decompress_slices_workspace_size(const zipnn_b200_slice_item* items, int n, size_t* out);
+int zipnn_b200_decompress_slices(const zipnn_b200_slice_item* items, int n, void* d_ws, size_t ws_bytes,
+                                 void* cuda_stream, int check);
+
 /* ---- stage 1 alone ------------------------------------------------------------ */
 /* d_planes: num_buf planes of `stride` bytes each; plane g receives byte g of every element
  * of the (optionally rotated) input.  Lengths as in the reference: n/num_buf, the first

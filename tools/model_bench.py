@@ -7,7 +7,11 @@ No network: the checkpoints are synthesised with the real tensor shapes and rand
 iterator does it (`with safe_open(f, framework="pt") as f: for name in f.keys(): f.get_tensor(name)`)
 through zipnn_b200.SafeOpen(device="cuda") -- compressed bytes H2D, decode on the GPU.
 
-usage: python tools/model_bench.py [gpt2|llama3-8b|granite-8b] [--layers N] [--dir /dev/shm]
+With --tp N the same file is loaded the way each rank of tensor-parallel N would load it (all ranks in turn on one
+GPU): column-parallel weights (q, k, v, gate, up, embedding, lm_head) by dim 0, row-parallel ones (o, down) by dim 1,
+through SafeOpen(slices=True) and through get_tensor + narrow, one JSON line per rank.
+
+usage: python tools/model_bench.py [gpt2|llama3-8b|granite-8b] [--layers N] [--dir /dev/shm] [--tp N]
 """
 import argparse
 import json
@@ -130,6 +134,92 @@ def load_chunk_sharded(path, rank, world, dev):
     return outs
 
 
+COLUMN_PARALLEL = ("q_proj", "k_proj", "v_proj", "gate_proj", "up_proj", "embed_tokens", "lm_head")   # sharded by dim 0
+ROW_PARALLEL = ("o_proj", "down_proj")                                                               # sharded by dim 1
+
+
+def tp_shard(name, shape, rank, world):
+    """(dim, start, stop) of rank's shard as transformers' get_tensor_shard cuts it (torch.chunk), or None for a
+    replicated tensor."""
+    kind = name.split(".")[-2]
+    dim = 0 if kind in COLUMN_PARALLEL else 1 if kind in ROW_PARALLEL else None
+    if dim is None or len(shape) < 2:
+        return None
+    size = -(-shape[dim] // world)
+    start = min(rank * size, shape[dim])
+    return dim, start, min(start + size, shape[dim])
+
+
+def load_tp_rank(path, rank, world, dev, slices):
+    """Every tensor of the file as rank `rank` of tensor-parallel `world` needs it: through CompressedSlice
+    (slices=True), or get_tensor + narrow.  -> ({name: tensor}, bytes read from the file, bytes copied H2D)."""
+    from zipnn_b200 import slicing
+    from zipnn_b200.safetensors_io import _safetensors_index
+    counted = [0]
+    orig_read, orig_into = slicing.FileSource.read, slicing.FileSource.read_into
+
+    def read(self, off, n):
+        counted[0] += n
+        return orig_read(self, off, n)
+
+    def read_into(self, off, mv):
+        counted[0] += len(mv)
+        return orig_into(self, off, mv)
+
+    got, plain = {}, 0
+    idx = _safetensors_index(path)
+    slicing.FileSource.read, slicing.FileSource.read_into = read, read_into
+    try:
+        with SafeOpen(path, "pt", str(dev), slices=slices) as f:
+            comp = f.compressed_tensors_metadata
+            for name in f.keys():
+                shape = json.loads(comp[name]["shape"]) if name in comp else f.get_slice(name).get_shape()
+                sh = tp_shard(name, shape, rank, world)
+                if name not in comp:
+                    plain += idx[name][1]
+                if slices:
+                    sl = f.get_slice(name)
+                    ix = (slice(None),) * sh[0] + (slice(sh[1], sh[2]),) if sh else slice(None)
+                    got[name] = sl[ix] if name in comp else sl[ix].to(dev)
+                elif sh is None:
+                    got[name] = f.get_tensor(name)
+                else:
+                    dim, a, b = sh
+                    got[name] = f.get_tensor(name).narrow(dim, a, b - a).contiguous()
+        torch.cuda.synchronize()
+    finally:
+        slicing.FileSource.read, slicing.FileSource.read_into = orig_read, orig_into
+    if not slices:   # the batched load path reads and uploads every compressed entry whole
+        counted[0] = sum(idx[k][1] for k in idx if k in comp)
+    return got, counted[0] + plain, counted[0] + plain
+
+
+def tp_bench(path, world, dev, model):
+    """One JSON line per rank of TP=world, all ranks in turn on one GPU: sliced reads next to get_tensor + narrow."""
+    from zipnn_b200 import _native
+    load_tp_rank(path, 0, world, dev, True)                  # warm-up (page cache, allocator, kernels)
+    load_tp_rank(path, 0, world, dev, False)
+    for rank in range(world):
+        row = dict(model=model, mode=f"tp rank {rank} of {world}", device=torch.cuda.get_device_name(dev))
+        outs = {}
+        for key, slices in (("slices", True), ("get_tensor_narrow", False)):
+            t0 = time.perf_counter()
+            got, nread, nh2d = load_tp_rank(path, rank, world, dev, slices)
+            wall = time.perf_counter() - t0
+            _native.timing_collect()
+            _native.timing_enable(True)
+            load_tp_rank(path, rank, world, dev, slices)
+            ker = _native.timing_collect()
+            _native.timing_enable(False)
+            row[key] = dict(wall_s=round(wall, 4), file_bytes_read=nread, h2d_bytes=nh2d,
+                            decode_kernel_ms=round(sum(ms for ms, _ in ker.values()), 3),
+                            decode_launches=sum(n for _, n in ker.values()))
+            outs[key] = got
+        row["exact"] = all(torch.equal(outs["slices"][k].view(torch.uint8), outs["get_tensor_narrow"][k].view(torch.uint8))
+                           for k in outs["slices"])
+        print(json.dumps(row), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("model", nargs="?", default="gpt2", choices=sorted(MODELS))
@@ -137,6 +227,8 @@ def main():
     ap.add_argument("--dir", default="/dev/shm")
     ap.add_argument("--keep", action="store_true")
     ap.add_argument("--sharded", action="store_true", help="under torchrun: every tensor partitioned by chunk range over the ranks")
+    ap.add_argument("--tp", type=int, default=0, help="load as each rank of tensor-parallel N would (one GPU, ranks in turn): "
+                                                      "sliced reads vs get_tensor + narrow, one JSON line per rank")
     args = ap.parse_args()
     rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
     shapes, dtype = MODELS[args.model](args.layers)
@@ -177,7 +269,9 @@ def main():
         torch.cuda.synchronize()
         return time.perf_counter() - t0, got
 
-    if args.sharded and world > 1:
+    if args.tp and rank == 0:
+        tp_bench(path, args.tp, dev, args.model)
+    elif args.sharded and world > 1:
         from zipnn_b200.sharded import byte_range
         load_chunk_sharded(path, rank, world, dev)          # warm-up
         torch.cuda.synchronize(); dist.barrier()

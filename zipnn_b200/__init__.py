@@ -7,10 +7,12 @@ plugin for `.znn` checkpoints, zipnn/zipnn.py:1221-1565; see hf.py for how it di
 from .zipnn import DecodePipe, ZipNN
 from .safetensors_io import (SafeOpen, compress_safetensors_file, decompress_safetensors_file,
                              decompress_safetensors_tensor, load_file, zipnn_safetensors)
+from .slicing import CompressedSlice
 
 
 from .hf import zipnn_hf
 
 
 __all__ = ["ZipNN", "zipnn_safetensors", "SafeOpen", "compress_safetensors_file",
-           "decompress_safetensors_file", "decompress_safetensors_tensor", "load_file", "DecodePipe", "zipnn_hf"]
+           "decompress_safetensors_file", "decompress_safetensors_tensor", "load_file", "DecodePipe", "zipnn_hf",
+           "CompressedSlice"]

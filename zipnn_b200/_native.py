@@ -29,6 +29,13 @@ class BatchItem(C.Structure):
                 ("bytes_mode", C.c_int), ("chunk", C.c_size_t), ("orig", C.c_size_t), ("d_out", C.c_void_p)]
 
 
+class SliceItem(C.Structure):
+    """zipnn_b200_slice_item (include/zipnn_b200.h)."""
+    _fields_ = [("d_body", C.c_void_p), ("body_len", C.c_size_t), ("num_buf", C.c_int), ("bits_mode", C.c_int),
+                ("bytes_mode", C.c_int), ("chunk", C.c_size_t), ("orig", C.c_size_t), ("base", C.c_size_t),
+                ("rows", C.c_size_t), ("pitch", C.c_size_t), ("len", C.c_size_t), ("d_out", C.c_void_p)]
+
+
 class ZipNNNativeError(RuntimeError):
     def __init__(self, status: int, msg: str):
         super().__init__(f"zipnn_b200: {msg} (status {status})")
@@ -81,6 +88,8 @@ def lib() -> C.CDLL:
                 "zipnn_b200_decompress": (i32, [vp, sz, i32, i32, i32, sz, sz, vp, vp, sz, vp, i32]),
                 "zipnn_b200_decompress_batch_workspace_size": (i32, [C.POINTER(BatchItem), i32, szp]),
                 "zipnn_b200_decompress_batch": (i32, [C.POINTER(BatchItem), i32, vp, sz, vp, i32]),
+                "zipnn_b200_decompress_slices_workspace_size": (i32, [C.POINTER(SliceItem), i32, szp]),
+                "zipnn_b200_decompress_slices": (i32, [C.POINTER(SliceItem), i32, vp, sz, vp, i32]),
                 "zipnn_b200_split": (i32, [vp, sz, i32, i32, vp, sz, vp]),
                 "zipnn_b200_regroup": (i32, [vp, sz, sz, i32, i32, vp, vp]),
                 "zipnn_b200_compress_host": (i32, [vp, sz, vp, sz, i32, i32, i32, sz, C.c_float, vp, sz, szp]),
@@ -102,7 +111,7 @@ EXPORTS = [
     "zipnn_b200_launch_count", "zipnn_b200_compress_bound", "zipnn_b200_compress_workspace_size",
     "zipnn_b200_decompress_workspace_size", "zipnn_b200_decompress_workspace_size_full", "zipnn_b200_compress",
     "zipnn_b200_decompress", "zipnn_b200_decompress_batch_workspace_size", "zipnn_b200_decompress_batch",
-    "zipnn_b200_split", "zipnn_b200_regroup", "zipnn_b200_compress_host", "zipnn_b200_decompress_host",
+    "zipnn_b200_decompress_slices_workspace_size", "zipnn_b200_decompress_slices", "zipnn_b200_split", "zipnn_b200_regroup", "zipnn_b200_compress_host", "zipnn_b200_decompress_host",
     "zipnn_b200_timing_enable", "zipnn_b200_timing_kernel_count", "zipnn_b200_timing_kernel_name",
     "zipnn_b200_timing_collect",
 ]

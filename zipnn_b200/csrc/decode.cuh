@@ -69,7 +69,75 @@ struct DecodeCfg {
   uint64_t k_full;      // chunks of full length (K, or K - 1 with a ragged last chunk)
   uint64_t side_pred[3];  // payload offset (inside body) of byte plane g's first item IF every group in front of it is all raw
   uint32_t side_r0[3];    // (body + side_pred[g]) & 15: the tensor maps start at the 16-byte boundary below
+  // Window over the decoded bytes (zipnn_b200_decompress_slices; batch kernels only): row r of the box is
+  // [box_base + r * box_pitch, + box_len), written packed to `out` at r * box_len.  box_len == 0: no window.
+  uint64_t box_base, box_rows, box_pitch, box_len;
+  uint64_t box_step_rows, box_step_cols;  // kBoxStep bytes as whole rows + columns: a thread's cursor advance per store step
+  uint32_t box_fast;                      // base, pitch and len are multiples of 16: every vector is in one row or outside
+  uint64_t c0;                            // first chunk the batch kernels visit (chunk_start counts from here)
 };
+
+// ---- the window's store path --------------------------------------------------------------------
+// Both output write sites (regroup_tile, the fused merge of sync_process) step a thread through the decoded
+// bytes kBoxStep at a time, so the row and column of its vector are computed once and then advanced.
+constexpr uint32_t kBoxStep = 4096;
+
+// Does the box meet decoded bytes [a, a + n)?  The first row whose end lies beyond a is the only candidate.
+__device__ __forceinline__ bool box_meets(const DecodeCfg& cfg, uint64_t a, uint64_t n) {
+  const uint64_t e0 = cfg.box_base + cfg.box_len;
+  const uint64_t r = a < e0 ? 0 : (a - e0) / cfg.box_pitch + 1;
+  return r < cfg.box_rows && cfg.box_base + r * cfg.box_pitch < a + n;
+}
+struct BoxCursor {
+  int64_t row;   // row of the vector's first byte (negative in front of the box)
+  uint64_t col;  // its offset from that row's start, in [0, box_pitch)
+};
+__device__ __forceinline__ BoxCursor box_cursor(const DecodeCfg& cfg, uint64_t v) {
+  BoxCursor k;
+  if (v >= cfg.box_base) {
+    const uint64_t q = (v - cfg.box_base) / cfg.box_pitch;
+    k.row = (int64_t)q;
+    k.col = v - cfg.box_base - q * cfg.box_pitch;
+  } else {
+    const uint64_t d = cfg.box_base - v, q = (d + cfg.box_pitch - 1) / cfg.box_pitch;
+    k.row = -(int64_t)q;
+    k.col = q * cfg.box_pitch - d;
+  }
+  return k;
+}
+__device__ __forceinline__ void box_advance(const DecodeCfg& cfg, BoxCursor& k) {
+  k.row += (int64_t)cfg.box_step_rows;
+  k.col += cfg.box_step_cols;
+  if (k.col >= cfg.box_pitch) {
+    k.col -= cfg.box_pitch;
+    k.row++;
+  }
+}
+// The 16 decoded bytes at the cursor (16-byte aligned in the decoded stream) -> those of them inside the box.
+// No store covers a byte outside the box: other CTAs own the rest of the output.
+__device__ __forceinline__ void box_store16(const DecodeCfg& cfg, uint8_t* __restrict__ out, const BoxCursor& k, const uint32_t (&r)[4]) {
+  if (cfg.box_fast) {
+    if (k.row >= 0 && (uint64_t)k.row < cfg.box_rows && k.col < cfg.box_len)
+      *reinterpret_cast<uint4*>(out + (uint64_t)k.row * cfg.box_len + k.col) = make_uint4(r[0], r[1], r[2], r[3]);
+    return;
+  }
+  int64_t row = k.row;
+  uint64_t col = k.col;
+#pragma unroll
+  for (int i = 0; i < 16; i++) {
+    if (row >= 0 && (uint64_t)row < cfg.box_rows && col < cfg.box_len) out[(uint64_t)row * cfg.box_len + col] = (uint8_t)(r[i >> 2] >> (8 * (i & 3)));
+    if (++col == cfg.box_pitch) {
+      col = 0;
+      row++;
+    }
+  }
+}
+// One decoded byte at v (the ragged tail of a stream's last chunk).
+__device__ __forceinline__ void box_put(const DecodeCfg& cfg, uint8_t* __restrict__ out, uint64_t v, uint8_t b) {
+  if (v < cfg.box_base) return;
+  const uint64_t q = (v - cfg.box_base) / cfg.box_pitch, col = v - cfg.box_base - q * cfg.box_pitch;
+  if (q < cfg.box_rows && col < cfg.box_len) out[q * cfg.box_len + col] = b;
+}
 
 
 // A chunk needs plane scratch (several coded groups, a ragged tail, or a table the fused kernel could not hold).
@@ -97,7 +165,9 @@ __device__ __forceinline__ uint32_t assign_general(const DecodeCfg& cfg, uint64_
 // Stream body layout (csrc/zipnn_core.c:105-244):
 //   types u8[G][K] | cum u64le[G][K] (inclusive, per group) | group-major payload
 // ====================================================================================
-// Chunks c = first, first + stride, ... of one tensor.
+// Chunks c = first, first + stride, ... of one tensor.  W: the tensor may carry a box; chunks outside it are
+// skipped before any of their table entries is read.
+template <bool W = false>
 __device__ __forceinline__ void decode_meta_body(const DecodeCfg& cfg, uint64_t first, uint64_t stride, bool leader) {
   const int G = cfg.G;
   const uint64_t K = cfg.K;
@@ -129,6 +199,10 @@ __device__ __forceinline__ void decode_meta_body(const DecodeCfg& cfg, uint64_t 
   }
   for (uint64_t c = first; c < K; c += stride) {
     const uint32_t chunk_len = (c == K - 1) ? (uint32_t)(cfg.orig - c * (uint64_t)cfg.chunk) : cfg.chunk;
+    if (W && cfg.box_len && !box_meets(cfg, c * (uint64_t)cfg.chunk, chunk_len)) {
+      cfg.mode[c] = (uint8_t)kModeSkip;
+      continue;
+    }
     int nhuf = 0, last_huf = -1;
     bool bad_chunk = !totals_ok;
     for (int g = 0; g < G; g++) {
@@ -234,8 +308,8 @@ __global__ void k_decode_meta_batch(BatchCfg B) {
   const uint64_t total = B.chunk_start[B.n];
   for (uint64_t w = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; w < total; w += (uint64_t)gridDim.x * blockDim.x) {
     const uint32_t t = batch_find(B.chunk_start, B.n, w);
-    const uint64_t c = w - B.chunk_start[t];
-    decode_meta_body(B.cfgs[t], c, ~0ull >> 1, c == 0);  // exactly one chunk
+    const uint64_t local = w - B.chunk_start[t];
+    decode_meta_body<true>(B.cfgs[t], B.cfgs[t].c0 + local, ~0ull >> 1, local == 0);  // exactly one chunk
   }
 }
 __global__ void k_batch_errors(BatchCfg B) {
@@ -1479,8 +1553,11 @@ __device__ __forceinline__ uint8_t plane_byte(const PlaneSrc& s, uint32_t j) {
 constexpr int kMergeThreads = 256;
 constexpr uint32_t kMergeTile = kMergeThreads * 16 * 4;  // bytes of output per block step (16 KiB)
 
+static_assert(kMergeThreads * 16 == kBoxStep, "regroup_tile advances the box cursor by kBoxStep");
+
 // One 16 KiB output tile of chunk c, by the kMergeThreads threads of a CTA.  `pslot` = the chunk's plane slot.
-template <int G>
+// W: `out` is the box of cfg (box_store16) instead of the whole tensor.
+template <int G, bool W = false>
 __device__ __forceinline__ void regroup_tile(const DecodeCfg& cfg, uint8_t* __restrict__ out, uint64_t c, uint32_t tile, uint32_t pslot,
                                              PlaneSrc (&src)[G]) {
   const uint64_t K = cfg.K;
@@ -1488,6 +1565,7 @@ __device__ __forceinline__ void regroup_tile(const DecodeCfg& cfg, uint8_t* __re
   const uint32_t chunk_len = (c == K - 1) ? (uint32_t)(cfg.orig - c * (uint64_t)chunk) : chunk;
   const uint32_t o_begin = tile * kMergeTile;
   if (o_begin >= chunk_len) return;  // (uniform across the CTA)
+  if (W && !box_meets(cfg, c * (uint64_t)chunk + o_begin, min(kMergeTile, chunk_len - o_begin))) return;  // (uniform)
   __syncthreads();
   if (threadIdx.x < G) {
     const int g = threadIdx.x;
@@ -1509,6 +1587,8 @@ __device__ __forceinline__ void regroup_tile(const DecodeCfg& cfg, uint8_t* __re
   uint8_t* out_c = out + c * (uint64_t)chunk;
   const uint32_t o_end = min(chunk_len, o_begin + kMergeTile);
   const uint32_t rot_words = (cfg.bits_mode == 1 && G > 1) ? (chunk_len >> 2) : 0;  // words that get un-rotated
+  BoxCursor bc;
+  if (W) bc = box_cursor(cfg, c * (uint64_t)chunk + o_begin + threadIdx.x * 16);
   for (uint32_t o = o_begin + threadIdx.x * 16; o < o_end; o += kMergeThreads * 16) {
     if (o + 16 <= o_end) {
       uint32_t r[4];
@@ -1539,7 +1619,12 @@ __device__ __forceinline__ void regroup_tile(const DecodeCfg& cfg, uint8_t* __re
 #pragma unroll
       for (int i = 0; i < 4; i++)
         if (w0 + i < rot_words) r[i] = unrot_word<G>(r[i]);
-      *reinterpret_cast<uint4*>(out_c + o) = make_uint4(r[0], r[1], r[2], r[3]);
+      if (W) {
+        box_store16(cfg, out, bc, r);
+        box_advance(cfg, bc);
+      } else {
+        *reinterpret_cast<uint4*>(out_c + o) = make_uint4(r[0], r[1], r[2], r[3]);
+      }
     } else {
       // ragged tail of the last chunk: byte by byte, whole words still get un-rotated
       for (uint32_t q = o; q < min(o + 16, o_end); q += 4) {
@@ -1550,12 +1635,25 @@ __device__ __forceinline__ void regroup_tile(const DecodeCfg& cfg, uint8_t* __re
           w |= (uint32_t)plane_byte(src[pos % G], pos / G) << (8 * i);
         }
         if ((q >> 2) < rot_words) w = unrot_word<G>(w);
-        for (uint32_t i = 0; i < nb; i++) out_c[q + i] = (uint8_t)(w >> (8 * i));
+        for (uint32_t i = 0; i < nb; i++) {
+          if (W) box_put(cfg, out, c * (uint64_t)chunk + q + i, (uint8_t)(w >> (8 * i)));
+          else out_c[q + i] = (uint8_t)(w >> (8 * i));
+        }
       }
     }
   }
 }
 
+template <bool W>
+__device__ __forceinline__ void regroup_tile_any(const DecodeCfg& cfg, uint64_t c, uint32_t tile, PlaneSrc (&src)[4]) {
+  if (cfg.G == 1) regroup_tile<1, W>(cfg, cfg.out, c, tile, cfg.slot[c], reinterpret_cast<PlaneSrc (&)[1]>(src));
+  else if (cfg.G == 2) regroup_tile<2, W>(cfg, cfg.out, c, tile, cfg.slot[c], reinterpret_cast<PlaneSrc (&)[2]>(src));
+  else regroup_tile<4, W>(cfg, cfg.out, c, tile, cfg.slot[c], src);
+}
+// a call of its own: the window's registers must not spill into the unwindowed loop of k_regroup_batch
+__device__ __noinline__ void regroup_tile_boxed(const DecodeCfg& cfg, uint64_t c, uint32_t tile, PlaneSrc (&src)[4]) {
+  regroup_tile_any<true>(cfg, c, tile, src);
+}
 __global__ void __launch_bounds__(kMergeThreads) k_regroup_batch(BatchCfg B) {
   __shared__ PlaneSrc src[4];
   const uint64_t total = B.tile_start[B.n];
@@ -1567,9 +1665,8 @@ __global__ void __launch_bounds__(kMergeThreads) k_regroup_batch(BatchCfg B) {
     if (local >= (uint64_t)cfg.ctrl->regroup_count * tiles_per_chunk) continue;  // (uniform)
     const uint64_t c = cfg.rlist[local / tiles_per_chunk];
     const uint32_t tile = (uint32_t)(local % tiles_per_chunk);
-    if (cfg.G == 1) regroup_tile<1>(cfg, cfg.out, c, tile, cfg.slot[c], reinterpret_cast<PlaneSrc (&)[1]>(src));
-    else if (cfg.G == 2) regroup_tile<2>(cfg, cfg.out, c, tile, cfg.slot[c], reinterpret_cast<PlaneSrc (&)[2]>(src));
-    else regroup_tile<4>(cfg, cfg.out, c, tile, cfg.slot[c], src);
+    if (cfg.box_len) regroup_tile_boxed(cfg, c, tile, src);
+    else regroup_tile_any<false>(cfg, c, tile, src);
   }
 }
 
@@ -1590,7 +1687,7 @@ __global__ void __launch_bounds__(kMergeThreads) k_regroup(DecodeCfg cfg, uint8_
 // bitstream, G x 4 <= 16 of them), then the whole CTA regroups the chunk and takes the next
 // one.  Costs nothing when the queue is empty (the normal case).
 // ====================================================================================
-template <int G>
+template <int G, bool W = false>
 __device__ __forceinline__ void decode_overflow_body(const DecodeCfg& cfg, uint8_t* __restrict__ out, DecodeSmem& S, PlaneSrc (&src)[G]) {
   const uint32_t n = cfg.ctrl->overflow_count;
   const uint32_t pslot = cfg.max_slots + blockIdx.x;
@@ -1612,7 +1709,7 @@ __device__ __forceinline__ void decode_overflow_body(const DecodeCfg& cfg, uint8
     }
     __threadfence_block();
     __syncthreads();  // the planes are complete
-    for (uint32_t tile = 0; tile < tiles_per_chunk; tile++) regroup_tile<G>(cfg, out, c, tile, pslot, src);
+    for (uint32_t tile = 0; tile < tiles_per_chunk; tile++) regroup_tile<G, W>(cfg, out, c, tile, pslot, src);
     __syncthreads();  // ... and read, before the next chunk overwrites them
   }
 }
@@ -1623,6 +1720,12 @@ __global__ void __launch_bounds__(kMergeThreads) k_decode_overflow(DecodeCfg cfg
   __shared__ PlaneSrc src[G];
   decode_overflow_body<G>(cfg, out, *reinterpret_cast<DecodeSmem*>(smem_raw), src);
 }
+template <bool W>
+__device__ __forceinline__ void decode_overflow_any(const DecodeCfg& cfg, DecodeSmem& S, PlaneSrc (&src)[4]) {
+  if (cfg.G == 1) decode_overflow_body<1, W>(cfg, cfg.out, S, reinterpret_cast<PlaneSrc (&)[1]>(src));
+  else if (cfg.G == 2) decode_overflow_body<2, W>(cfg, cfg.out, S, reinterpret_cast<PlaneSrc (&)[2]>(src));
+  else decode_overflow_body<4, W>(cfg, cfg.out, S, src);
+}
 // grid = (kOverflowCtas, tensors)
 __global__ void __launch_bounds__(kMergeThreads) k_decode_overflow_batch(BatchCfg B) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -1630,9 +1733,8 @@ __global__ void __launch_bounds__(kMergeThreads) k_decode_overflow_batch(BatchCf
   const DecodeCfg& cfg = B.cfgs[blockIdx.y];
   if (blockIdx.x >= cfg.ovf_slots || cfg.ctrl->overflow_count == 0) return;
   DecodeSmem& S = *reinterpret_cast<DecodeSmem*>(smem_raw);
-  if (cfg.G == 1) decode_overflow_body<1>(cfg, cfg.out, S, reinterpret_cast<PlaneSrc (&)[1]>(src));
-  else if (cfg.G == 2) decode_overflow_body<2>(cfg, cfg.out, S, reinterpret_cast<PlaneSrc (&)[2]>(src));
-  else decode_overflow_body<4>(cfg, cfg.out, S, src);
+  if (cfg.box_len) decode_overflow_any<true>(cfg, S, src);
+  else decode_overflow_any<false>(cfg, S, src);
 }
 
 }  // namespace zb

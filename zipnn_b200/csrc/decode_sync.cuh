@@ -354,7 +354,9 @@ __global__ void __launch_bounds__(kParseWarps * 32) k_parse_tables(DecodeCfg cfg
 __device__ __forceinline__ bool off_in_slack(uint32_t lut_s, const SyncShared& S) {  // the table must end where S begins
   return lut_s + 4096u != (uint32_t)__cvta_generic_to_shared(&S);
 }
-template <int G>
+// W: `out` is the box of cfg (box_store16) instead of the whole tensor.
+static_assert(kSyncThreads * 16 == kBoxStep, "the merge advances the box cursor by kBoxStep");
+template <int G, bool W = false>
 __device__ __forceinline__ void sync_process(const DecodeCfg& cfg, uint8_t* __restrict__ out, SyncShared& S, uint16_t* lut_tab, uint32_t lut_s,
                                              uint64_t work) {
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -540,6 +542,8 @@ __device__ __forceinline__ void sync_process(const DecodeCfg& cfg, uint8_t* __re
       uint8_t* out_q = out + c * (uint64_t)cfg.chunk + (uint64_t)out_off * G;
       const bool rot = (cfg.bits_mode == 1) && (G > 1);
       const uint32_t obytes = count * (uint32_t)G;
+      BoxCursor bc;
+      if (W) bc = box_cursor(cfg, c * (uint64_t)cfg.chunk + (uint64_t)out_off * G + (uint32_t)tid * 16u);
       for (uint32_t o = (uint32_t)tid * 16u; o < obytes; o += kSyncThreads * 16u) {
         uint32_t r[4];
         if (G == 1) {
@@ -569,7 +573,12 @@ __device__ __forceinline__ void sync_process(const DecodeCfg& cfg, uint8_t* __re
 #pragma unroll
           for (int i = 0; i < 4; i++) r[i] = unrot_word<G>(r[i]);
         }
-        *reinterpret_cast<uint4*>(out_q + o) = make_uint4(r[0], r[1], r[2], r[3]);
+        if (W) {
+          box_store16(cfg, out, bc, r);
+          box_advance(cfg, bc);
+        } else {
+          *reinterpret_cast<uint4*>(out_q + o) = make_uint4(r[0], r[1], r[2], r[3]);
+        }
       }
     } else {
       uint8_t* dst = cfg.planes + ((uint64_t)cfg.slot[c] * G + g) * cfg.pstride + out_off;
@@ -596,6 +605,12 @@ __global__ void __launch_bounds__(kSyncThreads) k_huf_decode_sync(DecodeCfg cfg,
   }
 }
 
+template <bool W>
+__device__ __forceinline__ void sync_process_any(const DecodeCfg& cfg, SyncShared& S, const SyncCarve& cv, uint64_t work) {
+  if (cfg.G == 1) sync_process<1, W>(cfg, cfg.out, S, cv.lut, cv.lut_s, work);
+  else if (cfg.G == 2) sync_process<2, W>(cfg, cfg.out, S, cv.lut, cv.lut_s, work);
+  else sync_process<4, W>(cfg, cfg.out, S, cv.lut, cv.lut_s, work);
+}
 // Bitstreams of every tensor of a batch in one grid (flat index -> tensor by binary search).
 __global__ void __launch_bounds__(kSyncThreads) k_huf_decode_sync_batch(BatchCfg B) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -608,9 +623,8 @@ __global__ void __launch_bounds__(kSyncThreads) k_huf_decode_sync_batch(BatchCfg
     const uint64_t work = w - B.item_start[t];
     if (work >= 4ull * cfg.ctrl->huf_count) continue;  // (uniform) the bound counts every item, only the coded ones are queued
     __syncthreads();
-    if (cfg.G == 1) sync_process<1>(cfg, cfg.out, S, cv.lut, cv.lut_s, work);
-    else if (cfg.G == 2) sync_process<2>(cfg, cfg.out, S, cv.lut, cv.lut_s, work);
-    else sync_process<4>(cfg, cfg.out, S, cv.lut, cv.lut_s, work);
+    if (cfg.box_len) sync_process_any<true>(cfg, S, cv, work);
+    else sync_process_any<false>(cfg, S, cv, work);
   }
 }
 

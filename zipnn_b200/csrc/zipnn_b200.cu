@@ -11,6 +11,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
+#include <numeric>
 #include <vector>
 
 #include "common.cuh"
@@ -136,10 +137,12 @@ bool byte_map_2d(CUtensorMap* m, const void* base, uint64_t inner, uint64_t rows
 struct Knobs {
   int tma = 2, grid_mode = 1, warps_per_sm = 0;  // tma: 1 = bulk-tensor stores of the output rows, 2 = bulk-tensor tiles for the side plane.
   long long sync_max = -1;  // chunks up to which k_huf_decode_sync replaces the one-thread-per-bitstream kernels (-1: default)
+  long long slice_piece = -1;  // covering chunks above which a slice item is split into pieces (-1: kSyncTablesMaxChunks; tests lower it)
   size_t smem_pad = 0;
 };
 Knobs knobs() {
   Knobs k;
+  if (const char* e = getenv("ZIPNN_B200_SLICE_PIECE_CHUNKS")) k.slice_piece = atoll(e);
   if (const char* e = getenv("ZIPNN_B200_TMA")) k.tma = atoi(e);
   if (const char* e = getenv("ZIPNN_B200_GRID_MODE")) k.grid_mode = atoi(e);
   if (const char* e = getenv("ZIPNN_B200_WARPS_PER_SM")) k.warps_per_sm = atoi(e);
@@ -182,9 +185,12 @@ constexpr uint64_t kSyncDefaultMaxChunks = 3072;  // crossover with the one-thre
 struct DecWs {
   size_t items_off, mode_off, slot_off, rlist_off, olist_off, hlist_off, tables_off, fill_off, planes_off, pstride, fixed;
 };
-inline DecWs dec_ws_layout(size_t orig, int G, size_t chunk) {
+// table_chunks: chunks whose coded items may be queued for the per-bitstream-CTA decoder (default: all of a
+// tensor it takes, none of a larger one; a slice piece: its covering chunk range)
+inline DecWs dec_ws_layout(size_t orig, int G, size_t chunk, uint64_t table_chunks = UINT64_MAX) {
   DecWs L;
   const uint64_t K = num_chunks(orig, chunk);
+  if (table_chunks == UINT64_MAX) table_chunks = K <= kSyncTablesMaxChunks ? K : 0;
   L.items_off = kCtrlBytes;
   L.mode_off = round_up(L.items_off + sizeof(ItemDesc) * (size_t)G * K, 256);
   L.slot_off = round_up(L.mode_off + K, 256);
@@ -193,7 +199,7 @@ inline DecWs dec_ws_layout(size_t orig, int G, size_t chunk) {
   L.hlist_off = round_up(L.olist_off + 4 * K, 256);
   // parsed table descriptions for the per-bitstream-CTA decoder: only tensors it takes (K <= kSyncTablesMaxChunks)
   L.tables_off = round_up(L.hlist_off + 4 * (size_t)G * K, 256);
-  L.fill_off = round_up(L.tables_off + (K <= kSyncTablesMaxChunks ? sizeof(ItemTable) * (size_t)G * K : 0), 256);
+  L.fill_off = round_up(L.tables_off + sizeof(ItemTable) * (size_t)G * table_chunks, 256);
   L.planes_off = round_up(L.fill_off + (size_t)kFillBytes * G * K, 256);
   L.pstride = round_up(chunk / (size_t)G, 16) + 16;
   L.fixed = L.planes_off + 256;
@@ -299,10 +305,10 @@ int zipnn_b200_decompress_workspace_size_full(size_t orig, int num_buf, size_t c
 
 // Fill a DecodeCfg for one tensor whose workspace slice is [ws, ws + ws_bytes).
 static int fill_decode_cfg(DecodeCfg& cfg, const void* d_body, size_t body_len, int G, int bits_mode, size_t chunk, size_t orig, void* d_out,
-                           uint8_t* ws, size_t ws_bytes, bool use_sync) {
+                           uint8_t* ws, size_t ws_bytes, bool use_sync, uint64_t table_chunks = UINT64_MAX) {
   const uint64_t K = num_chunks(orig, chunk);
   if (body_len < 9ull * G * K) return ZIPNN_B200_E_CORRUPT;
-  const DecWs L = dec_ws_layout(orig, G, chunk);
+  const DecWs L = dec_ws_layout(orig, G, chunk, table_chunks);
   if (ws_bytes < L.fixed) return ZIPNN_B200_E_CAPACITY;
   memset(&cfg, 0, sizeof(cfg));
   cfg.body = (const uint8_t*)d_body;
@@ -520,6 +526,9 @@ int zipnn_b200_decompress_batch_workspace_size(const zipnn_b200_batch_item* item
   return ZIPNN_B200_OK;
 }
 
+static int run_batch_kernels(const std::vector<DecodeCfg>& cfgs, const std::vector<uint64_t>& starts, int n, uint8_t* ws, uint64_t max_ovf,
+                             cudaStream_t st, BatchCfg& B);
+
 int zipnn_b200_decompress_batch(const zipnn_b200_batch_item* items, int n, void* d_ws, size_t ws_bytes, void* cuda_stream, int check) {
   if (n < 0 || (n && !items) || !d_ws || ((uintptr_t)d_ws & 255)) return ZIPNN_B200_E_ARG;
   if (n == 0) return ZIPNN_B200_OK;
@@ -563,12 +572,170 @@ int zipnn_b200_decompress_batch(const zipnn_b200_batch_item* items, int n, void*
     }
     at += slice;
   }
+  BatchCfg B;
+  {
+    const int rc = run_batch_kernels(cfgs, starts, n, ws, max_ovf, st, B);
+    if (rc) return rc;
+  }
+  for (int i : big) {
+    const zipnn_b200_batch_item& it = items[i];
+    const int rc = zipnn_b200_decompress(it.d_body, it.body_len, it.num_buf, it.bits_mode, it.bytes_mode, it.chunk, it.orig, it.d_out,
+                                         (void*)cfgs[i].ctrl, batch_slice_bytes(it), st, 0);
+    if (rc) return rc;
+  }
+  k_batch_errors<<<1, 256, 0, st>>>(B);
+  ZB_LAUNCHED();
+  if (check) return read_ctrl_error(d_ws, st);
+  return ZIPNN_B200_OK;
+}
+
+// ---- slices: a box of each stream's decoded bytes, by the batch kernels -------------------------------------
+namespace {
+struct SlicePiece {
+  int item;
+  uint64_t base, rows, pitch, len, out_off, c0, c1;  // the piece's box, where its output starts, its covering chunks
+};
+uint64_t slice_piece_limit() {
+  const Knobs kn = knobs();
+  return kn.slice_piece >= 0 ? std::max<uint64_t>(2, (uint64_t)kn.slice_piece) : kSyncTablesMaxChunks;
+}
+// Checks item i and appends its pieces: the box, split so that no piece covers more than `limit` chunks -- by rows,
+// or by bytes at chunk boundaries (moved by less than 16 bytes) when the box is one run -- with every piece's output
+// on a 16-byte boundary.
+int slice_pieces(const zipnn_b200_slice_item& it, int i, uint64_t limit, std::vector<SlicePiece>& out) {
+  if (!valid_layout(it.num_buf, it.bytes_mode, it.chunk)) return ZIPNN_B200_E_ARG;
+  if (it.rows == 0 || it.len == 0) return ZIPNN_B200_OK;
+  if (it.base > it.orig || it.len > it.orig - it.base) return ZIPNN_B200_E_ARG;
+  if (it.rows > 1 && (it.len > it.pitch || it.rows - 1 > (it.orig - it.base - it.len) / it.pitch)) return ZIPNN_B200_E_ARG;
+  if (!it.d_body || !it.d_out || ((uintptr_t)it.d_out & 15)) return ZIPNN_B200_E_ARG;
+  const uint64_t chunk = it.chunk;
+  auto push = [&](uint64_t base, uint64_t rows, uint64_t pitch, uint64_t len, uint64_t off) {
+    if (rows == 1) pitch = round_up(len, 16);  // (one row: the pitch only has to keep the store path's invariants)
+    out.push_back({i, base, rows, pitch, len, off, base / chunk, (base + (rows - 1) * pitch + len + chunk - 1) / chunk});
+  };
+  auto run = [&](uint64_t b, uint64_t e, uint64_t off) {  // bytes [b, e) to output offset off (16-byte aligned)
+    const uint64_t unit = std::max<uint64_t>(chunk, 16);
+    const uint64_t step = std::max<uint64_t>(1, limit * chunk / unit - 1);
+    const uint64_t delta = b & 15;  // split points p = b (mod 16) keep off + (p - b) aligned
+    while (b < e) {
+      const uint64_t p = std::min<uint64_t>(e, (b / unit + step) * unit + delta);
+      push(b, 1, 0, p - b, off);
+      off += p - b;
+      b = p;
+    }
+  };
+  if (it.rows == 1 || it.pitch == it.len) {
+    run(it.base, it.base + it.rows * it.len, 0);
+    return ZIPNN_B200_OK;
+  }
+  const uint64_t m = 16 / std::gcd<uint64_t>(it.len, 16);  // rows per piece come in multiples of m: piece outputs start at r * len
+  const uint64_t span = (limit - 1) * chunk;                // what a piece may span and still cover at most `limit` chunks
+  uint64_t R = span >= it.len ? (span - it.len) / it.pitch + 1 : 0;
+  R = R / m * m;
+  if (R == 0 && m == 1) {  // rows longer than a piece: each row on its own
+    for (uint64_t r = 0; r < it.rows; r++) run(it.base + r * it.pitch, it.base + r * it.pitch + it.len, r * it.len);
+    return ZIPNN_B200_OK;
+  }
+  R = std::max(R, m);  // (pieces past the limit only when 16 rows of an odd row length span more than it; their tables are sized to fit)
+  for (uint64_t r0 = 0; r0 < it.rows; r0 += R) push(it.base + r0 * it.pitch, std::min(R, it.rows - r0), it.pitch, it.len, r0 * it.len);
+  return ZIPNN_B200_OK;
+}
+int plan_slices(const zipnn_b200_slice_item* items, int n, std::vector<SlicePiece>& pieces) {
+  if (n < 0 || (n && !items)) return ZIPNN_B200_E_ARG;
+  const uint64_t limit = slice_piece_limit();
+  for (int i = 0; i < n; i++) {
+    const int rc = slice_pieces(items[i], i, limit, pieces);
+    if (rc) return rc;
+  }
+  if (pieces.size() > 0x7fffffffull) return ZIPNN_B200_E_ARG;
+  return ZIPNN_B200_OK;
+}
+size_t slice_piece_bytes(const zipnn_b200_slice_item& it, const SlicePiece& p) {
+  const uint64_t kc = p.c1 - p.c0;
+  const DecWs L = dec_ws_layout(it.orig, it.num_buf, it.chunk, kc);
+  const uint64_t slots = kc <= kDefaultSlots ? kc : kDefaultSlots + kOverflowCtas;
+  return round_up(L.fixed + (size_t)slots * it.num_buf * L.pstride, 256);
+}
+}  // namespace
+
+int zipnn_b200_decompress_slices_workspace_size(const zipnn_b200_slice_item* items, int n, size_t* out) {
+  if (!out) return ZIPNN_B200_E_ARG;
+  std::vector<SlicePiece> pieces;
+  const int rc = plan_slices(items, n, pieces);
+  if (rc) return rc;
+  size_t total = batch_header_bytes((int)pieces.size());
+  for (const SlicePiece& p : pieces) total += slice_piece_bytes(items[p.item], p);
+  *out = total;
+  return ZIPNN_B200_OK;
+}
+
+int zipnn_b200_decompress_slices(const zipnn_b200_slice_item* items, int n, void* d_ws, size_t ws_bytes, void* cuda_stream, int check) {
+  if (!d_ws || ((uintptr_t)d_ws & 255)) return ZIPNN_B200_E_ARG;
+  std::vector<SlicePiece> pieces;
+  {
+    const int rc = plan_slices(items, n, pieces);
+    if (rc) return rc;
+  }
+  const int np = (int)pieces.size();
+  if (np == 0) return ZIPNN_B200_OK;
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  uint8_t* ws = (uint8_t*)d_ws;
+  size_t at = batch_header_bytes(np);
+  if (ws_bytes < at) return ZIPNN_B200_E_CAPACITY;
+  std::vector<DecodeCfg> cfgs((size_t)np);
+  std::vector<uint64_t> starts(3 * ((size_t)np + 1), 0);
+  uint64_t* chunk_start = starts.data();
+  uint64_t* item_start = chunk_start + (np + 1);
+  uint64_t* tile_start = item_start + (np + 1);
+  uint64_t max_ovf = 1;  // the overflow kernel always runs (its CTAs return at once when no piece has overflow slots): a fixed launch count
+  ZB_CUDA(cudaMemsetAsync(ws, 0, 256, st));
+  for (int j = 0; j < np; j++) {
+    const SlicePiece& p = pieces[j];
+    const zipnn_b200_slice_item& it = items[p.item];
+    const size_t slice = slice_piece_bytes(it, p);
+    if (at + slice > ws_bytes) return ZIPNN_B200_E_CAPACITY;
+    const uint64_t kc = p.c1 - p.c0;
+    DecodeCfg& cfg = cfgs[j];
+    const int rc = fill_decode_cfg(cfg, it.d_body, it.body_len, it.num_buf, it.bits_mode, it.chunk, it.orig, (uint8_t*)it.d_out + p.out_off,
+                                   ws + at, slice, true, kc);
+    if (rc) return rc;
+    cfg.box_base = p.base;
+    cfg.box_rows = p.rows;
+    cfg.box_pitch = p.pitch;
+    cfg.box_len = p.len;
+    cfg.box_step_rows = kBoxStep / p.pitch;
+    cfg.box_step_cols = kBoxStep % p.pitch;
+    cfg.box_fast = ((p.base | p.pitch | p.len) & 15) == 0;
+    cfg.c0 = p.c0;
+    ZB_CUDA(cudaMemsetAsync(ws + at, 0, kCtrlBytes, st));
+    chunk_start[j + 1] = chunk_start[j] + kc;
+    item_start[j + 1] = item_start[j] + 4ull * it.num_buf * kc;
+    tile_start[j + 1] = tile_start[j] + kc * ((it.chunk + kMergeTile - 1) / kMergeTile);
+    max_ovf = std::max<uint64_t>(max_ovf, cfg.ovf_slots);
+    at += slice;
+  }
+  BatchCfg B;
+  {
+    const int rc = run_batch_kernels(cfgs, starts, np, ws, max_ovf, st, B);
+    if (rc) return rc;
+  }
+  k_batch_errors<<<1, 256, 0, st>>>(B);
+  ZB_LAUNCHED();
+  if (check) return read_ctrl_error(d_ws, st);
+  return ZIPNN_B200_OK;
+}
+
+// Descriptors to the device, then one launch of each kernel of the per-bitstream-CTA family for all of them.
+static int run_batch_kernels(const std::vector<DecodeCfg>& cfgs, const std::vector<uint64_t>& starts, int n, uint8_t* ws, uint64_t max_ovf,
+                             cudaStream_t st, BatchCfg& B) {
+  const uint64_t* chunk_start = starts.data();
+  const uint64_t* item_start = chunk_start + (n + 1);
+  const uint64_t* tile_start = item_start + (n + 1);
   // descriptors to the device (pageable source: the copy is staged before the call returns)
   uint8_t* d_cfgs = ws + 256;
   uint8_t* d_starts = d_cfgs + sizeof(DecodeCfg) * (size_t)n;
   ZB_CUDA(cudaMemcpyAsync(d_cfgs, cfgs.data(), sizeof(DecodeCfg) * (size_t)n, cudaMemcpyHostToDevice, st));
   ZB_CUDA(cudaMemcpyAsync(d_starts, starts.data(), sizeof(uint64_t) * starts.size(), cudaMemcpyHostToDevice, st));
-  BatchCfg B;
   B.cfgs = (const DecodeCfg*)d_cfgs;
   B.chunk_start = (const uint64_t*)d_starts;
   B.item_start = B.chunk_start + (n + 1);
@@ -617,15 +784,6 @@ int zipnn_b200_decompress_batch(const zipnn_b200_batch_item* items, int n, void*
       ZB_LAUNCHED();
     }
   }
-  for (int i : big) {
-    const zipnn_b200_batch_item& it = items[i];
-    const int rc = zipnn_b200_decompress(it.d_body, it.body_len, it.num_buf, it.bits_mode, it.bytes_mode, it.chunk, it.orig, it.d_out,
-                                         (void*)cfgs[i].ctrl, batch_slice_bytes(it), st, 0);
-    if (rc) return rc;
-  }
-  k_batch_errors<<<1, 256, 0, st>>>(B);
-  ZB_LAUNCHED();
-  if (check) return read_ctrl_error(d_ws, st);
   return ZIPNN_B200_OK;
 }
 

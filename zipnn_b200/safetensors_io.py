@@ -12,12 +12,14 @@ comes back on the host, as in the reference.
 """
 from __future__ import annotations
 
+import functools
 import os
 
 import torch
 from safetensors import safe_open as _safe_open
 from safetensors.torch import save_file as _save_file
 
+from .slicing import CompressedSlice
 from .util_header import EnumFormat
 from .util_patch import multi_process_patcher
 from .util_safetensors import (COMPRESSED_DTYPE, COMPRESSION_METHOD, build_compressed_tensor_info,
@@ -52,11 +54,18 @@ class SafeOpen:
     """`safetensors.safe_open` wrapper that decodes compressed tensors on access
     (zipnn/zipnn.py:1592-1626)."""
 
-    def __init__(self, filename, framework, device="cpu", batch=True):
+    def __init__(self, filename, framework, device="cpu", batch=True, slices=False):
         """`batch` (CUDA devices only): decode all compressed tensors of the file with one batched call on
-        the first access instead of one call per tensor; costs device memory for the whole file at once."""
+        the first access instead of one call per tensor; costs device memory for the whole file at once.
+        `slices`: `get_slice` of a compressed entry returns a `CompressedSlice`, whose `[index]` reads and
+        decodes only the chunks the index covers (a tensor-parallel loader's shards).  Off by default, where
+        `get_slice` answers as the reference does."""
         self._device = device
         self._batch = batch
+        self._slices = slices
+        self._slice_fd = None      # own descriptor of the slices' reads (payload ranges straight into pinned memory)
+        self._slice_index = None
+        self._slice_cache = {}
         self._ready = {}
         self._filename = filename
         self._f = _safe_open(filename, framework, device)
@@ -96,6 +105,7 @@ class SafeOpen:
         pipe, self._pipe = self._pipe, None
         fd, self._fd = self._fd, None
         self._ready = {}
+        self._close_slices()
         try:
             if pipe is not None:
                 pipe.finish()
@@ -108,7 +118,21 @@ class SafeOpen:
     def get_slice(self, name):
         if name not in self.compressed_tensors_metadata:
             return self._f.get_slice(name)
-        return NotImplementedError  # as the reference: slices of compressed tensors are unsupported
+        if not self._slices:
+            return NotImplementedError  # as the reference: slices of compressed tensors are unsupported
+        if name not in self._slice_cache:
+            if self._slice_fd is None:
+                self._slice_index = _safetensors_index(self._filename)
+                self._slice_fd = os.open(self._filename, os.O_RDONLY)
+            off, nbytes = self._slice_index[name]
+            self._slice_cache[name] = CompressedSlice(self._slice_fd, off, nbytes, self._cuda)
+        return self._slice_cache[name]
+
+    def _close_slices(self):
+        fd, self._slice_fd = self._slice_fd, None
+        self._slice_cache = {}
+        if fd is not None:
+            os.close(fd)
 
     def __enter__(self):
         return self
@@ -119,6 +143,7 @@ class SafeOpen:
                 self.close()
         finally:
             self._pipe = None
+            self._close_slices()
             if self._fd is not None:
                 os.close(self._fd)
                 self._fd = None
@@ -146,15 +171,20 @@ def load_file(filename, device="cpu") -> dict:
         return {name: f.get_tensor(name) for name in f.keys()}
 
 
-def _zipnn_safetensors():
+def _zipnn_safetensors(slices=False):
     import safetensors.torch
-    safetensors.torch.safe_open = SafeOpen
+    safetensors.torch.safe_open = functools.partial(SafeOpen, slices=True) if slices else SafeOpen
 
 
-def zipnn_safetensors():
+# one object per variant: the patcher applies each patch function once, and pickles it into spawned processes
+_zipnn_safetensors_slices = functools.partial(_zipnn_safetensors, slices=True)
+
+
+def zipnn_safetensors(slices=False):
     """Patch `safetensors.torch.safe_open` in this process and in every process spawned
-    from it (zipnn/zipnn.py:1629-1643)."""
-    multi_process_patcher(_zipnn_safetensors)
+    from it (zipnn/zipnn.py:1629-1643).  `slices=True` installs a SafeOpen whose `get_slice`
+    of a compressed entry returns a `CompressedSlice`."""
+    multi_process_patcher(_zipnn_safetensors_slices if slices else _zipnn_safetensors)
 
 
 def compress_safetensors_file(filename, delete=False, force=True, method=None, threads=None, device="cuda"):

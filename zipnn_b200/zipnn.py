@@ -397,6 +397,18 @@ class ZipNN:
             return x if on_gpu else x.tobytes()
         return result
 
+    def decompress_slice(self, data, index):
+        """`decompress(data)[index]` while decoding only the chunks the index touches (zipnn_b200/slicing.py).
+        `data` is a torch-format stream; `index` takes ints, slices with positive steps and one Ellipsis, as
+        safetensors' slices do.  A CUDA stream is decoded in place with a window; a host stream is first cut to
+        the chunks the index covers, which are copied to the GPU at once.  The result lies where `decompress`
+        would put it: on the stream's GPU, or on the host for a host stream.  Streaming frames and delta streams
+        raise ValueError."""
+        from .slicing import slice_stream
+        if self.delta_compressed_type != 0:
+            raise ValueError("decompress_slice does not take delta streams")
+        return slice_stream(_as_stream(data), index)
+
     def _decompress_frames_at_once(self, stream: np.ndarray):
         """Every frame of a streaming file in one batched decode (zipnn_b200_decompress_batch): one H2D copy of
         the file, one launch per kernel, one D2H copy -- instead of a copy, five launches and two
