@@ -57,6 +57,8 @@ def lib() -> C.CDLL:
         L.zo_zipnn_decompress.restype = C.c_int
         L.zo_zipnn_decompress.argtypes = [u8p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_size_t,
                                           C.c_size_t, u8p, C.c_int]
+        L.zo_huf_read_table.restype = C.c_size_t
+        L.zo_huf_read_table.argtypes = [u8p, C.c_size_t, u8p, u8p, u8p]
         L.zo_split_chunk.restype = None
         L.zo_split_chunk.argtypes = [u8p, C.c_size_t, C.c_int, C.c_int, u8p, C.c_size_t]
         _LIB = L
@@ -92,6 +94,18 @@ def huf_decompress(src, n: int):
     if r == ERR:
         raise ValueError("oracle: corrupt HUF block")
     return dst[:n]
+
+
+def huf_read_table(block):
+    """Table description at the start of a HUF block -> (size in bytes, weights[nsym], tableLog)."""
+    s = _u8(block)
+    w = np.zeros(256, dtype=np.uint8)
+    nsym = np.zeros(1, dtype=np.uint32)
+    log = np.zeros(1, dtype=np.uint32)
+    h = lib().zo_huf_read_table(_ptr(s), s.size, _ptr(w), _ptr(nsym), _ptr(log))
+    if h == ERR:
+        raise ValueError("oracle: corrupt HUF table description")
+    return int(h), w[: int(nsym[0])].copy(), int(log[0])
 
 
 def huf_table_from_counts(counts, n: int):
