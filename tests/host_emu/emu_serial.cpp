@@ -22,6 +22,11 @@ int emu_table_from_counts(const uint32_t* count, uint32_t n, uint8_t* nb, uint16
   return h;
 }
 
+// zb::huf_block_decision: 0 = raw, 1 = RLE, else the coded block's size.
+uint32_t emu_block_decision(int rle, const uint32_t* bits, int hsize, uint32_t plen, uint64_t cap, double thr) {
+  return zb::huf_block_decision(rle != 0, bits, hsize, plen, cap, thr);
+}
+
 int emu_read_weights(const uint8_t* src, uint32_t size, uint8_t* weights, int* nsym, int* lg) {
   static thread_local zb::FseDec D;
   return zb::huf_read_weights(weights, nsym, lg, src, size, D);

@@ -7,6 +7,8 @@ the port with the reference without needing the reference's sources or binary.
   streams     zipnn_core on each case of test_oracle.stream_inputs(): length and sha256 of the stream
               (checked here to decode back to the input with the reference's combine_dtype)
   windows     zipnn_core on the chunk windows of test_stream_windows.window_input()
+  settings    zipnn_core on each case of chunk_settings.settings_inputs(): every chunk size from G to 2^12 and
+              2^19-2^21, thresholds 0-1.5, planes at the threshold and capacity edges (checked to decode back)
 
 usage:  python tests/make_golden_ref_checks.py
 """
@@ -20,6 +22,7 @@ ROOT = os.path.dirname(HERE)
 for p in (ROOT, HERE):
     sys.path.insert(0, p)
 
+from chunk_settings import header as settings_header, settings_inputs  # noqa: E402
 from golden_inputs import REF_CHECKS  # noqa: E402
 from oracle import oracle as O  # noqa: E402
 from test_oracle import block_inputs, stream_inputs  # noqa: E402
@@ -49,11 +52,19 @@ def main():
         part = data[c0 * chunk: c1 * chunk]
         r = bytes(ref.zipnn_core(bytes(_hdr()), bytearray(part.tobytes()), G, 1, 10, 0, chunk, 0.95, 10, 4))
         windows.append({"c0": c0, "c1": c1, "input_sha256": sha(part), "stream_len": len(r), "stream_sha256": sha(r)})
+    settings = []
+    h = settings_header()
+    for c in settings_inputs():
+        G, bits, chunk, data = c["G"], c["bits"], c["chunk"], c["data"]
+        bm = 220 if G == 4 else 10
+        r = bytes(ref.zipnn_core(h, bytearray(data.tobytes()), G, bits, bm, 0, chunk, c["thr"], 10, 4))
+        assert bytes(ref.combine_dtype(r[32:], G, bits, bm, chunk, data.size, 2)) == data.tobytes(), c["name"]
+        settings.append({"name": c["name"], "input_sha256": sha(data), "stream_len": len(r), "stream_sha256": sha(r)})
     with open(REF_CHECKS, "w") as f:
         json.dump({"reference": "zipnn/zipnn v0.5.3 (0e9beed), C extension built -O3",
-                   "huf_blocks": blocks, "streams": streams, "windows": windows}, f, indent=0)
+                   "huf_blocks": blocks, "streams": streams, "windows": windows, "settings": settings}, f, indent=0)
         f.write("\n")
-    print(f"wrote {len(blocks)} blocks, {len(streams)} streams, {len(windows)} windows to {REF_CHECKS}")
+    print(f"wrote {len(blocks)} blocks, {len(streams)} streams, {len(windows)} windows, {len(settings)} settings to {REF_CHECKS}")
 
 
 if __name__ == "__main__":

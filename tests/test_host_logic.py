@@ -86,6 +86,8 @@ def _emu():
     E = C.CDLL(so)
     E.emu_table_from_counts.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     E.emu_read_weights.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
+    E.emu_block_decision.restype = C.c_uint32
+    E.emu_block_decision.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_uint32, C.c_uint64, C.c_double]
     return E
 
 
@@ -150,3 +152,53 @@ def test_device_weight_parser_rejects_garbage():
         r = E.emu_read_weights(buf.ctypes.data, n, w.ctypes.data, C.byref(ns), C.byref(lg))
         assert r == -1 or (0 < r <= n and 1 <= lg.value <= 12 and 2 <= ns.value <= 256)
 
+
+
+def _device_decision(E, plane: np.ndarray, cap: int, thr: float) -> int:
+    """What k_encode_table stores for one plane: its early-outs, then huf_block_decision (huf_serial.cuh)."""
+    n = plane.size
+    cnt = np.bincount(plane, minlength=256).astype(np.uint32)
+    bits = np.zeros(4, np.uint32)
+    thr64 = float(np.float32(thr))
+    if cnt.max() == n:
+        return int(E.emu_block_decision(1, bits.ctypes.data, 0, n, cap, thr64))
+    if cnt.max() <= (n >> 7) + 4:
+        return 0
+    nb = np.zeros(256, np.uint8)
+    val = np.zeros(256, np.uint16)
+    hdr = np.zeros(512, np.uint8)
+    lg = C.c_int(0)
+    h = E.emu_table_from_counts(cnt.ctypes.data, n, nb.ctypes.data, val.ctypes.data, hdr.ctypes.data, C.byref(lg))
+    seg = (n + 3) // 4
+    for q in range(4):
+        bits[q] = int(nb[plane[q * seg: min(n, (q + 1) * seg)]].astype(np.int64).sum())
+    return int(E.emu_block_decision(0, bits.ctypes.data, h, n, cap, thr64))
+
+
+def test_block_decision_matches_oracle_with_capacity():
+    """huf_block_decision, the raw/RLE/coded rule the encoder runs per plane, against the oracle's HUF_compress
+    with the same destination capacity and the threshold.  The capacity is the chunk: the plane itself for one
+    byte group, 2x or 4x the plane for two or four; plus an unbounded one.  Every plane chunk_settings built on a
+    capacity or threshold edge is included."""
+    import chunk_settings as CS
+    E = _emu()
+    rng = np.random.default_rng(23)
+    planes = []
+    for it in range(3000):
+        plen = int(rng.choice([2, 3, 8, 13, 14, 16, 17, 24, 32, 48, 64, 100, 128, 256, 512, 4096, int(rng.integers(2, 2049))]))
+        k = int(rng.integers(1, 81))
+        p = rng.dirichlet(np.ones(k) * rng.uniform(0.05, 2.0))
+        planes.append((rng.choice(k, plen, p=p).astype(np.uint8), float(rng.choice(CS.THRESHOLDS))))
+    edge = [(p, 0.95) for plen in CS.FLIP_PLENS for p in CS.capacity_flip_planes(plen)]
+    edge.append((CS.slack_plane(), 1.0))
+    edge += [(CS.exact_threshold_plane(plen, thr, s), thr) for thr in (0.5, 0.75) for plen in CS.EXACT_PLENS for s in range(3)]
+    flips = 0
+    for i, (plane, thr) in enumerate(planes + edge):
+        caps = [plane.size, 2 * plane.size, 4 * plane.size, 1 << 20]
+        got = [_device_decision(E, plane, cap, thr) for cap in caps]
+        want = [CS.stored_size(plane, cap, thr) for cap in caps]
+        assert got == want, (i, plane.size, thr, got, want)
+        flips += got[0] != got[-1]
+    for plane, thr in edge[: len(CS.FLIP_PLENS) * CS.FLIPS_PER_PLEN + 1]:
+        assert _device_decision(E, plane, plane.size, thr) == 0 and _device_decision(E, plane, 1 << 20, thr) > 1
+    assert flips >= len(CS.FLIP_PLENS) * CS.FLIPS_PER_PLEN + 1

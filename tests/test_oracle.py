@@ -6,6 +6,7 @@ import hashlib
 import numpy as np
 import pytest
 
+import chunk_settings as CS
 from conftest import golden_stream, load_manifest
 from golden_inputs import load_ref_checks, make_input, raw_bytes
 from oracle import oracle as O
@@ -106,3 +107,59 @@ def test_port_matches_compiled_reference_streams():
         o = O.zipnn_compress(h, data, G, bits, bm, chunk, 0.95, threads=2).tobytes()
         assert (len(o), sha(o)) == (w["stream_len"], w["stream_sha256"])
         assert O.zipnn_decompress(np.frombuffer(o[32:], dtype=np.uint8), G, bits, bm, chunk, data.size, threads=2).tobytes() == data.tobytes()
+
+
+def test_port_matches_compiled_reference_settings():
+    """zipnn_core of the port == the reference's stream at every chunk size from G to 2^12 and 2^19-2^21,
+    thresholds 0-1.5, and the planes built to sit on the threshold and capacity edges; the port decodes each."""
+    want = load_ref_checks()["settings"]
+    cases = CS.settings_inputs()
+    assert [c["name"] for c in cases] == [w["name"] for w in want]
+    h = CS.header()
+    for c, w in zip(cases, want):
+        G, bits, chunk, data = c["G"], c["bits"], c["chunk"], c["data"]
+        bm = 220 if G == 4 else 10
+        assert sha(data) == w["input_sha256"], f"the seeded input generator drifted: {c['name']}"
+        o = O.zipnn_compress(h, data, G, bits, bm, chunk, c["thr"], threads=4).tobytes()
+        assert (len(o), sha(o)) == (w["stream_len"], w["stream_sha256"]), c["name"]
+        back = O.zipnn_decompress(np.frombuffer(o[32:], dtype=np.uint8), G, bits, bm, chunk, data.size, threads=4)
+        assert back.tobytes() == data.tobytes(), c["name"]
+
+
+def _types(stream, G, chunk, n):
+    K = -(-n // chunk)
+    return np.frombuffer(stream, dtype=np.uint8)[32: 32 + G * K]
+
+
+def test_settings_planes_sit_on_their_edges():
+    """The searched planes are what chunk_settings says they are, in the reference's streams (same digests)."""
+    h = CS.header()
+    by_kind = {}
+    for c in CS.settings_inputs(big=False):
+        by_kind.setdefault(c["kind"], []).append(c)
+    # capacity flips: raw in the stream (destination = plen); an unbounded destination would code every one
+    for c in by_kind["capflip"] + [c for c in CS.settings_inputs() if c["kind"] == "capslack"]:
+        plen, data = c["plen"], c["data"]
+        planes = data.reshape(-1, plen)
+        assert all(CS.stored_size(p, plen, c["thr"]) == 0 for p in planes)
+        blind = [CS.stored_size(p, 1 << 20, c["thr"]) for p in planes]
+        assert all(b > 1 for b in blind), c["name"]
+        if c["kind"] == "capslack":
+            assert plen - 9 <= blind[0] <= plen - 2
+        s = O.zipnn_compress(h, data, 1, 0, 10, plen, c["thr"]).tobytes()
+        assert not _types(s, 1, plen, data.size).any()
+    # coded size exactly plen * thr: raw, and coded at any higher threshold
+    for c in by_kind["exact"]:
+        plen, planes = c["plen"], c["data"].reshape(-1, c["plen"])
+        for p in planes:
+            r, _ = O.huf_compress(p, plen)
+            assert r == plen * c["thr"]
+            assert CS.stored_size(p, plen, c["thr"]) == 0 and CS.stored_size(p, plen, c["thr"] + 0.01) == r
+    # RLE at 2 and 3 bytes: kept exactly when 1 < plen * thr
+    for c in by_kind["rle"]:
+        G, chunk, data = c["G"], c["chunk"], c["data"]
+        s = O.zipnn_compress(h, data, G, c["bits"], 220 if G == 4 else 10, chunk, c["thr"]).tobytes()
+        t = _types(s, G, chunk, data.size).reshape(G, -1)
+        plen = c["plen"]
+        col = t[:, -1] if plen == 3 else t[:, 0]
+        assert (col == (1 if 1 < plen * np.float32(c["thr"]) else 0)).all(), c["name"]

@@ -173,8 +173,9 @@ struct __align__(16) TableWarp {
 constexpr int kTableWarps = 4;
 
 // hist = this item's four per-stream histograms, u16[4][256] in global memory (read twice: totals, exact sizes)
-__device__ void warp_block_decision(TableWarp& S, const uint16_t* __restrict__ hist, uint32_t plen, double thr, uint8_t* type_out,
-                                    uint32_t* size_out, EncSave* save) {
+// cap = the chunk size: the destination capacity the reference gives HUF_compress (zipnn_core.c:365-368)
+__device__ void warp_block_decision(TableWarp& S, const uint16_t* __restrict__ hist, uint32_t plen, uint32_t cap, double thr,
+                                    uint8_t* type_out, uint32_t* size_out, EncSave* save) {
   const int lane = threadIdx.x & 31;
   uint32_t* total = S.total;
   uint32_t largest = 0;
@@ -191,19 +192,15 @@ __device__ void warp_block_decision(TableWarp& S, const uint16_t* __restrict__ h
     max_sym = max(max_sym, __shfl_xor_sync(0xffffffffu, max_sym, o));
   }
   __syncwarp();
-  uint8_t type = 0;
-  uint32_t size = plen;
+  uint32_t stored = 0;  // huf_block_decision: 0 = raw, 1 = RLE, else the coded block's size
   bool huf = false;
   if (plen == 0 || plen > (uint32_t)kHufBlockMax) {
     // empty plane, or HUF_compress rejects > 128 KiB (huf_compress.c:658) -> raw
   } else if (largest == plen) {
-    if (1.0 < (double)plen * thr) {  // RLE block of 1 byte (huf_compress.c:673)
-      type = 1;
-      size = 1;
-      if (lane == 0) {
-        save->hdr[0] = (uint8_t)max_sym;
-        save->hsize = 0;
-      }
+    stored = huf_block_decision(true, nullptr, 0, plen, cap, thr);  // RLE block of 1 byte (huf_compress.c:673)
+    if (stored && lane == 0) {
+      save->hdr[0] = (uint8_t)max_sym;
+      save->hsize = 0;
     }
   } else if (largest <= (plen >> 7) + 4) {
     // heuristic "probably not compressible" (huf_compress.c:674)
@@ -243,7 +240,7 @@ __device__ void warp_block_decision(TableWarp& S, const uint16_t* __restrict__ h
     lg = __shfl_sync(0xffffffffu, lg, 0);
     hsize = __shfl_sync(0xffffffffu, hsize, 0);
     __syncwarp();
-    if (hsize > 0 && (uint32_t)hsize + 12 < plen && plen >= 12) {
+    if (hsize > 0 && (uint32_t)hsize + 12 < plen) {
       uint32_t bits[4] = {0, 0, 0, 0};
       for (int s = lane; s <= max_sym; s += 32) {
         const uint32_t l = S.nb[s];
@@ -254,30 +251,24 @@ __device__ void warp_block_decision(TableWarp& S, const uint16_t* __restrict__ h
       for (int q = 0; q < 4; q++)
 #pragma unroll
         for (int o = 16; o; o >>= 1) bits[q] += __shfl_xor_sync(0xffffffffu, bits[q], o);
-      uint32_t sb[4], csize = (uint32_t)hsize + 6;
-#pragma unroll
-      for (int q = 0; q < 4; q++) {
-        sb[q] = (bits[q] >> 3) + 1;  // ceil((bits + end mark) / 8), bitstream.h:254-260
-        csize += sb[q];
-      }
-      // (the reference's dst capacity, = chunk, can only bind when the block is kept raw anyway)
-      if (csize < plen - 1 && (double)csize < (double)plen * thr) {  // huf_compress.c:625, zipnn_core.c:371-373
-        type = 1;
-        size = csize;
+      // The capacity binds for one byte group, where it equals the plane length: a block that fits in
+      // plen - 1 bytes can still be refused for the 8-byte slack of a bitstream.
+      stored = huf_block_decision(false, bits, hsize, plen, cap, thr);
+      if (stored) {
         for (int s = lane; s < 256; s += 32) save->nb[s] = S.nb[s];
         for (int i = lane; i < hsize; i += 32) save->hdr[i] = T.hdr[i];
         if (lane == 0) {
           save->hsize = (uint32_t)hsize;
           save->lg = (uint32_t)lg;
 #pragma unroll
-          for (int q = 0; q < 4; q++) save->sbytes[q] = sb[q];
+          for (int q = 0; q < 4; q++) save->sbytes[q] = (bits[q] >> 3) + 1;  // bitstream.h:254-260
         }
       }
     }
   }
   if (lane == 0) {
-    *type_out = type;
-    *size_out = size;
+    *type_out = stored ? 1 : 0;
+    *size_out = stored ? stored : plen;
   }
 }
 
@@ -294,7 +285,7 @@ __global__ void __launch_bounds__(kTableWarps * 32) k_encode_table(const uint16_
     const int g = (int)(item / K);
     const uint64_t c = item - (uint64_t)g * K;
     const uint32_t chunk_len = (c == K - 1) ? (uint32_t)(n - c * (uint64_t)chunk) : chunk;
-    warp_block_decision(S, hist + item * 1024, plane_len(chunk_len, G, g), thr, types + item, sizes + item, saves + item);
+    warp_block_decision(S, hist + item * 1024, plane_len(chunk_len, G, g), chunk, thr, types + item, sizes + item, saves + item);
     __syncwarp();
     // payload bytes of this group per block of kScanItems chunks: lets the scan run on many CTAs
     if (lane == 0) atomicAdd(partials + (uint64_t)g * ((K + kScanItems - 1) / kScanItems) + c / kScanItems, (unsigned long long)sizes[item]);

@@ -524,6 +524,37 @@ ZB_HD inline int huf_write_table(TreeScratch& T, const uint8_t* nb, int max_sym,
 }
 
 // ---------------------------------------------------------------------------------
+// Block decision: what the reference stores for one byte plane of plen bytes.
+// ---------------------------------------------------------------------------------
+// HUF_compress into a destination of cap bytes (huf_compress.c:637-724), then the threshold of
+// zipnn_core.c:371-373.  The caller has already applied the early-outs that need the histogram:
+// rle = every byte of the plane is equal (huf_compress.c:673); otherwise the plane passed the
+// "probably not compressible" test (:674), hsize is the size of its table description (< 0: the
+// format has none for it, :141) and bits[q] the number of code bits of bitstream q.  cap >= plen;
+// the reference passes the chunk size, so for one byte group (cap = plen) the capacity decides:
+//   * the four-stream encoder needs 17 bytes after the table description (:564);
+//   * each bitstream is refused when its room is 8 bytes or less (bitstream.h:190-191) and
+//     reported as overflowed once its write pointer reaches room - 8 (bitstream.h:258).
+// Returns the bytes stored: 0 = raw (the plane itself), 1 = the RLE byte, else the coded block.
+ZB_HD inline uint32_t huf_block_decision(bool rle, const uint32_t bits[4], int hsize, uint32_t plen, uint64_t cap,
+                                         double thr) {
+  if (rle) return (1.0 < (double)plen * thr) ? 1u : 0u;
+  if (hsize <= 0 || (uint64_t)hsize > cap || (uint32_t)hsize + 12 >= plen) return 0;
+  uint64_t room = cap - (uint64_t)hsize;
+  if (room < 6 + 1 + 1 + 1 + 8) return 0;
+  room -= 6;  // jump table
+  uint32_t csize = (uint32_t)hsize + 6;
+  for (int q = 0; q < 4; q++) {
+    if (room <= 8 || (uint64_t)((bits[q] + 1) >> 3) >= room - 8) return 0;
+    const uint32_t sb = (bits[q] >> 3) + 1;  // ceil((bits + end mark) / 8), bitstream.h:254-260
+    room -= sb;
+    csize += sb;
+  }
+  if (csize >= plen - 1) return 0;               // huf_compress.c:625
+  return ((double)csize < (double)plen * thr) ? csize : 0u;
+}
+
+// ---------------------------------------------------------------------------------
 // Decoder: table description -> weights.
 // ---------------------------------------------------------------------------------
 // NSYM = how many distinct weight values the tANS header may declare.  The format allows 256;

@@ -615,7 +615,10 @@ int slice_pieces(const zipnn_b200_slice_item& it, int i, uint64_t limit, std::ve
   };
   auto run = [&](uint64_t b, uint64_t e, uint64_t off) {  // bytes [b, e) to output offset off (16-byte aligned)
     const uint64_t unit = std::max<uint64_t>(chunk, 16);
-    const uint64_t step = std::max<uint64_t>(1, limit * chunk / unit - 1);
+    // units per piece; at least one, also when limit * chunk < 16 (chunks under 8 bytes with a small limit), where
+    // such a piece covers more than `limit` chunks (its tables are sized by its own chunk range)
+    const uint64_t per = limit * chunk / unit;
+    const uint64_t step = per > 1 ? per - 1 : 1;
     const uint64_t delta = b & 15;  // split points p = b (mod 16) keep off + (p - b) aligned
     while (b < e) {
       const uint64_t p = std::min<uint64_t>(e, (b / unit + step) * unit + delta);
