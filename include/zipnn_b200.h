@@ -83,6 +83,27 @@ int zipnn_b200_compress(const void* d_in, size_t n, const void* h_hdr, size_t hd
                         int bits_mode, int bytes_mode, size_t chunk, float threshold, void* d_out,
                         size_t out_cap, size_t* out_len, void* d_ws, size_t ws_bytes, void* cuda_stream);
 
+/* ---- many tensors at once (the checkpoint save path) --------------------------------
+ * The reference compresses a safetensors file one zipnn_core call per tensor
+ * (scripts/zipnn_compress_safetensors.py:77-97).  Every item is what one zipnn_b200_compress call
+ * would take, and its stream is byte for byte what that call writes, whatever the other items are.
+ * All items are coded by ONE launch of each encode kernel per byte-group class (num_buf) present,
+ * plus one memset and one host-to-device copy, all on cuda_stream; the launch count does not depend
+ * on the number of items.  Every item is checked before anything is enqueued (the rules of
+ * zipnn_b200_compress: E_ARG, E_CAPACITY); a bad item means nothing is written.
+ * out_lens: NULL -> the call stays asynchronous, each stream's bytes [24:32] carry its length;
+ *           else a host array of n lengths, filled after ONE synchronisation of the stream. */
+typedef struct zipnn_b200_compress_item {
+  const void* d_in; size_t n;          /* device, 16-byte aligned (as zipnn_b200_compress)          */
+  const void* h_hdr; size_t hdr_len;   /* host, 32..4096 bytes; [24:32] patched in the output        */
+  int num_buf, bits_mode, bytes_mode;
+  size_t chunk; float threshold;
+  void* d_out; size_t out_cap;         /* out_cap >= zipnn_b200_compress_bound(n, num_buf, chunk, hdr_len) */
+} zipnn_b200_compress_item;
+int zipnn_b200_compress_batch_workspace_size(const zipnn_b200_compress_item* items, int n, size_t* out);
+int zipnn_b200_compress_batch(const zipnn_b200_compress_item* items, int n, size_t* out_lens,
+                              void* d_ws, size_t ws_bytes, void* cuda_stream);
+
 /*
  * d_body : the stream AFTER the python header (what the reference passes to combine_dtype)
  * d_out  : orig bytes, 16-byte aligned

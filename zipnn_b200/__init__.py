@@ -6,7 +6,7 @@ plugin for `.znn` checkpoints, zipnn/zipnn.py:1221-1565; see hf.py for how it di
 """
 from .zipnn import DecodePipe, ZipNN
 from .safetensors_io import (SafeOpen, compress_safetensors_file, decompress_safetensors_file,
-                             decompress_safetensors_tensor, load_file, zipnn_safetensors)
+                             decompress_safetensors_tensor, load_file, save_file, zipnn_safetensors)
 from .slicing import CompressedSlice
 
 
@@ -14,5 +14,5 @@ from .hf import zipnn_hf
 
 
 __all__ = ["ZipNN", "zipnn_safetensors", "SafeOpen", "compress_safetensors_file",
-           "decompress_safetensors_file", "decompress_safetensors_tensor", "load_file", "DecodePipe", "zipnn_hf",
-           "CompressedSlice"]
+           "decompress_safetensors_file", "decompress_safetensors_tensor", "load_file", "save_file", "DecodePipe",
+           "zipnn_hf", "CompressedSlice"]

@@ -36,6 +36,13 @@ class SliceItem(C.Structure):
                 ("rows", C.c_size_t), ("pitch", C.c_size_t), ("len", C.c_size_t), ("d_out", C.c_void_p)]
 
 
+class CompressItem(C.Structure):
+    """zipnn_b200_compress_item (include/zipnn_b200.h)."""
+    _fields_ = [("d_in", C.c_void_p), ("n", C.c_size_t), ("h_hdr", C.c_void_p), ("hdr_len", C.c_size_t),
+                ("num_buf", C.c_int), ("bits_mode", C.c_int), ("bytes_mode", C.c_int), ("chunk", C.c_size_t),
+                ("threshold", C.c_float), ("d_out", C.c_void_p), ("out_cap", C.c_size_t)]
+
+
 class ZipNNNativeError(RuntimeError):
     def __init__(self, status: int, msg: str):
         super().__init__(f"zipnn_b200: {msg} (status {status})")
@@ -85,6 +92,8 @@ def lib() -> C.CDLL:
                 "zipnn_b200_decompress_workspace_size": (i32, [sz, i32, sz, szp]),
                 "zipnn_b200_decompress_workspace_size_full": (i32, [sz, i32, sz, szp]),
                 "zipnn_b200_compress": (i32, [vp, sz, vp, sz, i32, i32, i32, sz, C.c_float, vp, sz, szp, vp, sz, vp]),
+                "zipnn_b200_compress_batch_workspace_size": (i32, [C.POINTER(CompressItem), i32, szp]),
+                "zipnn_b200_compress_batch": (i32, [C.POINTER(CompressItem), i32, szp, vp, sz, vp]),
                 "zipnn_b200_decompress": (i32, [vp, sz, i32, i32, i32, sz, sz, vp, vp, sz, vp, i32]),
                 "zipnn_b200_decompress_batch_workspace_size": (i32, [C.POINTER(BatchItem), i32, szp]),
                 "zipnn_b200_decompress_batch": (i32, [C.POINTER(BatchItem), i32, vp, sz, vp, i32]),
@@ -110,7 +119,7 @@ EXPORTS = [
     "zipnn_b200_version", "zipnn_b200_strerror", "zipnn_b200_last_cuda_error", "zipnn_b200_sm_count",
     "zipnn_b200_launch_count", "zipnn_b200_compress_bound", "zipnn_b200_compress_workspace_size",
     "zipnn_b200_decompress_workspace_size", "zipnn_b200_decompress_workspace_size_full", "zipnn_b200_compress",
-    "zipnn_b200_decompress", "zipnn_b200_decompress_batch_workspace_size", "zipnn_b200_decompress_batch",
+    "zipnn_b200_compress_batch_workspace_size", "zipnn_b200_compress_batch", "zipnn_b200_decompress", "zipnn_b200_decompress_batch_workspace_size", "zipnn_b200_decompress_batch",
     "zipnn_b200_decompress_slices_workspace_size", "zipnn_b200_decompress_slices", "zipnn_b200_split", "zipnn_b200_regroup", "zipnn_b200_compress_host", "zipnn_b200_decompress_host",
     "zipnn_b200_timing_enable", "zipnn_b200_timing_kernel_count", "zipnn_b200_timing_kernel_name",
     "zipnn_b200_timing_collect",

@@ -61,6 +61,17 @@ __host__ __device__ __forceinline__ uint32_t plane_len(uint32_t chunk_len, int G
   return chunk_len / (uint32_t)G + ((uint32_t)g < chunk_len % (uint32_t)G ? 1u : 0u);
 }
 
+// ---- batches of tensors: start[t] is the exclusive prefix sum of tensor t's work, start[n] the total;
+//      the tensor that owns flat work index w (w < start[n]; tensors without work are never returned)
+__device__ __forceinline__ uint32_t batch_find(const uint64_t* start, uint32_t n, uint64_t w) {
+  uint32_t lo = 0, hi = n;  // start[lo] <= w < start[hi]
+  while (hi - lo > 1) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (start[mid] <= w) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
 // ---- unaligned little-endian loads from global memory -----------------------------
 __device__ __forceinline__ uint64_t ld_u64_bytes(const uint8_t* p) {
   uint64_t v = 0;

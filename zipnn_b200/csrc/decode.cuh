@@ -296,14 +296,6 @@ struct BatchCfg {
   uint32_t n;
   uint32_t* error_out;           // OR of every tensor's error word (first word of the batch workspace)
 };
-__device__ __forceinline__ uint32_t batch_find(const uint64_t* start, uint32_t n, uint64_t w) {
-  uint32_t lo = 0, hi = n;  // start[lo] <= w < start[hi]
-  while (hi - lo > 1) {
-    const uint32_t mid = (lo + hi) >> 1;
-    if (start[mid] <= w) lo = mid; else hi = mid;
-  }
-  return lo;
-}
 __global__ void k_decode_meta_batch(BatchCfg B) {
   const uint64_t total = B.chunk_start[B.n];
   for (uint64_t w = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; w < total; w += (uint64_t)gridDim.x * blockDim.x) {

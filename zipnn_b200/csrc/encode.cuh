@@ -20,6 +20,8 @@
 #include "common.cuh"
 #include "stage1.cuh"
 
+#include <type_traits>
+
 namespace zb {
 
 // Saved per item by pass A for pass B.
@@ -34,6 +36,40 @@ struct EncSave {
 static_assert(sizeof(EncSave) == 416, "EncSave layout");
 
 constexpr int kEncThreads = 256;
+
+// ---- batches of tensors ------------------------------------------------------------------------------------
+// A batch kernel runs the single-tensor kernel's per-chunk or per-item code for every tensor of one byte-group
+// class in one launch.  A flat work index finds its tensor by binary search over an exclusive prefix sum of that
+// kernel's per-tensor work (batch_find), so tensors of any size share one grid.  The hist body and the write kernels
+// take the batch as a template parameter; its NoBatch form is the single-tensor kernel, whose code is unchanged, with
+// the tensor's arguments taken from the kernel parameters.
+struct EncTensor {
+  const uint8_t* in;
+  uint8_t* out;
+  const uint8_t* hdr;        // this tensor's python header inside the batch's packed header area
+  uint64_t n, K;
+  uint32_t chunk, hdr_len;
+  int G, bits_mode;
+  double thr;
+  Ctrl* ctrl;                // Ctrl and scan partials: the batch's zeroed region
+  unsigned long long* partials;
+  uint8_t* types;            // the tensor's slice of the workspace (enc_ws_layout)
+  uint32_t* sizes;
+  uint64_t* item_off;
+  EncSave* saves;
+  uint16_t* hist;
+};
+
+struct EncBatch {
+  const EncTensor* t;        // the class's tensors
+  const uint64_t* start;     // [n + 1] exclusive prefix of this kernel's work per tensor
+  uint32_t n;
+};
+struct NoBatch {};
+template <class Batch>
+constexpr bool kIsBatch = !std::is_same<Batch, NoBatch>::value;
+__device__ __forceinline__ uint64_t batch_work(NoBatch, uint64_t single) { return single; }
+__device__ __forceinline__ uint64_t batch_work(const EncBatch& B, uint64_t) { return B.start[B.n]; }
 
 // A byte of the (rotated) chunk at byte position pos; words [0, rot_words) are rotated.
 template <int G>
@@ -69,9 +105,11 @@ struct HistSmem {
   uint32_t rep[G][256][HistCfg<G>::R];
 };
 
-template <int G>
-__global__ void __launch_bounds__(kEncThreads) k_encode_hist(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk,
-                                                             uint64_t K, int bits_mode, uint16_t* __restrict__ hist) {
+// The whole kernel, inlined into k_encode_hist (B = NoBatch) and k_encode_hist_batch, which differ only in their
+// launch bounds.
+template <int G, class Batch>
+__device__ __forceinline__ void encode_hist(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk, uint64_t K, int bits_mode,
+                                            uint16_t* __restrict__ hist, Batch B) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   HistSmem<G>& S = *reinterpret_cast<HistSmem<G>*>(smem_raw);
   constexpr int R = HistCfg<G>::R;
@@ -80,7 +118,14 @@ __global__ void __launch_bounds__(kEncThreads) k_encode_hist(const uint8_t* __re
   unsigned char* const col_p = reinterpret_cast<unsigned char*>(&S.rep[0][0][0]) + col_bytes;  // rep[0][0][lane % R]
   for (int i = tid; i < G * 256 * R; i += kEncThreads) (&S.rep[0][0][0])[i] = 0;
   __syncthreads();
-  for (uint64_t c = blockIdx.x; c < K; c += gridDim.x) {
+  for (uint64_t w = blockIdx.x; w < batch_work(B, K); w += gridDim.x) {
+    uint64_t c = w;
+    if constexpr (kIsBatch<Batch>) {  // work = chunks
+      const uint32_t i = batch_find(B.start, B.n, w);
+      const EncTensor& T = B.t[i];
+      in = T.in; n = T.n; chunk = T.chunk; K = T.K; bits_mode = T.bits_mode; hist = T.hist;
+      c = w - B.start[i];
+    }
     const uint8_t* in_c = in + c * (uint64_t)chunk;
     const uint32_t chunk_len = (c == K - 1) ? (uint32_t)(n - c * (uint64_t)chunk) : chunk;
     const uint32_t rot_words = (bits_mode == 1 && G > 1) ? (chunk_len >> 2) : 0;
@@ -156,6 +201,20 @@ __global__ void __launch_bounds__(kEncThreads) k_encode_hist(const uint8_t* __re
       __syncthreads();
     }
   }
+}
+
+template <int G>
+__global__ void __launch_bounds__(kEncThreads) k_encode_hist(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk,
+                                                             uint64_t K, int bits_mode, uint16_t* __restrict__ hist) {
+  encode_hist<G>(in, n, chunk, K, bits_mode, hist, NoBatch{});
+}
+
+// work = chunks.  Held to the CTAs per SM of the single-tensor kernel (two for one group, three -- the shared-memory
+// limit -- for two and four): left alone the two-group form takes 111 registers instead of 80, only two CTAs fit,
+// and a 16 GiB bf16 tensor codes 2-3 % slower.
+template <int G>
+__global__ void __launch_bounds__(kEncThreads, G == 1 ? 2 : 3) k_encode_hist_batch(EncBatch B) {
+  encode_hist<G>(nullptr, 0, 0, 0, 0, nullptr, B);
 }
 
 // =====================================================================================
@@ -272,6 +331,22 @@ __device__ void warp_block_decision(TableWarp& S, const uint16_t* __restrict__ h
   }
 }
 
+// One warp: item (g, c) of one tensor, item = g * K + c.
+template <int G>
+__device__ __forceinline__ void encode_table_item(TableWarp& S, const uint16_t* __restrict__ hist, uint64_t n, uint32_t chunk, uint64_t K,
+                                                  double thr, uint8_t* types, uint32_t* sizes, EncSave* saves,
+                                                  unsigned long long* partials, const int lane, uint64_t item) {
+  {
+    const int g = (int)(item / K);
+    const uint64_t c = item - (uint64_t)g * K;
+    const uint32_t chunk_len = (c == K - 1) ? (uint32_t)(n - c * (uint64_t)chunk) : chunk;
+    warp_block_decision(S, hist + item * 1024, plane_len(chunk_len, G, g), chunk, thr, types + item, sizes + item, saves + item);
+    __syncwarp();
+    // payload bytes of this group per block of kScanItems chunks: lets the scan run on many CTAs
+    if (lane == 0) atomicAdd(partials + (uint64_t)g * ((K + kScanItems - 1) / kScanItems) + c / kScanItems, (unsigned long long)sizes[item]);
+  }
+}
+
 template <int G>
 __global__ void __launch_bounds__(kTableWarps * 32) k_encode_table(const uint16_t* __restrict__ hist, uint64_t n, uint32_t chunk,
                                                                    uint64_t K, double thr, uint8_t* types, uint32_t* sizes,
@@ -281,15 +356,8 @@ __global__ void __launch_bounds__(kTableWarps * 32) k_encode_table(const uint16_
   const int lane = threadIdx.x & 31;
   const uint64_t nitems = (uint64_t)G * K;
   for (uint64_t item = (uint64_t)blockIdx.x * kTableWarps + (threadIdx.x >> 5); item < nitems;
-       item += (uint64_t)gridDim.x * kTableWarps) {
-    const int g = (int)(item / K);
-    const uint64_t c = item - (uint64_t)g * K;
-    const uint32_t chunk_len = (c == K - 1) ? (uint32_t)(n - c * (uint64_t)chunk) : chunk;
-    warp_block_decision(S, hist + item * 1024, plane_len(chunk_len, G, g), chunk, thr, types + item, sizes + item, saves + item);
-    __syncwarp();
-    // payload bytes of this group per block of kScanItems chunks: lets the scan run on many CTAs
-    if (lane == 0) atomicAdd(partials + (uint64_t)g * ((K + kScanItems - 1) / kScanItems) + c / kScanItems, (unsigned long long)sizes[item]);
-  }
+       item += (uint64_t)gridDim.x * kTableWarps)
+    encode_table_item<G>(S, hist, n, chunk, K, thr, types, sizes, saves, partials, lane, item);
 }
 
 // =====================================================================================
@@ -302,17 +370,17 @@ constexpr int kScanThreads = 256;
 // such block in partials[g][blk]; a CTA adds up what lies in front of it (all blocks of the groups
 // before, the earlier blocks of its own group), scans its own 2048 sizes (8 per thread) and writes its
 // slice of the cumulative table, the item offsets and the type bytes.  CTA 0 also writes the header.
-__global__ void __launch_bounds__(kScanThreads) k_encode_scan(const uint32_t* __restrict__ sizes, const uint8_t* __restrict__ types,
-                                                              int G, uint64_t K, const uint8_t* __restrict__ hdr_dev,
-                                                              uint32_t hdr_len, uint8_t* out, uint64_t* item_off, Ctrl* ctrl,
-                                                              const unsigned long long* __restrict__ partials) {
+// CTA `bid` of one tensor's scan (bid < G * nblk).
+__device__ __forceinline__ void encode_scan_block(const uint32_t* __restrict__ sizes, const uint8_t* __restrict__ types, int G, uint64_t K,
+                                                  const uint8_t* __restrict__ hdr_dev, uint32_t hdr_len, uint8_t* out, uint64_t* item_off,
+                                                  Ctrl* ctrl, const unsigned long long* __restrict__ partials, uint32_t bid) {
   __shared__ uint64_t warp_tot[kScanThreads / 32];
   __shared__ uint64_t red[kScanThreads / 32][3];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint64_t nitems = (uint64_t)G * K;
   const uint64_t nblk = (K + kScanItems - 1) / kScanItems;
-  const int g = (int)(blockIdx.x / nblk);
-  const uint64_t blk = blockIdx.x - (uint64_t)g * nblk;
+  const int g = (int)(bid / nblk);
+  const uint64_t blk = bid - (uint64_t)g * nblk;
   // ---- what lies in front of this CTA: whole earlier groups, earlier blocks of this group, everything
   uint64_t s_groups = 0, s_blocks = 0, s_all = 0;
   for (uint64_t i = tid; i < (uint64_t)G * nblk; i += kScanThreads) {
@@ -371,7 +439,7 @@ __global__ void __launch_bounds__(kScanThreads) k_encode_scan(const uint32_t* __
     for (uint64_t j = 0; j < nblk; j++) tot += partials[(uint64_t)g * nblk + j];
     ctrl->group_total[g] = tot;
   }
-  if (blockIdx.x == 0) {
+  if (bid == 0) {
     // python header with the total length patched in (csrc/zipnn_core.c:121)
     const uint64_t total = payload0 + s_all;
     for (uint32_t i = tid; i < hdr_len; i += kScanThreads) {
@@ -381,6 +449,13 @@ __global__ void __launch_bounds__(kScanThreads) k_encode_scan(const uint32_t* __
     }
     if (tid == 0) ctrl->total_len = total;
   }
+}
+
+__global__ void __launch_bounds__(kScanThreads) k_encode_scan(const uint32_t* __restrict__ sizes, const uint8_t* __restrict__ types,
+                                                              int G, uint64_t K, const uint8_t* __restrict__ hdr_dev,
+                                                              uint32_t hdr_len, uint8_t* out, uint64_t* item_off, Ctrl* ctrl,
+                                                              const unsigned long long* __restrict__ partials) {
+  encode_scan_block(sizes, types, G, K, hdr_dev, hdr_len, out, item_off, ctrl, partials, blockIdx.x);
 }
 
 // =====================================================================================
@@ -487,19 +562,30 @@ __device__ __forceinline__ void warp_build_codes(const uint8_t* nb, int lg, uint
   }
 }
 
-template <int G>
+template <int G, class Batch = NoBatch>
 __global__ void __launch_bounds__(kEncThreads) k_encode_write(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk, uint64_t K,
                                                               int bits_mode, const uint8_t* __restrict__ types,
                                                               const uint32_t* __restrict__ sizes, const EncSave* __restrict__ saves,
                                                               const uint64_t* __restrict__ item_off, uint8_t* out,
-                                                              int only_ragged) {
+                                                              int only_ragged, Batch B = {}) {
   __shared__ WriteSmem S;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint64_t nitems = (uint64_t)G * K;
   // only_ragged: just the G items of the last chunk (launched with G blocks)
   const uint64_t first = only_ragged ? (uint64_t)blockIdx.x * K + (K - 1) : blockIdx.x;
   const uint64_t step = only_ragged ? nitems : gridDim.x;
-  for (uint64_t item = first; item < nitems; item += step) {
+  for (uint64_t w = first; w < batch_work(B, nitems); w += step) {
+    uint64_t item = w;
+    if constexpr (kIsBatch<Batch>) {
+      // work = every item of a tensor whose chunk is under 64*G, the G items of its last chunk when that one
+      // is not a multiple of 64*G (only_ragged is 0: the prefix already holds just those)
+      const uint32_t i = batch_find(B.start, B.n, w);
+      const EncTensor& T = B.t[i];
+      in = T.in; n = T.n; chunk = T.chunk; K = T.K; bits_mode = T.bits_mode;
+      types = T.types; sizes = T.sizes; saves = T.saves; item_off = T.item_off; out = T.out;
+      const uint64_t j = w - B.start[i];
+      item = (chunk % (64u * G) != 0) ? j : j * K + (K - 1);
+    }
     const int g = (int)(item / K);
     const uint64_t c = item - (uint64_t)g * K;
     const uint8_t* in_c = in + c * (uint64_t)chunk;
@@ -727,15 +813,24 @@ __device__ __forceinline__ void wb_flush(uint32_t* bitbuf, WbStream& st, int lan
   __syncwarp();
 }
 
-template <int G>
+template <int G, class Batch = NoBatch>
 __global__ void __launch_bounds__(kWbWarps * 32) k_encode_write_warp(const uint8_t* __restrict__ in, uint64_t n, uint32_t chunk,
                                                                      uint64_t K, int bits_mode, const uint8_t* __restrict__ types,
                                                                      const uint32_t* __restrict__ sizes,
                                                                      const EncSave* __restrict__ saves,
-                                                                     const uint64_t* __restrict__ item_off, uint8_t* out) {
+                                                                     const uint64_t* __restrict__ item_off, uint8_t* out,
+                                                                     Batch B = {}) {
   __shared__ WbSmem<G> S;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  for (uint64_t c = blockIdx.x; c < K; c += gridDim.x) {
+  for (uint64_t w = blockIdx.x; w < batch_work(B, K); w += gridDim.x) {
+    uint64_t c = w;
+    if constexpr (kIsBatch<Batch>) {  // work = K chunks of every tensor whose chunk is a multiple of 64*G
+      const uint32_t i = batch_find(B.start, B.n, w);
+      const EncTensor& T = B.t[i];
+      in = T.in; n = T.n; chunk = T.chunk; K = T.K; bits_mode = T.bits_mode;
+      types = T.types; sizes = T.sizes; saves = T.saves; item_off = T.item_off; out = T.out;
+      c = w - B.start[i];
+    }
     const uint32_t chunk_len = (c == K - 1) ? (uint32_t)(n - c * (uint64_t)chunk) : chunk;
     if (chunk_len % (64u * G) != 0) continue;  // ragged tail: k_encode_write
     const uint8_t* in_c = in + c * (uint64_t)chunk;
@@ -970,6 +1065,38 @@ __global__ void __launch_bounds__(kWbWarps * 32) k_encode_write_warp(const uint8
       }
     }
   }
+}
+
+// =====================================================================================
+// batches: the table and scan kernels' bodies for many tensors of one byte-group class, one launch
+// per kernel (the hist body and the write kernels take a batch through their `Batch` parameter).
+// =====================================================================================
+// work = G * K items, one warp each
+template <int G>
+__global__ void __launch_bounds__(kTableWarps * 32) k_encode_table_batch(EncBatch B) {
+  extern __shared__ __align__(1024) unsigned char smem_raw[];
+  TableWarp& S = reinterpret_cast<TableWarp*>(smem_raw)[threadIdx.x >> 5];
+  const int lane = threadIdx.x & 31;
+  const uint64_t total = B.start[B.n];
+  for (uint64_t w = (uint64_t)blockIdx.x * kTableWarps + (threadIdx.x >> 5); w < total; w += (uint64_t)gridDim.x * kTableWarps) {
+    const uint32_t i = batch_find(B.start, B.n, w);
+    const EncTensor& T = B.t[i];
+    encode_table_item<G>(S, T.hist, T.n, T.chunk, T.K, T.thr, T.types, T.sizes, T.saves, T.partials, lane, w - B.start[i]);
+  }
+}
+
+// work = G * nblk scan CTAs; an empty tensor has one, which writes its header-only stream
+__global__ void __launch_bounds__(kScanThreads) k_encode_scan_batch(EncBatch B) {
+  const uint32_t i = batch_find(B.start, B.n, blockIdx.x);
+  const EncTensor& T = B.t[i];
+  if (T.K == 0) {  // reference: zero chunks -> the header alone, total length = header length
+    for (uint32_t j = threadIdx.x; j < T.hdr_len; j += kScanThreads)
+      T.out[j] = (j >= 24 && j < 32) ? (uint8_t)((uint64_t)T.hdr_len >> (8 * (j - 24))) : T.hdr[j];
+    if (threadIdx.x == 0) T.ctrl->total_len = T.hdr_len;
+    return;
+  }
+  encode_scan_block(T.sizes, T.types, T.G, T.K, T.hdr, T.hdr_len, T.out, T.item_off, T.ctrl, T.partials,
+                    (uint32_t)(blockIdx.x - B.start[i]));
 }
 
 }  // namespace zb

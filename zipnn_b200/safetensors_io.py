@@ -14,6 +14,7 @@ from __future__ import annotations
 
 import functools
 import os
+import time
 
 import torch
 from safetensors import safe_open as _safe_open
@@ -187,6 +188,192 @@ def zipnn_safetensors(slices=False):
     multi_process_patcher(_zipnn_safetensors_slices if slices else _zipnn_safetensors)
 
 
+# Input bytes per batched compress call when a file is written from many tensors: bounds the device memory
+# of one group (its inputs, the streams' bound and the workspace).  A larger tensor is a group on its own.
+SAVE_GROUP_BYTES = 1 << 30
+
+
+def _plan_groups(sizes, budget: int) -> list:
+    """Consecutive index groups whose byte sizes add up to at most `budget`; an entry larger than the budget
+    is a group on its own.  Order is kept."""
+    groups, cur, acc = [], [], 0
+    for i, s in enumerate(sizes):
+        if cur and acc + s > budget:
+            groups.append(cur)
+            cur, acc = [], 0
+        cur.append(i)
+        acc += s
+    if cur:
+        groups.append(cur)
+    return groups
+
+
+# safetensors dtype names of the floating-point types (anything else is stored as it is)
+_ST_DTYPES = {"F64": "float64", "F32": "float32", "F16": "float16", "BF16": "bfloat16", "F8_E4M3": "float8_e4m3fn",
+              "F8_E5M2": "float8_e5m2"}
+
+
+class _FileRange:
+    """A tensor's bytes in a file: `nbytes` at `offset` of the open descriptor `fd`."""
+
+    def __init__(self, fd: int, offset: int, nbytes: int, dtype: torch.dtype, shape):
+        self.fd, self.offset, self.nbytes, self.dtype, self.shape = fd, offset, nbytes, dtype, list(shape)
+
+
+def _entry_bytes(src) -> int:
+    return src.nbytes if isinstance(src, _FileRange) else src.element_size() * src.nelement()
+
+
+def _pread_into(fd: int, mv, off: int) -> None:
+    while len(mv):
+        got = os.preadv(fd, [mv], off)
+        if got <= 0:
+            raise OSError(f"short read at offset {off}")
+        mv, off = mv[got:], off + got
+
+
+def _compress_entries(entries, device, timings=None):
+    """Floating-point entries [(name, CPU/CUDA tensor or _FileRange)] -> ({name: CPU tensor}, infos,
+    compressed bytes, original bytes), the choices `compress_safetensors_file` makes per tensor (a stream
+    that is not smaller keeps the original bytes).  Groups of SAVE_GROUP_BYTES: host bytes are staged in
+    pinned memory (file ranges read with pread) and copied with one host-to-device copy per group, a group
+    is one `ZipNN.compress_batch` call, and every stream is copied back into pinned memory.
+    `timings` (a dict): seconds per phase, added up -- stage, h2d, kernels, d2h (device phases by events)."""
+    from .zipnn import _pinned_empty
+    dev = torch.device(device)
+    if dev.type == "cuda" and dev.index is None:
+        dev = torch.device("cuda", torch.cuda.current_device())
+    out, infos = {}, {}
+    comp_len = og_len = 0
+    sizes = [_entry_bytes(src) for _, src in entries]
+    groups = _plan_groups(sizes, SAVE_GROUP_BYTES)
+    align = lambda v: (v + 255) // 256 * 256  # noqa: E731
+    with torch.cuda.device(dev):
+        stream = torch.cuda.current_stream()
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+        for grp in groups:
+            t0 = time.perf_counter()
+            host = [i for i in grp if not (isinstance(entries[i][1], torch.Tensor) and entries[i][1].is_cuda)]
+            at, place = 0, {}
+            for i in host:
+                place[i] = at
+                at += align(sizes[i])
+            stage = _pinned_empty(at)
+            for i in host:
+                src, a = entries[i][1], place[i]
+                if isinstance(src, _FileRange):
+                    _pread_into(src.fd, memoryview(stage.numpy())[a: a + src.nbytes], src.offset)
+                elif sizes[i]:
+                    stage[a: a + sizes[i]].copy_(src.detach().contiguous().reshape(-1).view(torch.uint8))
+            t1 = time.perf_counter()
+            ev[0].record(stream)
+            d_stage = stage[:at].to(dev, non_blocking=True) if host else None
+            ev[1].record(stream)
+            flats = []
+            for i in grp:
+                src = entries[i][1]
+                if i in place:
+                    s = d_stage[place[i]: place[i] + sizes[i]]
+                    dt = src.dtype
+                    shape = src.shape if isinstance(src, _FileRange) else tuple(src.shape)
+                    flats.append(s.view(dt).view(shape) if sizes[i] else torch.empty(shape, dtype=dt, device=dev))
+                else:
+                    flats.append(src)
+            znn = ZipNN(input_format="torch", method=COMPRESSION_METHOD)
+            streams = znn.compress_batch(flats)
+            ev[2].record(stream)
+            lens = [s.numel() for s in streams]
+            keep = [k for k, i in enumerate(grp) if lens[k] < sizes[i]]
+            at, hplace = 0, {}
+            for k in keep:
+                hplace[k] = at
+                at += align(lens[k])
+            hout = _pinned_empty(at)
+            for k in keep:
+                hout[hplace[k]: hplace[k] + lens[k]].copy_(streams[k], non_blocking=True)
+            ev[3].record(stream)
+            stream.synchronize()
+            for k, i in enumerate(grp):
+                name, src = entries[i]
+                og_len += sizes[i]
+                if k in hplace:
+                    comp_len += lens[k]
+                    out[name] = hout[hplace[k]: hplace[k] + lens[k]]
+                    infos[name] = build_compressed_tensor_info(flats[k])
+                else:   # not smaller: the original bytes
+                    comp_len += sizes[i]
+                    if isinstance(src, _FileRange):
+                        out[name] = stage[place[i]: place[i] + sizes[i]].clone().view(src.dtype).view(src.shape)
+                    else:
+                        out[name] = src.cpu()
+            if timings is not None:
+                timings["stage"] = timings.get("stage", 0.0) + (t1 - t0)
+                for key, a, b in (("h2d", 0, 1), ("kernels", 1, 2), ("d2h", 2, 3)):
+                    timings[key] = timings.get(key, 0.0) + ev[a].elapsed_time(ev[b]) / 1e3
+    return out, infos, comp_len, og_len
+
+
+def _check_like_safetensors(tensors) -> None:
+    """What `safetensors.torch.save_file` refuses, before any GPU work: a non-dict, non-tensors, sparse or
+    non-contiguous tensors and tensors sharing storage."""
+    from safetensors.torch import _find_shared_tensors
+    if not isinstance(tensors, dict):
+        raise ValueError(f"Expected a dict of [str, torch.Tensor] but received {type(tensors)}")
+    for k, v in tensors.items():
+        if not isinstance(v, torch.Tensor):
+            raise ValueError(f"Key `{k}` is invalid, expected torch.Tensor but received {type(v)}")
+    sparse = [k for k, v in tensors.items() if v.layout != torch.strided]
+    if sparse:
+        raise ValueError(f"You are trying to save a sparse tensors: `{sparse}` which this library does not support.")
+    failing = [names for names in _find_shared_tensors(tensors) if len(names) > 1]
+    if failing:
+        raise RuntimeError(f"Some tensors share memory, this will lead to duplicate memory on disk: {failing}.")
+    for k, v in tensors.items():
+        if not v.is_contiguous():
+            raise ValueError(f"You are trying to save a non contiguous tensor: `{k}` which is not allowed.")
+
+
+def _write_compressed(tensors, infos, metadata, path) -> None:
+    metadata = dict(metadata) if metadata else {}
+    set_compressed_tensors_metadata(infos, metadata)
+    _save_file(tensors, path, metadata)
+
+
+def _cuda_device(device):
+    """The CUDA device that `device` names (a torch.device, "cuda" / "cuda:i", or a device index), else None."""
+    if isinstance(device, bool) or device is None:
+        return None
+    if isinstance(device, int):
+        return torch.device("cuda", device)
+    try:
+        d = torch.device(device)
+    except (RuntimeError, TypeError, ValueError):
+        return None
+    return d if d.type == "cuda" else None
+
+
+def save_file(tensors, filename, metadata=None) -> None:
+    """The counterpart of `load_file`: a dict of CUDA and/or CPU tensors -> a `.znn.safetensors` file,
+    byte for byte what `safetensors.torch.save_file` of the tensors followed by `compress_safetensors_file`
+    writes.  Floating-point tensors are compressed on the GPU (CPU ones are staged in pinned memory and
+    copied over), many per kernel launch; the file is written by `safetensors.torch.save_file`."""
+    _check_like_safetensors(tensors)
+    plain, floats = {}, []
+    for name in sorted(tensors):   # the order a reader of the plain file lists them in, which the metadata JSON follows
+        t = tensors[name]
+        if zipnn_is_floating_point(EnumFormat.TORCH.value, t, t.dtype):
+            floats.append((name, t))
+        else:
+            plain[name] = t.cpu()
+    devices = {t.device for _, t in floats if t.is_cuda}
+    if len(devices) > 1:
+        raise ValueError(f"save_file compresses on one GPU, but the tensors are on {sorted(map(str, devices))}: "
+                         "move them to one device (or to the CPU) first")
+    out, infos, _, _ = _compress_entries(floats, devices.pop() if devices else torch.device("cuda"))
+    plain.update(out)
+    _write_compressed(plain, infos, metadata, filename)
+
+
 def compress_safetensors_file(filename, delete=False, force=True, method=None, threads=None, device="cuda"):
     """`x.safetensors` -> `x.znn.safetensors` (scripts/zipnn_compress_safetensors.py:37-148).
 
@@ -194,12 +381,38 @@ def compress_safetensors_file(filename, delete=False, force=True, method=None, t
     stream is not smaller stays raw.  Deliberate divergence: the raw fallback stores the
     ORIGINAL bytes (the reference stores its in-place-rotated copy, SURVEY.md section 8b),
     and the metadata key is written even when the source file had no metadata dict.
+    With a CUDA `device` ("cuda", "cuda:i", a torch.device or a device index), the floating-point entries are
+    read with pread into pinned memory and compressed a group at a time by the batched encoder on that device
+    (as `save_file`); any other `device` keeps the per-tensor path (tensor.to(device), then ZipNN.compress).
     Returns (compressed_path, compressed_bytes, original_bytes).
     """
     assert filename.endswith(".safetensors")
     compressed_path = filename[: -len(".safetensors")] + ".znn.safetensors"
     if not force and os.path.exists(compressed_path):
         raise FileExistsError(compressed_path)
+    cuda = _cuda_device(device)
+    if cuda is not None and method in (None, COMPRESSION_METHOD):
+        index = _safetensors_index(filename)
+        tensors, floats = {}, []
+        fd = os.open(filename, os.O_RDONLY)
+        try:
+            with _safe_open(filename, "pt", "cpu") as f:
+                for name in f.keys():
+                    sl = f.get_slice(name)
+                    dtype = getattr(torch, _ST_DTYPES.get(sl.get_dtype(), "uint8"))
+                    if dtype.is_floating_point:
+                        floats.append((name, _FileRange(fd, *index[name], dtype, sl.get_shape())))
+                    else:
+                        tensors[name] = f.get_tensor(name)
+                metadata = f.metadata()
+            out, infos, comp_len, og_len = _compress_entries(floats, cuda)
+        finally:
+            os.close(fd)
+        tensors.update(out)
+        _write_compressed(tensors, infos, metadata, compressed_path)
+        if delete:
+            os.remove(filename)
+        return compressed_path, comp_len, og_len
     tensors, infos = {}, {}
     comp_len = og_len = 0
     with _safe_open(filename, "pt", "cpu") as f:

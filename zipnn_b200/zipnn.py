@@ -44,6 +44,14 @@ def _as_u8_numpy(data) -> np.ndarray:
     return np.frombuffer(data, dtype=np.uint8)
 
 
+def _torch_flat_u8(data: torch.Tensor) -> torch.Tensor:
+    """Flat contiguous uint8 view of a tensor's bytes (a copy only when it is not contiguous)."""
+    t = data.detach().contiguous().reshape(-1)
+    if t.numel() == 0:   # (an empty tensor may carry a zero stride, which view() refuses)
+        t = torch.empty(0, dtype=t.dtype, device=t.device)
+    return t.view(torch.uint8) if t.dtype != torch.uint8 else t
+
+
 def _xor_bytes(a, b):
     """Delta step (reference: np.bitwise_xor on host bytes, zipnn/zipnn.py:636-640, 997-1004).  If either side
     lives on a GPU the XOR runs there and a CUDA uint8 tensor comes back; otherwise a numpy array."""
@@ -281,10 +289,7 @@ class ZipNN:
         self._header[5], self._header[6], self._header[15] = byte_reorder, bit_reorder, code
 
         if fmt == EnumFormat.TORCH.value:
-            t = data.detach().contiguous().reshape(-1)
-            if t.numel() == 0:   # (an empty tensor may carry a zero stride, which view() refuses)
-                t = torch.empty(0, dtype=t.dtype, device=t.device)
-            flat = t.view(torch.uint8) if t.dtype != torch.uint8 else t
+            flat = _torch_flat_u8(data)
         elif fmt == EnumFormat.NUMPY.value:
             flat = torch.from_numpy(np.ascontiguousarray(data).reshape(-1).view(np.uint8))
         elif isinstance(data, torch.Tensor):   # byte format, bytes held in a (possibly CUDA) uint8 tensor
@@ -316,6 +321,22 @@ class ZipNN:
         if getattr(self, "_want_device_result", False):
             return torch.from_numpy(np.asarray(out)).cuda()
         return out
+
+    def compress_batch(self, tensors) -> list:
+        """Many CUDA tensors (one device) in one `zipnn_b200_compress_batch` call: one launch per encode
+        kernel and byte-group class, one host synchronisation.  Element i equals `self.compress(tensors[i])`;
+        the streams are views into one output buffer.  Torch input format only, without streaming or delta."""
+        if self.input_format != EnumFormat.TORCH.value or self.is_streaming or self.delta_compressed_type:
+            raise ValueError("compress_batch takes torch tensors, without streaming or delta compression")
+        tensors = list(tensors)
+        if not all(isinstance(t, torch.Tensor) and t.is_cuda for t in tensors):
+            raise ValueError("compress_batch takes CUDA tensors")
+        if len({t.device for t in tensors}) > 1:
+            raise ValueError("compress_batch takes tensors on one device")
+        if not tensors:
+            return []
+        plans = [self.plan(t) for t in tensors]
+        return _compress_device_batch([_torch_flat_u8(t) for t in tensors], plans)
 
     def plan(self, data) -> dict:
         """Everything `compress(data)` would hand to the native call, without calling it:
@@ -859,6 +880,45 @@ def _compress_device(flat_u8: torch.Tensor, header: bytes, num_buf: int, bits_mo
                                             bytes_mode, chunk, threshold, out.data_ptr(), bound, C.byref(out_len),
                                             ws.data_ptr(), ws.numel(), _cuda_stream_handle()))
     return out[: out_len.value]
+
+
+def _batch_items(flats: list, plans: list):
+    """-> (zipnn_b200_compress_item array without d_out, header buffers to keep alive, output offsets, output
+    bytes): item i codes flats[i] as `plan()` i says, into its bound at its offset (256-byte steps) of one buffer."""
+    items = (_native.CompressItem * len(flats))()
+    hdrs, offs, at = [], [], 0
+    for it, f, p in zip(items, flats, plans):
+        hdr = C.create_string_buffer(p["header"], len(p["header"]))
+        hdrs.append(hdr)
+        it.d_in, it.n = (f.data_ptr() if f.numel() else None), f.numel()
+        it.h_hdr, it.hdr_len = C.cast(hdr, C.c_void_p), len(p["header"])
+        it.num_buf, it.bits_mode, it.bytes_mode = p["num_buf"], p["bit_reorder"], p["byte_reorder"]
+        it.chunk, it.threshold = p["chunk"], p["threshold"]
+        it.out_cap = _native.compress_bound(f.numel(), p["num_buf"], p["chunk"], len(p["header"]))
+        offs.append(at)
+        at += (it.out_cap + 255) // 256 * 256
+    return items, hdrs, offs, at
+
+
+def _compress_device_batch(flats: list, plans: list) -> list:
+    """Flat uint8 CUDA tensors (one device) and their `ZipNN.plan()`s -> their streams, views into one
+    output buffer, from one `zipnn_b200_compress_batch` call and one workspace."""
+    _native.require_cuda()
+    L = _native.lib()
+    flats = [_aligned(f) for f in flats]
+    n = len(flats)
+    items, hdrs, offs, at = _batch_items(flats, plans)   # (hdrs: alive until the call returns, which copies them)
+    dev = flats[0].device
+    with torch.cuda.device(dev):
+        out = torch.empty(at, dtype=torch.uint8, device=dev)
+        for it, o in zip(items, offs):
+            it.d_out = out.data_ptr() + o
+        wsz = C.c_size_t(0)
+        _native.check(L.zipnn_b200_compress_batch_workspace_size(items, n, C.byref(wsz)))
+        ws = torch.empty(max(wsz.value, 1), dtype=torch.uint8, device=dev)
+        lens = (C.c_size_t * n)()
+        _native.check(L.zipnn_b200_compress_batch(items, n, lens, ws.data_ptr(), ws.numel(), _cuda_stream_handle()))
+    return [out[o: o + lens[i]] for i, o in enumerate(offs)]
 
 
 def _decompress_device(body: torch.Tensor, num_buf: int, bits_mode: int, bytes_mode: int, chunk: int,
