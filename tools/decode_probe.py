@@ -13,13 +13,15 @@ from zipnn_b200 import ZipNN, _native  # noqa: E402
 
 CONFIGS = [
     {},
-    {"ZIPNN_B200_SMEM_PAD": "1024"},    # fewer resident warps per SM (shared memory is what limits them)
-    {"ZIPNN_B200_SMEM_PAD": "3072"},
-    {"ZIPNN_B200_SMEM_PAD": "6144"},
-    {"ZIPNN_B200_SMEM_PAD": "12288"},
+    {"ZIPNN_B200_GRID_MODE": "1", "ZIPNN_B200_SMEM_PAD": "1024"},    # fewer resident warps per SM (shared memory is what limits them; one-warp CTAs)
+    {"ZIPNN_B200_GRID_MODE": "1", "ZIPNN_B200_SMEM_PAD": "3072"},
+    {"ZIPNN_B200_GRID_MODE": "1", "ZIPNN_B200_SMEM_PAD": "6144"},
+    {"ZIPNN_B200_GRID_MODE": "1", "ZIPNN_B200_SMEM_PAD": "12288"},
     {"ZIPNN_B200_TMA": "0"},            # side plane through cp.async slots instead of bulk tensor tiles
     {"ZIPNN_B200_TMA": "1"},            # ... and the output rows by bulk tensor stores
-    {"ZIPNN_B200_GRID_MODE": "0"},      # persistent grid
+    {"ZIPNN_B200_GRID_MODE": "0"},      # persistent grid of one-warp CTAs
+    {"ZIPNN_B200_GRID_MODE": "1"},      # one one-warp CTA per chunk group
+    {"ZIPNN_B200_GRID_MODE": "2"},      # one CTA of several warps per SM that claim groups (tools/decode_packing.py has more)
 ]
 
 

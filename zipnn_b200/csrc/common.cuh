@@ -16,6 +16,7 @@ struct Ctrl {
   uint32_t work_counter; // persistent-kernel work queue
   uint32_t regroup_count; // decode: chunks that go through k_regroup (listed in DecodeCfg::rlist)
   uint32_t huf_count;     // decode: coded items queued for k_huf_decode_sync (DecodeCfg::hlist)
+  uint32_t fused_next;    // decode: next chunk group a warp of the packed k_huf_decode_fused launch claims
 };
 static_assert(sizeof(Ctrl) <= 256, "ctrl block");
 constexpr size_t kCtrlBytes = 256;

@@ -26,10 +26,6 @@
 #endif
 
 #ifndef ZB_SIDE_SLOTS
-#ifndef ZB_FUSED_MIN_BLOCKS
-#define ZB_FUSED_MIN_BLOCKS 16  // resident warps per SM the register allocation must allow (shared memory allows 15-16; the
-                                // four-plane variant has 17 KiB per warp = 12 warps, and is 5 % faster with the 168 registers that allows)
-#endif
 #define ZB_SIDE_SLOTS 4  // 16-byte cp.async slots per lane and side plane of the fused kernel.  2 would do (block k+3 is
                          // requested two iterations before it is read) and saves 1 KiB per plane, but a cp.async into a slot
                          // that an LDS read an instant earlier is slow
@@ -66,6 +62,7 @@ struct DecodeCfg {
   uint32_t* hlist;      // [G*K] coded items (g*K + c) for k_huf_decode_sync, ctrl->huf_count of them; nullptr: not used
   struct ItemTable* tables;  // [G*K] parsed table descriptions, parallel to hlist (k_parse_tables)
   uint32_t tma_flags;   // kTmaOut | kTmaSide: which tensor maps of the fused kernel's TmaMaps argument are valid
+  uint32_t fused_claim; // k_huf_decode_fused: warps claim their groups from ctrl->fused_next instead of striding
   uint64_t k_full;      // chunks of full length (K, or K - 1 with a ragged last chunk)
   uint64_t side_pred[3];  // payload offset (inside body) of byte plane g's first item IF every group in front of it is all raw
   uint32_t side_r0[3];    // (body + side_pred[g]) & 15: the tensor maps start at the 16-byte boundary below
@@ -876,11 +873,12 @@ __global__ void __launch_bounds__(32) k_huf_decode_planar(DecodeCfg cfg) {
 // a replicated RLE block read with stride 0), interleaves, un-rotates and emits 16*G bytes
 // of elements.
 //
-// Persistent: the grid is (SM count x resident warps per SM) one-warp CTAs and CTA i takes
-// the chunk groups i, i + grid, ...  A bitstream is serial, so a group costs the same time
-// however the launch is shaped; with one CTA per group the last, partial wave lands on a
-// few SMs that run it at full-wave speed while the rest idle.  A static round-robin leaves
-// every SM the same share of the remainder.
+// Warps work alone: a CTA of W warps is W independent decoders, each with its own shared-memory
+// region (fused_smem_carve) and its own pair of mbarriers; nothing after the setup synchronises
+// the CTA.  A warp takes chunk groups by a static stride or claims them one at a time.  Packing the
+// warps into one CTA per SM pays Hopper's per-CTA shared-memory reserve once instead of once per
+// warp, which is what makes room for the 16th and 17th bf16 warp.  With W = 1 the same code is
+// one CTA per group, or a persistent grid of one-warp CTAs (the host's ZIPNN_B200_GRID_MODE).
 //
 // Bulk tensor copies (TMA) carry everything that is regular:
 //   * side planes: for full chunks whose other planes are all stored raw (what float
@@ -944,8 +942,9 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 //   side                           cp.async path: (G-1) x 2 KiB of slots (4 x 16 bytes per lane and plane);
 //                                  bulk-tensor path (16-bit types): 2 stages x [32 lanes][48 bytes] = 3 KiB.
 //                                  The two uses alias.
-//   bars                   16 B    the two mbarriers
-// bf16: 2 + 1 + 2 + 1 + 4 + 3 = 13 KiB -> 16 warps per SM;  fp32: 3 + 2 + 1 + 4 + 6 = 16 KiB -> 13.
+// bf16: 2 + 1 + 2 + 1 + 4 + 3 = 13 KiB;  fp32: 3 + 2 + 1 + 4 + 6 = 16 KiB;  fp16: 17 KiB;  fp8: 14 KiB.
+// A CTA holds W such regions back to back (fused_warp_stride, a whole number of KiB, so every region starts 0 or 1 KiB
+// past a 2 KiB boundary, which the carve absorbs) and behind them one pair of mbarriers per warp (16 B each).
 template <int G>
 struct FusedGeom {
   static constexpr int kIters = 8 / G;                 // iterations (16 symbols) per 128-byte output row
@@ -962,15 +961,42 @@ struct FusedGeom {
 __host__ __device__ constexpr uint32_t fused_tail_bytes(int pb) { return pb == 0 ? 4096u : 2048u; }
 __host__ __device__ constexpr uint32_t fused_tail_cap(int pb) { return fused_tail_bytes(pb) / 2u; }  // entries: 8 chunks x 128 fit exactly
 template <int G>
-__host__ __device__ constexpr size_t fused_smem_bytes(int pb) {
-  return (pb == 0 ? (size_t)4096 + 32 * kRingBytes : (size_t)3072 + 16 * kRingBytes) + FusedGeom<G>::kSideAll + fused_tail_bytes(pb) + 32 * 128 + 16;
+__host__ __device__ constexpr uint32_t fused_warp_stride(int pb) {  // one warp's region, without its mbarriers
+  return (pb == 0 ? 4096u + 32 * kRingBytes : 3072u + 16 * kRingBytes) + FusedGeom<G>::kSideAll + fused_tail_bytes(pb) + 32 * 128;
 }
+constexpr uint32_t kFusedBarBytes = 16;  // the two mbarriers of a warp
+template <int G>
+__host__ __device__ constexpr size_t fused_smem_bytes(int pb, int warps = 1) {
+  return (size_t)warps * (fused_warp_stride<G>(pb) + kFusedBarBytes);
+}
+// Warps per CTA the kernel is compiled for (__launch_bounds__, and so its register budget): as many regions as the
+// 227 KiB a Hopper CTA may opt into hold (bf16 17, fp8 16, fp32 14, fp16 13), but at most ZB_FUSED_MAX_WARPS.  The
+// register file is split between the SM's four schedulers, so ptxas budgets for W rounded up to a multiple of 4:
+// 17 warps leave 96 registers per thread (bf16 spills), 16 leave 128 (no spills), and the 17th warp would be a fifth
+// one on a scheduler whose other four already keep it busy.  DESIGN.md 3.1 has the measurements.
+#ifndef ZB_FUSED_MAX_WARPS
+#define ZB_FUSED_MAX_WARPS 16
+#endif
+constexpr uint32_t kFusedCtaSmemMax = 232448;
+template <int G, int PB>
+__host__ __device__ constexpr int fused_smem_warps() {
+  return (int)(kFusedCtaSmemMax / (fused_warp_stride<G>(PB) + kFusedBarBytes));
+}
+template <int G, int PB>
+__host__ __device__ constexpr int fused_max_warps() {
+  return fused_smem_warps<G, PB>() < ZB_FUSED_MAX_WARPS ? fused_smem_warps<G, PB>() : ZB_FUSED_MAX_WARPS;
+}
+static_assert(fused_warp_stride<1>(0) % 1024 == 0 && fused_warp_stride<2>(0) % 1024 == 0 && fused_warp_stride<2>(5) % 1024 == 0 &&
+                  fused_warp_stride<4>(0) % 1024 == 0 && fused_warp_stride<4>(5) % 1024 == 0,
+              "every warp region must start on a 1 KiB boundary (fused_smem_carve)");
+static_assert(fused_smem_warps<2, 5>() == 17 && fused_smem_warps<4, 5>() == 14 && fused_smem_warps<2, 0>() == 13 && fused_smem_warps<1, 0>() == 16,
+              "the warps per CTA that DESIGN.md 3.1 lists");
 struct FusedSmem {
   unsigned char* raw;
   uint32_t base_s;     // shared address of raw
   uint32_t table_off;  // cols (PB = 5) or prim (PB = 0)
   uint32_t ring_lo_off, ring_hi_off;  // rings of lanes 0..15 / 16..31 (PB = 5: the first half fills the KiB next to the columns)
-  uint32_t tail_off, bar_off, stage_off, side_off;
+  uint32_t tail_off, stage_off, side_off;
   __device__ __forceinline__ uint16_t* tail() const { return reinterpret_cast<uint16_t*>(raw + tail_off); }
   __device__ __forceinline__ uint8_t* ring(int lane) const { return raw + (lane < 16 ? ring_lo_off : ring_hi_off) + kRingBytes * (uint32_t)(lane & 15); }
   // parse scratch: 256 weight bytes per chunk slot, four slots in each half of the rings
@@ -1006,7 +1032,6 @@ __device__ __forceinline__ FusedSmem fused_smem_carve(unsigned char* raw) {
   S.stage_off = at;  // 1 KiB multiple in both layouts
   at += 32 * 128;
   S.side_off = at;
-  S.bar_off = at + FusedGeom<G>::kSideAll;  // the two mbarriers, 16 bytes behind everything else
   return S;
 }
 // Shared address of side-tile stage st / of plane g's cp.async slots (both inside the side region).
@@ -1162,21 +1187,24 @@ __device__ __forceinline__ void fused_iteration(BitWindow& b, const LUT& lut, Si
 }
 
 template <int G, int PB>
-__global__ void __launch_bounds__(32, G == 4 ? 12 : ZB_FUSED_MIN_BLOCKS) k_huf_decode_fused(DecodeCfg cfg, uint8_t* __restrict__ out, const __grid_constant__ TmaMaps maps) {
+__global__ void __launch_bounds__(32 * fused_max_warps<G, PB>(), 1) k_huf_decode_fused(DecodeCfg cfg, uint8_t* __restrict__ out, const __grid_constant__ TmaMaps maps) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   using Geo = FusedGeom<G>;
   using LUT = typename std::conditional<PB == 0, LutTwo, LutCol<(PB ? PB : 5)>>::type;
   constexpr int kIters = Geo::kIters;
   constexpr int NS = Geo::NS;
-  const FusedSmem S = fused_smem_carve<G, PB>(smem_raw);
-  const int lane = threadIdx.x, slot = lane >> 2, stream = lane & 3;
+  constexpr uint32_t kStride = fused_warp_stride<G>(PB);
+  const uint32_t warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  const FusedSmem S = fused_smem_carve<G, PB>(smem_raw + warp * kStride);
+  const int lane = threadIdx.x & 31, slot = lane >> 2, stream = lane & 3;
   const uint64_t K = cfg.K;
   const uint64_t ngroups = (K + kDecItemsPerWarp - 1) / kDecItemsPerWarp;
   if (PB != 0 && S.table_off > 1024u) {  // the dynamic buffer is not 1 KiB aligned: cannot happen, but never decode wrongly
     if (lane == 0 && blockIdx.x == 0) atomicOr(&cfg.ctrl->error, kErrUnsupported);
     return;
   }
-  const uint32_t bar_s = S.base_s + S.bar_off;  // two mbarriers, one per side-tile stage
+  // two mbarriers, one per side-tile stage, in the array behind the W regions (from the opaque base: see the carve)
+  const uint32_t bar_s = S.base_s + (nwarps - warp) * kStride + kFusedBarBytes * warp;
   if (lane == 0) {
     mbar_init(bar_s, 1);
     mbar_init(bar_s + 8, 1);
@@ -1191,7 +1219,16 @@ __global__ void __launch_bounds__(32, G == 4 ? 12 : ZB_FUSED_MIN_BLOCKS) k_huf_d
   const uint32_t rot_mask = rot ? 0x80808080u : 0u;
   const uint4* hi_block = reinterpret_cast<const uint4*>(((uintptr_t)(cfg.body + cfg.body_len) - 1) & ~(uintptr_t)15);
 
-  for (uint64_t grp = blockIdx.x; grp < ngroups; grp += gridDim.x) {
+  // Static: warp w of CTA b takes groups b W + w, + grid W, ...  Claimed (cfg.fused_claim): each warp takes the next
+  // unclaimed group when it is done with one, so no SM runs out of groups while another still has a round to go.
+  const bool claim = cfg.fused_claim != 0;
+  auto next_group = [&](uint64_t after) -> uint64_t {
+    if (!claim) return after + (uint64_t)gridDim.x * nwarps;
+    uint32_t g = 0;
+    if (lane == 0) g = atomicAdd(&cfg.ctrl->fused_next, 1u);
+    return __shfl_sync(0xffffffffu, g, 0);
+  };
+  for (uint64_t grp = claim ? next_group(0) : (uint64_t)blockIdx.x * nwarps + warp; grp < ngroups; grp = next_group(grp)) {
     const uint64_t c = grp * kDecItemsPerWarp + slot;
     const bool active = (c < K) && cfg.mode[c] == kModeFused;
     if (__ballot_sync(0xffffffffu, active) == 0) continue;

@@ -135,7 +135,12 @@ bool byte_map_2d(CUtensorMap* m, const void* base, uint64_t inner, uint64_t rows
 }
 
 struct Knobs {
-  int tma = 2, grid_mode = 1, warps_per_sm = 0;  // tma: 1 = bulk-tensor stores of the output rows, 2 = bulk-tensor tiles for the side plane.
+  int tma = 2;  // 1 = bulk-tensor stores of the output rows, 2 = bulk-tensor tiles for the side plane
+  // The fused decode's launch (launch_fused): 1 = one one-warp CTA per chunk group, 2 = one CTA of several warps per SM
+  // that claim their groups, 0 = a persistent grid of one-warp CTAs, -1 = the variant's default (fused_default_warps).
+  // warps_per_sm > 0 caps the resident warps: in mode 2 it sets the warps per CTA (up to what fits), in mode 0 the CTAs
+  // per SM.  smem_pad only pads the one-warp modes.
+  int grid_mode = -1, warps_per_sm = 0;
   long long sync_max = -1;  // chunks up to which k_huf_decode_sync replaces the one-thread-per-bitstream kernels (-1: default)
   long long slice_piece = -1;  // covering chunks above which a slice item is split into pieces (-1: kSyncTablesMaxChunks; tests lower it)
   size_t smem_pad = 0;
@@ -152,10 +157,77 @@ Knobs knobs() {
 }
 
 template <typename Kernel>
-int resident_blocks(Kernel k, size_t smem) {
+int resident_blocks(Kernel k, size_t smem, int threads = 32) {
   int nb = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k, 32, smem) != cudaSuccess || nb < 1) nb = 1;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k, threads, smem) != cudaSuccess || nb < 1) nb = 1;
   return nb;
+}
+
+// Most warps one CTA of k_huf_decode_fused<G, PB> can hold and still be resident: fused_max_warps by the shared-memory
+// arithmetic, confirmed by the occupancy calculator (which knows the per-CTA reserve and the allocation granularity).
+template <int G, int PB>
+int fused_cta_warps() {
+  static const int w = [] {
+    constexpr int wmax = fused_max_warps<G, PB>();
+    int best = 1;
+    if (cudaFuncSetAttribute(k_huf_decode_fused<G, PB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fused_smem_bytes<G>(PB, wmax)) == cudaSuccess) {
+      for (int v = wmax; v > 1; v--) {
+        int nb = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_huf_decode_fused<G, PB>, 32 * v, fused_smem_bytes<G>(PB, v)) == cudaSuccess && nb >= 1) {
+          best = v;
+          break;
+        }
+      }
+    }
+    (void)cudaGetLastError();
+    return best;
+  }();
+  return w;
+}
+
+// Warps per CTA of the default launch of each variant, 0 for one one-warp CTA per chunk group.  From about 9 warps per SM
+// on an SM's decode rate hardly grows with more warps, and more warps make more concurrent bitstreams; the fewest that
+// keep the rate were fastest for the rotated types (16 GiB tensors, H100 80GB HBM3 at 400 W, tools/decode_packing.py:
+// bf16 13 warps 13.2 ms against 13.9 for one-warp CTAs at 16 per SM, fp32 10 warps 15.5 ms against 19.7 at 13 per SM);
+// fp16 and fp8 showed no clear winner and keep the one-warp launch (DESIGN.md 3.1).
+template <int G, int PB>
+constexpr int fused_default_warps() {
+  return PB == 5 ? (G == 2 ? 13 : 10) : 0;
+}
+
+// Mode 2: one CTA of W warps per SM whose warps claim chunk groups one at a time (DecodeCfg::fused_claim), so the
+// groups spread over the SMs as evenly as their speed allows whatever W is.  W: ZIPNN_B200_WARPS_PER_SM if set, else the
+// variant's default, and below one round of the machine no more warps per SM than it takes to give every SM its share.
+template <int G, int PB>
+void launch_fused(DecodeCfg cfg, uint8_t* out, const TmaMaps& maps, uint64_t groups, const Knobs& kn, cudaStream_t st) {
+  const uint64_t sms = (uint64_t)sm_count_cached();
+  constexpr int kDefault = fused_default_warps<G, PB>();
+  const int mode = kn.grid_mode >= 0 ? kn.grid_mode : (kDefault > 0 ? 2 : 1);
+  int W = 1;
+  unsigned grid;
+  size_t smem;
+  cfg.fused_claim = 0;
+  if (mode == 2) {
+    const int wmax = fused_cta_warps<G, PB>();
+    if (kn.warps_per_sm > 0) {
+      W = std::min(wmax, kn.warps_per_sm);
+    } else {
+      W = std::min(wmax, kDefault > 0 ? kDefault : wmax);
+      W = (int)std::min<uint64_t>((uint64_t)W, (groups + sms - 1) / sms);
+    }
+    grid = (unsigned)std::min<uint64_t>((groups + W - 1) / W, sms);
+    smem = fused_smem_bytes<G>(PB, W);
+    cfg.fused_claim = 1;
+  } else {
+    smem = fused_smem_bytes<G>(PB) + kn.smem_pad;
+    int nb = resident_blocks(k_huf_decode_fused<G, PB>, smem);
+    if (kn.warps_per_sm > 0) nb = std::min(nb, kn.warps_per_sm);
+    grid = mode == 1 ? (unsigned)groups : (unsigned)std::min<uint64_t>(groups, (uint64_t)nb * sms);
+  }
+  if (getenv("ZIPNN_B200_DEBUG"))
+    fprintf(stderr, "[zipnn_b200] fused launch: G=%d PB=%d mode=%d warps_per_cta=%d grid=%u resident_warps_per_sm=%d\n", G, PB, mode, W, grid,
+            W * resident_blocks(k_huf_decode_fused<G, PB>, smem, 32 * W));
+  k_huf_decode_fused<G, PB><<<grid, 32 * W, smem, st>>>(cfg, out, maps);
 }
 
 inline bool valid_layout(int num_buf, int bytes_mode, size_t chunk) {
@@ -450,21 +522,14 @@ int zipnn_b200_decompress(const void* d_body, size_t body_len, int num_buf, int 
       ScopedTimer tm(kKHufDecode, st);
       int rc = dispatch_G(G, [&](auto g) -> int {
         constexpr int GG = decltype(g)::value;
-        const int sms = sm_count_cached();
-        auto grid_for = [&](int nb) -> unsigned {
-          if (kn.grid_mode == 1) return (unsigned)groups;                            // one CTA per chunk group
-          if (kn.warps_per_sm > 0) nb = std::min(nb, kn.warps_per_sm);
-          return (unsigned)std::min<uint64_t>(groups, (uint64_t)nb * sms);          // persistent
-        };
-        if (short_codes) {
-          const size_t smem = fused_smem_bytes<GG>(5) + kn.smem_pad;
-          const int nb = resident_blocks(k_huf_decode_fused<GG, 5>, smem);
-          k_huf_decode_fused<GG, 5><<<grid_for(nb), 32, smem, st>>>(cfg, (uint8_t*)d_out, maps);
-        } else {
-          const size_t smem = fused_smem_bytes<GG>(0) + kn.smem_pad;
-          const int nb = resident_blocks(k_huf_decode_fused<GG, 0>, smem);
-          k_huf_decode_fused<GG, 0><<<grid_for(nb), 32, smem, st>>>(cfg, (uint8_t*)d_out, maps);
+        if constexpr (GG > 1) {  // (short codes only occur with two or four groups: no <1, 5> instance)
+          if (short_codes) {
+            launch_fused<GG, 5>(cfg, (uint8_t*)d_out, maps, groups, kn, st);
+            ZB_LAUNCHED();
+            return ZIPNN_B200_OK;
+          }
         }
+        launch_fused<GG, 0>(cfg, (uint8_t*)d_out, maps, groups, kn, st);
         ZB_LAUNCHED();
         return ZIPNN_B200_OK;
       });
