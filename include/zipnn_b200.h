@@ -154,6 +154,39 @@ int zipnn_b200_decompress_slices_workspace_size(const zipnn_b200_slice_item* ite
 int zipnn_b200_decompress_slices(const zipnn_b200_slice_item* items, int n, void* d_ws, size_t ws_bytes,
                                  void* cuda_stream, int check);
 
+/* ---- decode plans: decode the same streams again and again (weights kept compressed in HBM) ----------
+ * A plan splits a slice decode into what depends only on the streams -- validation, item tables, work lists,
+ * parsed Huffman tables and the start of every segment of the per-bitstream-CTA decoder, done once by _create --
+ * and a run that only enqueues kernels: at most four launches whatever n is (one when every item is empty), no
+ * host-to-device copy, no memset, no synchronisation, so a run can be captured in a CUDA graph.  A run decodes
+ * each segment once from its recorded start instead of searching for the starts.  Every run writes the same
+ * bytes to the same d_out addresses.
+ * Items are slice items (a whole tensor: base 0, rows 1, len orig); they follow the rules of
+ * zipnn_b200_decompress_slices, large boxes are split into pieces the same way, and a piece that is a whole
+ * tensor decodes without the window.
+ * Memory, owned by the caller, split by lifetime:
+ *   plan memory  (plan_bytes, 256-byte aligned): descriptors, item tables, work lists, parsed tables, RLE fill
+ *                blocks, the error word and the segment index (8 KiB per Huffman-coded item); must stay
+ *                allocated and untouched while the plan is used;
+ *   scratch      (scratch_bytes, 256-byte aligned): plane pools, written and read within one run only.  Plans
+ *                whose runs are ordered on one stream may share one scratch buffer.
+ * The streams (d_body) must stay allocated at the same address and unchanged, and d_out allocated, for the life
+ * of the plan.
+ * _size synchronises cuda_stream: it reads each item's type rows to count its coded items.
+ * _create checks every item, decodes once into every d_out (recording the segment starts), synchronises
+ * cuda_stream and returns that decode's status (E_CORRUPT, E_UNSUPPORTED, ...); a plan whose create failed makes
+ * _run, _status and _index return E_ARG.
+ * _status synchronises cuda_stream and returns the error word of the plan's runs so far.
+ * _index gives the bytes of the plan's segment index and the coded items it covers. */
+typedef struct zipnn_b200_decode_plan { uint64_t opaque[16]; } zipnn_b200_decode_plan;   /* host, filled by _create */
+int zipnn_b200_decode_plan_size(const zipnn_b200_slice_item* items, int n, void* cuda_stream,
+                                size_t* plan_bytes, size_t* scratch_bytes);
+int zipnn_b200_decode_plan_create(const zipnn_b200_slice_item* items, int n, void* d_plan, size_t plan_bytes,
+                                  void* d_scratch, size_t scratch_bytes, zipnn_b200_decode_plan* plan, void* cuda_stream);
+int zipnn_b200_decode_plan_run(const zipnn_b200_decode_plan* plan, void* cuda_stream);
+int zipnn_b200_decode_plan_status(const zipnn_b200_decode_plan* plan, void* cuda_stream);
+int zipnn_b200_decode_plan_index(const zipnn_b200_decode_plan* plan, size_t* index_bytes, size_t* coded_items);
+
 /* ---- stage 1 alone ------------------------------------------------------------ */
 /* d_planes: num_buf planes of `stride` bytes each; plane g receives byte g of every element
  * of the (optionally rotated) input.  Lengths as in the reference: n/num_buf, the first

@@ -8,6 +8,8 @@ from .zipnn import DecodePipe, ZipNN
 from .safetensors_io import (SafeOpen, compress_safetensors_file, decompress_safetensors_file,
                              decompress_safetensors_tensor, load_file, save_file, zipnn_safetensors)
 from .slicing import CompressedSlice
+from .plan import DecodePlan
+from .resident import compress_module, decompress_module
 
 
 from .hf import zipnn_hf
@@ -15,4 +17,4 @@ from .hf import zipnn_hf
 
 __all__ = ["ZipNN", "zipnn_safetensors", "SafeOpen", "compress_safetensors_file",
            "decompress_safetensors_file", "decompress_safetensors_tensor", "load_file", "save_file", "DecodePipe",
-           "zipnn_hf", "CompressedSlice"]
+           "zipnn_hf", "CompressedSlice", "DecodePlan", "compress_module", "decompress_module"]

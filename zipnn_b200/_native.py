@@ -43,6 +43,11 @@ class CompressItem(C.Structure):
                 ("threshold", C.c_float), ("d_out", C.c_void_p), ("out_cap", C.c_size_t)]
 
 
+class DecodePlanStruct(C.Structure):
+    """zipnn_b200_decode_plan (include/zipnn_b200.h): host memory, filled by zipnn_b200_decode_plan_create."""
+    _fields_ = [("opaque", C.c_uint64 * 16)]
+
+
 class ZipNNNativeError(RuntimeError):
     def __init__(self, status: int, msg: str):
         super().__init__(f"zipnn_b200: {msg} (status {status})")
@@ -99,6 +104,11 @@ def lib() -> C.CDLL:
                 "zipnn_b200_decompress_batch": (i32, [C.POINTER(BatchItem), i32, vp, sz, vp, i32]),
                 "zipnn_b200_decompress_slices_workspace_size": (i32, [C.POINTER(SliceItem), i32, szp]),
                 "zipnn_b200_decompress_slices": (i32, [C.POINTER(SliceItem), i32, vp, sz, vp, i32]),
+                "zipnn_b200_decode_plan_size": (i32, [C.POINTER(SliceItem), i32, vp, szp, szp]),
+                "zipnn_b200_decode_plan_create": (i32, [C.POINTER(SliceItem), i32, vp, sz, vp, sz, C.POINTER(DecodePlanStruct), vp]),
+                "zipnn_b200_decode_plan_run": (i32, [C.POINTER(DecodePlanStruct), vp]),
+                "zipnn_b200_decode_plan_status": (i32, [C.POINTER(DecodePlanStruct), vp]),
+                "zipnn_b200_decode_plan_index": (i32, [C.POINTER(DecodePlanStruct), szp, szp]),
                 "zipnn_b200_split": (i32, [vp, sz, i32, i32, vp, sz, vp]),
                 "zipnn_b200_regroup": (i32, [vp, sz, sz, i32, i32, vp, vp]),
                 "zipnn_b200_compress_host": (i32, [vp, sz, vp, sz, i32, i32, i32, sz, C.c_float, vp, sz, szp]),
@@ -120,7 +130,8 @@ EXPORTS = [
     "zipnn_b200_launch_count", "zipnn_b200_compress_bound", "zipnn_b200_compress_workspace_size",
     "zipnn_b200_decompress_workspace_size", "zipnn_b200_decompress_workspace_size_full", "zipnn_b200_compress",
     "zipnn_b200_compress_batch_workspace_size", "zipnn_b200_compress_batch", "zipnn_b200_decompress", "zipnn_b200_decompress_batch_workspace_size", "zipnn_b200_decompress_batch",
-    "zipnn_b200_decompress_slices_workspace_size", "zipnn_b200_decompress_slices", "zipnn_b200_split", "zipnn_b200_regroup", "zipnn_b200_compress_host", "zipnn_b200_decompress_host",
+    "zipnn_b200_decompress_slices_workspace_size", "zipnn_b200_decompress_slices", "zipnn_b200_decode_plan_size",
+    "zipnn_b200_decode_plan_create", "zipnn_b200_decode_plan_run", "zipnn_b200_decode_plan_status", "zipnn_b200_decode_plan_index", "zipnn_b200_split", "zipnn_b200_regroup", "zipnn_b200_compress_host", "zipnn_b200_decompress_host",
     "zipnn_b200_timing_enable", "zipnn_b200_timing_kernel_count", "zipnn_b200_timing_kernel_name",
     "zipnn_b200_timing_collect",
 ]

@@ -354,11 +354,22 @@ __global__ void __launch_bounds__(kParseWarps * 32) k_parse_tables(DecodeCfg cfg
 __device__ __forceinline__ bool off_in_slack(uint32_t lut_s, const SyncShared& S) {  // the table must end where S begins
   return lut_s + 4096u != (uint32_t)__cvta_generic_to_shared(&S);
 }
+// Modes of sync_process.  Decode: find the segment starts by the rounds below.  Record (a decode plan's create): the
+// same, and once the checks passed every thread stores its segment start and symbol count in `segs[tid]`.  Replay (a
+// plan's run, the stream unchanged since the record): table and stream are staged as in decode, the rounds and the
+// checks are skipped, each thread loads its start and count from `segs[tid]` and emits once.
+enum SyncMode : int { kSyncDecode = 0, kSyncRecord = 1, kSyncReplay = 2 };
+// One entry of a plan's segment index: per (coded item of the plan's hlist, bitstream, thread).
+struct SegEntry {
+  uint32_t from;  // bit position the thread's segment starts at (stream-buffer coordinates, fixed for a fixed address)
+  uint32_t n;     // symbols in the segment
+};
+static_assert(sizeof(SegEntry) == 8, "8 bytes per segment: 8 KiB per coded item");
 // W: `out` is the box of cfg (box_store16) instead of the whole tensor.
 static_assert(kSyncThreads * 16 == kBoxStep, "the merge advances the box cursor by kBoxStep");
-template <int G, bool W = false>
+template <int G, bool W = false, int M = kSyncDecode>
 __device__ __forceinline__ void sync_process(const DecodeCfg& cfg, uint8_t* __restrict__ out, SyncShared& S, uint16_t* lut_tab, uint32_t lut_s,
-                                             uint64_t work) {
+                                             uint64_t work, SegEntry* segs = nullptr) {
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const uint64_t K = cfg.K;
   {
@@ -478,6 +489,11 @@ __device__ __forceinline__ void sync_process(const DecodeCfg& cfg, uint8_t* __re
     const uint32_t top = (uint64_t)tid * segbits < bits ? mark - (uint32_t)tid * segbits : first;          // guess (exact for tid 0)
     const uint32_t bound = (uint64_t)(tid + 1) * segbits < bits ? mark - (uint32_t)(tid + 1) * segbits : first;
     uint32_t from = top, stop = top, n = 0, n_rec = 0;
+    if constexpr (M == kSyncReplay) {
+      const SegEntry e = segs[tid];
+      from = e.from;
+      n = e.n;
+    } else {
     int ncp = 0;                                                    // recorded boundaries of this thread's first pass
     uint16_t* cp = reinterpret_cast<uint16_t*>(S.plane);            // [kSyncCheckpoints][kSyncThreads]; the plane is written after the rounds
     bool need = true;
@@ -498,6 +514,7 @@ __device__ __forceinline__ void sync_process(const DecodeCfg& cfg, uint8_t* __re
       from = nf;
       if (!__syncthreads_or(need)) break;
     }
+    }
     // ---- output offsets; the stream must hold exactly `count` symbols and be consumed exactly ----
     uint32_t incl = n;
 #pragma unroll
@@ -515,10 +532,13 @@ __device__ __forceinline__ void sync_process(const DecodeCfg& cfg, uint8_t* __re
       total += v;
     }
     const uint32_t off = before + incl - n;
-    if (total != count || S.stop[kSyncThreads - 1] != first) {
-      if (tid == 0) atomicOr(&cfg.ctrl->error, kErrCorrupt);
-      return;  // (uniform)
+    if constexpr (M != kSyncReplay) {
+      if (total != count || S.stop[kSyncThreads - 1] != first) {
+        if (tid == 0) atomicOr(&cfg.ctrl->error, kErrCorrupt);
+        return;  // (uniform)
+      }
     }
+    if constexpr (M == kSyncRecord) segs[tid] = SegEntry{from, n};
     if (in_smem) swin_emit(sw, from, n, S.plane, off);
     else sync_emit(b, lut, from, n, S.plane, off);
     __syncthreads();
@@ -605,11 +625,11 @@ __global__ void __launch_bounds__(kSyncThreads) k_huf_decode_sync(DecodeCfg cfg,
   }
 }
 
-template <bool W>
-__device__ __forceinline__ void sync_process_any(const DecodeCfg& cfg, SyncShared& S, const SyncCarve& cv, uint64_t work) {
-  if (cfg.G == 1) sync_process<1, W>(cfg, cfg.out, S, cv.lut, cv.lut_s, work);
-  else if (cfg.G == 2) sync_process<2, W>(cfg, cfg.out, S, cv.lut, cv.lut_s, work);
-  else sync_process<4, W>(cfg, cfg.out, S, cv.lut, cv.lut_s, work);
+template <bool W, int M = kSyncDecode>
+__device__ __forceinline__ void sync_process_any(const DecodeCfg& cfg, SyncShared& S, const SyncCarve& cv, uint64_t work, SegEntry* seg = nullptr) {
+  if (cfg.G == 1) sync_process<1, W, M>(cfg, cfg.out, S, cv.lut, cv.lut_s, work, seg);
+  else if (cfg.G == 2) sync_process<2, W, M>(cfg, cfg.out, S, cv.lut, cv.lut_s, work, seg);
+  else sync_process<4, W, M>(cfg, cfg.out, S, cv.lut, cv.lut_s, work, seg);
 }
 // Bitstreams of every tensor of a batch in one grid (flat index -> tensor by binary search).
 __global__ void __launch_bounds__(kSyncThreads) k_huf_decode_sync_batch(BatchCfg B) {
@@ -625,6 +645,31 @@ __global__ void __launch_bounds__(kSyncThreads) k_huf_decode_sync_batch(BatchCfg
     __syncthreads();
     if (cfg.box_len) sync_process_any<true>(cfg, S, cv, work);
     else sync_process_any<false>(cfg, S, cv, work);
+  }
+}
+
+// A decode plan's segment index: entries seg[base[t] + work * kSyncThreads + tid] for bitstream `work` of tensor t
+// (base[t]: 4 * kSyncThreads * the coded items of the tensors in front of t, counted from their type rows).
+struct SegIndex {
+  SegEntry* seg;
+  const uint64_t* base;  // [n + 1]
+};
+// k_huf_decode_sync_batch in record (M = kSyncRecord) or replay (M = kSyncReplay) mode.
+template <int M>
+__global__ void __launch_bounds__(kSyncThreads) k_huf_decode_sync_plan(BatchCfg B, SegIndex X) {
+  extern __shared__ __align__(1024) unsigned char smem_raw[];
+  const SyncCarve cv = sync_carve(smem_raw);
+  SyncShared& S = *cv.S;
+  const uint64_t total = B.item_start[B.n];
+  for (uint64_t w = blockIdx.x; w < total; w += gridDim.x) {
+    const uint32_t t = batch_find(B.item_start, B.n, w);
+    const DecodeCfg& cfg = B.cfgs[t];
+    const uint64_t work = w - B.item_start[t];
+    if (work >= 4ull * cfg.ctrl->huf_count) continue;  // (uniform)
+    SegEntry* seg = X.seg + X.base[t] + work * kSyncThreads;
+    __syncthreads();
+    if (cfg.box_len) sync_process_any<true, M>(cfg, S, cv, work, seg);
+    else sync_process_any<false, M>(cfg, S, cv, work, seg);
   }
 }
 

@@ -375,13 +375,15 @@ int zipnn_b200_decompress_workspace_size_full(size_t orig, int num_buf, size_t c
   return ZIPNN_B200_OK;
 }
 
-// Fill a DecodeCfg for one tensor whose workspace slice is [ws, ws + ws_bytes).
+// Fill a DecodeCfg for one tensor whose workspace slice is [ws, ws + ws_bytes).  With `planes` the slice holds only
+// what precedes the plane pool (L.planes_off bytes: a decode plan's metadata) and the pool is [planes, + planes_bytes).
 static int fill_decode_cfg(DecodeCfg& cfg, const void* d_body, size_t body_len, int G, int bits_mode, size_t chunk, size_t orig, void* d_out,
-                           uint8_t* ws, size_t ws_bytes, bool use_sync, uint64_t table_chunks = UINT64_MAX) {
+                           uint8_t* ws, size_t ws_bytes, bool use_sync, uint64_t table_chunks = UINT64_MAX, uint8_t* planes = nullptr,
+                           size_t planes_bytes = 0) {
   const uint64_t K = num_chunks(orig, chunk);
   if (body_len < 9ull * G * K) return ZIPNN_B200_E_CORRUPT;
   const DecWs L = dec_ws_layout(orig, G, chunk, table_chunks);
-  if (ws_bytes < L.fixed) return ZIPNN_B200_E_CAPACITY;
+  if (ws_bytes < (planes ? L.planes_off : L.fixed)) return ZIPNN_B200_E_CAPACITY;
   memset(&cfg, 0, sizeof(cfg));
   cfg.body = (const uint8_t*)d_body;
   cfg.out = (uint8_t*)d_out;
@@ -397,10 +399,10 @@ static int fill_decode_cfg(DecodeCfg& cfg, const void* d_body, size_t body_len, 
   cfg.slot = (uint32_t*)(ws + L.slot_off);
   cfg.rlist = (uint32_t*)(ws + L.rlist_off);
   cfg.fill = ws + L.fill_off;
-  cfg.planes = ws + L.planes_off;
+  cfg.planes = planes ? planes : ws + L.planes_off;
   cfg.pstride = L.pstride;
   cfg.olist = (uint32_t*)(ws + L.olist_off);
-  const uint64_t have = (ws_bytes - L.fixed) / ((size_t)G * L.pstride);
+  const uint64_t have = (planes ? planes_bytes : ws_bytes - L.fixed) / ((size_t)G * L.pstride);
   if (have >= K) {
     cfg.max_slots = (uint32_t)K;
     cfg.ovf_slots = 0;
@@ -591,8 +593,120 @@ int zipnn_b200_decompress_batch_workspace_size(const zipnn_b200_batch_item* item
   return ZIPNN_B200_OK;
 }
 
+// ---- the per-bitstream-CTA family over a batch, in two halves ----
+// The prepare half depends on the streams only: descriptors to the device, item tables, modes and work lists
+// (k_decode_meta_batch), parsed Huffman table descriptions (k_parse_tables_batch).  The decode half writes the
+// output: it only reads the counts, lists and tables the prepare half left, and writes the output, the plane pool
+// and the error bits, so a decode plan enqueues it again for every run.
+struct BatchGrid {
+  uint64_t chunks, items, tiles, max_ovf;  // chunk_start[n], item_start[n], tile_start[n]; overflow CTAs per tensor
+};
+
+static int batch_prepare(const std::vector<DecodeCfg>& cfgs, const std::vector<uint64_t>& starts, int n, uint8_t* ws, uint64_t max_ovf,
+                         cudaStream_t st, BatchCfg& B, BatchGrid& grid) {
+  grid.chunks = starts[n];
+  grid.items = starts[2 * (n + 1) - 1];
+  grid.tiles = starts[3 * (n + 1) - 1];
+  grid.max_ovf = max_ovf;
+  // descriptors to the device (pageable source: the copy is staged before the call returns)
+  uint8_t* d_cfgs = ws + 256;
+  uint8_t* d_starts = d_cfgs + sizeof(DecodeCfg) * (size_t)n;
+  ZB_CUDA(cudaMemcpyAsync(d_cfgs, cfgs.data(), sizeof(DecodeCfg) * (size_t)n, cudaMemcpyHostToDevice, st));
+  ZB_CUDA(cudaMemcpyAsync(d_starts, starts.data(), sizeof(uint64_t) * starts.size(), cudaMemcpyHostToDevice, st));
+  B.cfgs = (const DecodeCfg*)d_cfgs;
+  B.chunk_start = (const uint64_t*)d_starts;
+  B.item_start = B.chunk_start + (n + 1);
+  B.tile_start = B.item_start + (n + 1);
+  B.n = (uint32_t)n;
+  B.error_out = (uint32_t*)ws;
+  if (grid.chunks) {
+    {
+      const int threads = 128;
+      const unsigned blocks = (unsigned)std::min<uint64_t>((grid.chunks + threads - 1) / threads, 4096);
+      ScopedTimer tm(kKDecodeMeta, st);
+      k_decode_meta_batch<<<blocks, threads, 0, st>>>(B);
+      ZB_LAUNCHED();
+    }
+    {
+      ScopedTimer tp(kKParseTables, st);
+      k_parse_tables_batch<<<(unsigned)(((grid.items >> 2) + kParseWarps - 1) / kParseWarps), kParseWarps * 32, 0, st>>>(B);
+      ZB_LAUNCHED();
+    }
+  }
+  return ZIPNN_B200_OK;
+}
+
+// The sync decoder of a decode plan: record (create) or replay (run) of the segment starts.
+extern "C++" template <int M>
+int launch_sync_plan(const BatchCfg& B, const SegIndex& X, uint64_t items, cudaStream_t st) {
+  static bool attr_done = false;
+  if (!attr_done) {
+    ZB_CUDA(cudaFuncSetAttribute(k_huf_decode_sync_plan<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSyncSmemBytes));
+    attr_done = true;
+  }
+  static const int nb = [] {
+    int v = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_huf_decode_sync_plan<M>, kSyncThreads, kSyncSmemBytes) != cudaSuccess || v < 1) v = 1;
+    return v;
+  }();
+  const unsigned blocks = (unsigned)std::min<uint64_t>(items, (uint64_t)nb * sm_count_cached());
+  ScopedTimer tm(kKHufDecodeSync, st);
+  k_huf_decode_sync_plan<M><<<blocks, kSyncThreads, kSyncSmemBytes, st>>>(B, X);
+  ZB_LAUNCHED();
+  return ZIPNN_B200_OK;
+}
+
+// No host work besides the launches once a first call has set the kernel attribute (a decode plan's create does).
+// mode: kSyncDecode (the batch and slice calls), or kSyncRecord / kSyncReplay with a plan's segment index X.
+static int batch_decode(const BatchCfg& B, const BatchGrid& grid, cudaStream_t st, int mode = kSyncDecode, const SegIndex* X = nullptr) {
+  if (!grid.chunks) return ZIPNN_B200_OK;
+  const int sms = sm_count_cached();
+  if (mode != kSyncDecode) {
+    const int rc = mode == kSyncRecord ? launch_sync_plan<kSyncRecord>(B, *X, grid.items, st) : launch_sync_plan<kSyncReplay>(B, *X, grid.items, st);
+    if (rc) return rc;
+  } else {
+    static bool attr_done = false;
+    if (!attr_done) {
+      ZB_CUDA(cudaFuncSetAttribute(k_huf_decode_sync_batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSyncSmemBytes));
+      attr_done = true;
+    }
+    static const int nb = [] {
+      int v = 0;
+      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_huf_decode_sync_batch, kSyncThreads, kSyncSmemBytes) != cudaSuccess || v < 1) v = 1;
+      return v;
+    }();
+    const unsigned blocks = (unsigned)std::min<uint64_t>(grid.items, (uint64_t)nb * sms);
+    ScopedTimer tm(kKHufDecodeSync, st);
+    k_huf_decode_sync_batch<<<blocks, kSyncThreads, kSyncSmemBytes, st>>>(B);
+    ZB_LAUNCHED();
+  }
+  {
+    const unsigned blocks = (unsigned)std::min<uint64_t>(grid.tiles, (uint64_t)sms * 16);
+    ScopedTimer tm(kKRegroup, st);
+    k_regroup_batch<<<blocks, kMergeThreads, 0, st>>>(B);
+    ZB_LAUNCHED();
+  }
+  if (grid.max_ovf) {
+    ScopedTimer tm(kKDecodeOverflow, st);
+    k_decode_overflow_batch<<<dim3((unsigned)grid.max_ovf, B.n), kMergeThreads, sizeof(DecodeSmem), st>>>(B);
+    ZB_LAUNCHED();
+  }
+  return ZIPNN_B200_OK;
+}
+
+// OR of every tensor's error word into the batch's (its workspace's first word).
+static int batch_errors(const BatchCfg& B, cudaStream_t st) {
+  k_batch_errors<<<1, 256, 0, st>>>(B);
+  ZB_LAUNCHED();
+  return ZIPNN_B200_OK;
+}
+
 static int run_batch_kernels(const std::vector<DecodeCfg>& cfgs, const std::vector<uint64_t>& starts, int n, uint8_t* ws, uint64_t max_ovf,
-                             cudaStream_t st, BatchCfg& B);
+                             cudaStream_t st, BatchCfg& B) {
+  BatchGrid grid;
+  const int rc = batch_prepare(cfgs, starts, n, ws, max_ovf, st, B, grid);
+  return rc ? rc : batch_decode(B, grid, st);
+}
 
 int zipnn_b200_decompress_batch(const zipnn_b200_batch_item* items, int n, void* d_ws, size_t ws_bytes, void* cuda_stream, int check) {
   if (n < 0 || (n && !items) || !d_ws || ((uintptr_t)d_ws & 255)) return ZIPNN_B200_E_ARG;
@@ -648,8 +762,10 @@ int zipnn_b200_decompress_batch(const zipnn_b200_batch_item* items, int n, void*
                                          (void*)cfgs[i].ctrl, batch_slice_bytes(it), st, 0);
     if (rc) return rc;
   }
-  k_batch_errors<<<1, 256, 0, st>>>(B);
-  ZB_LAUNCHED();
+  {
+    const int rc = batch_errors(B, st);
+    if (rc) return rc;
+  }
   if (check) return read_ctrl_error(d_ws, st);
   return ZIPNN_B200_OK;
 }
@@ -787,72 +903,199 @@ int zipnn_b200_decompress_slices(const zipnn_b200_slice_item* items, int n, void
     const int rc = run_batch_kernels(cfgs, starts, np, ws, max_ovf, st, B);
     if (rc) return rc;
   }
-  k_batch_errors<<<1, 256, 0, st>>>(B);
-  ZB_LAUNCHED();
+  {
+    const int rc = batch_errors(B, st);
+    if (rc) return rc;
+  }
   if (check) return read_ctrl_error(d_ws, st);
   return ZIPNN_B200_OK;
 }
 
-// Descriptors to the device, then one launch of each kernel of the per-bitstream-CTA family for all of them.
-static int run_batch_kernels(const std::vector<DecodeCfg>& cfgs, const std::vector<uint64_t>& starts, int n, uint8_t* ws, uint64_t max_ovf,
-                             cudaStream_t st, BatchCfg& B) {
-  const uint64_t* chunk_start = starts.data();
-  const uint64_t* item_start = chunk_start + (n + 1);
-  const uint64_t* tile_start = item_start + (n + 1);
-  // descriptors to the device (pageable source: the copy is staged before the call returns)
-  uint8_t* d_cfgs = ws + 256;
-  uint8_t* d_starts = d_cfgs + sizeof(DecodeCfg) * (size_t)n;
-  ZB_CUDA(cudaMemcpyAsync(d_cfgs, cfgs.data(), sizeof(DecodeCfg) * (size_t)n, cudaMemcpyHostToDevice, st));
-  ZB_CUDA(cudaMemcpyAsync(d_starts, starts.data(), sizeof(uint64_t) * starts.size(), cudaMemcpyHostToDevice, st));
-  B.cfgs = (const DecodeCfg*)d_cfgs;
-  B.chunk_start = (const uint64_t*)d_starts;
-  B.item_start = B.chunk_start + (n + 1);
-  B.tile_start = B.item_start + (n + 1);
-  B.n = (uint32_t)n;
-  B.error_out = (uint32_t*)ws;
-  const int sms = sm_count_cached();
-  if (chunk_start[n]) {
-    {
-      const int threads = 128;
-      const unsigned blocks = (unsigned)std::min<uint64_t>((chunk_start[n] + threads - 1) / threads, 4096);
-      ScopedTimer tm(kKDecodeMeta, st);
-      k_decode_meta_batch<<<blocks, threads, 0, st>>>(B);
-      ZB_LAUNCHED();
+// ---- decode plans: the prepare half once, the decode half per run ------------------------------------------
+// Plan memory: [256 B: error word][DecodeCfg np][chunk_start, item_start, tile_start][segment index base, np + 1]
+// [per piece: the workspace slice up to its plane pool][segment index].  Scratch: per piece, the plane pool of a
+// slice piece.
+namespace {
+constexpr uint64_t kPlanMagic = 0x7a6e6e706c616e32ull;  // "znnplan2"
+constexpr uint64_t kSegPerItem = 4ull * kSyncThreads;   // index entries per coded item (4 bitstreams x 256 threads)
+struct PlanState {
+  uint64_t magic;  // kPlanMagic once create succeeded
+  BatchCfg B;
+  BatchGrid grid;
+  SegIndex X;
+  uint64_t coded;  // coded items the segment index has room for
+  int32_t mode;    // kSyncReplay, or kSyncDecode for a plan without an index
+};
+static_assert(sizeof(PlanState) <= sizeof(zipnn_b200_decode_plan), "the plan state must fit the ABI's opaque struct");
+size_t plan_piece_meta_bytes(const zipnn_b200_slice_item& it, const SlicePiece& p) {
+  return round_up(dec_ws_layout(it.orig, it.num_buf, it.chunk, p.c1 - p.c0).planes_off, 256);
+}
+size_t plan_piece_scratch_bytes(const zipnn_b200_slice_item& it, const SlicePiece& p) {
+  const uint64_t kc = p.c1 - p.c0;
+  const DecWs L = dec_ws_layout(it.orig, it.num_buf, it.chunk, kc);
+  const uint64_t slots = kc <= kDefaultSlots ? kc : kDefaultSlots + kOverflowCtas;
+  return round_up((size_t)slots * it.num_buf * L.pstride, 256);
+}
+bool plan_state(const zipnn_b200_decode_plan* plan, PlanState& s) {
+  if (!plan) return false;
+  memcpy(&s, plan->opaque, sizeof(s));
+  return s.magic == kPlanMagic;
+}
+struct PlanLayout {
+  std::vector<SlicePiece> pieces;
+  std::vector<uint64_t> seg_base;  // [np + 1] index entries in front of each piece
+  size_t base_off, metas_off, index_off, plan_bytes, scratch_bytes;
+  bool replay;
+};
+// Pieces, the coded items each of them may queue and the memory split.  The coded items of a piece are the type-1
+// entries of its stream's type rows over the piece's covering chunks: every item k_decode_meta_batch can put on the
+// piece's hlist is one of them.  Reading the type rows synchronises `st`.  ZIPNN_B200_PLAN_REPLAY=0 builds plans
+// without an index, whose runs take the rounds of the decode mode (tools/plan_bench.py compares the two).
+int plan_layout(const zipnn_b200_slice_item* items, int n, cudaStream_t st, PlanLayout& P) {
+  const int rc = plan_slices(items, n, P.pieces);
+  if (rc) return rc;
+  const char* e = getenv("ZIPNN_B200_PLAN_REPLAY");
+  P.replay = !(e && atoi(e) == 0);
+  const size_t np = P.pieces.size();
+  std::vector<std::vector<uint8_t>> types((size_t)n);
+  if (P.replay) {
+    for (const SlicePiece& p : P.pieces) {
+      const zipnn_b200_slice_item& it = items[p.item];
+      const uint64_t K = num_chunks(it.orig, it.chunk), rows = (uint64_t)it.num_buf * K;
+      if (!types[p.item].empty() || it.body_len < 9 * rows) continue;  // (a short body fails at create)
+      types[p.item].resize(rows);
+      ZB_CUDA(cudaMemcpyAsync(types[p.item].data(), it.d_body, rows, cudaMemcpyDeviceToHost, st));
     }
-    {
-      static bool attr_done = false;
-      if (!attr_done) {
-        ZB_CUDA(cudaFuncSetAttribute(k_huf_decode_sync_batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSyncSmemBytes));
-        attr_done = true;
-      }
-      static const int nb = [] {
-        int v = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_huf_decode_sync_batch, kSyncThreads, kSyncSmemBytes) != cudaSuccess || v < 1) v = 1;
-        return v;
-      }();
-      const unsigned grid = (unsigned)std::min<uint64_t>(item_start[n], (uint64_t)nb * sms);
-      {
-        ScopedTimer tp(kKParseTables, st);
-        k_parse_tables_batch<<<(unsigned)(((item_start[n] >> 2) + kParseWarps - 1) / kParseWarps), kParseWarps * 32, 0, st>>>(B);
-        ZB_LAUNCHED();
-      }
-      ScopedTimer tm(kKHufDecodeSync, st);
-      k_huf_decode_sync_batch<<<grid, kSyncThreads, kSyncSmemBytes, st>>>(B);
-      ZB_LAUNCHED();
-    }
-    {
-      const unsigned grid = (unsigned)std::min<uint64_t>(tile_start[n], (uint64_t)sms * 16);
-      ScopedTimer tm(kKRegroup, st);
-      k_regroup_batch<<<grid, kMergeThreads, 0, st>>>(B);
-      ZB_LAUNCHED();
-    }
-    if (max_ovf) {
-      ScopedTimer tm(kKDecodeOverflow, st);
-      k_decode_overflow_batch<<<dim3((unsigned)max_ovf, (unsigned)n), kMergeThreads, sizeof(DecodeSmem), st>>>(B);
-      ZB_LAUNCHED();
-    }
+    ZB_CUDA(cudaStreamSynchronize(st));
   }
+  P.seg_base.assign(np + 1, 0);
+  for (size_t j = 0; j < np; j++) {
+    const SlicePiece& p = P.pieces[j];
+    const zipnn_b200_slice_item& it = items[p.item];
+    const std::vector<uint8_t>& ty = types[p.item];
+    uint64_t coded = 0;
+    if (!ty.empty()) {
+      const uint64_t K = num_chunks(it.orig, it.chunk);
+      for (int g = 0; g < it.num_buf; g++)
+        for (uint64_t c = p.c0; c < p.c1; c++) coded += ty[(uint64_t)g * K + c] == 1;
+    }
+    P.seg_base[j + 1] = P.seg_base[j] + coded * kSegPerItem;
+  }
+  P.base_off = batch_header_bytes((int)np);
+  P.metas_off = P.base_off + round_up(sizeof(uint64_t) * (np + 1), 256);
+  size_t at = P.metas_off, scratch = 0;
+  for (const SlicePiece& p : P.pieces) {
+    at += plan_piece_meta_bytes(items[p.item], p);
+    scratch += plan_piece_scratch_bytes(items[p.item], p);
+  }
+  P.index_off = at;
+  P.plan_bytes = at + sizeof(SegEntry) * (size_t)P.seg_base[np];
+  P.scratch_bytes = scratch;
   return ZIPNN_B200_OK;
+}
+}  // namespace
+
+int zipnn_b200_decode_plan_size(const zipnn_b200_slice_item* items, int n, void* cuda_stream, size_t* plan_bytes, size_t* scratch_bytes) {
+  if (!plan_bytes || !scratch_bytes) return ZIPNN_B200_E_ARG;
+  PlanLayout P;
+  const int rc = plan_layout(items, n, (cudaStream_t)cuda_stream, P);
+  if (rc) return rc;
+  *plan_bytes = P.plan_bytes;
+  *scratch_bytes = P.scratch_bytes;
+  return ZIPNN_B200_OK;
+}
+
+int zipnn_b200_decode_plan_create(const zipnn_b200_slice_item* items, int n, void* d_plan, size_t plan_bytes, void* d_scratch,
+                                  size_t scratch_bytes, zipnn_b200_decode_plan* plan, void* cuda_stream) {
+  if (!plan) return ZIPNN_B200_E_ARG;
+  memset(plan, 0, sizeof(*plan));
+  if (!d_plan || ((uintptr_t)d_plan & 255) || ((uintptr_t)d_scratch & 255) || (scratch_bytes && !d_scratch)) return ZIPNN_B200_E_ARG;
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  PlanLayout P;
+  {
+    const int rc = plan_layout(items, n, st, P);
+    if (rc) return rc;
+  }
+  if (plan_bytes < P.plan_bytes || scratch_bytes < P.scratch_bytes) return ZIPNN_B200_E_CAPACITY;
+  const int np = (int)P.pieces.size();
+  uint8_t* meta = (uint8_t*)d_plan;
+  uint8_t* scratch = (uint8_t*)d_scratch;
+  size_t at = P.metas_off, sat = 0;
+  std::vector<DecodeCfg> cfgs((size_t)np);
+  std::vector<uint64_t> starts(3 * ((size_t)np + 1), 0);
+  uint64_t* chunk_start = starts.data();
+  uint64_t* item_start = chunk_start + (np + 1);
+  uint64_t* tile_start = item_start + (np + 1);
+  uint64_t max_ovf = 1;  // (as in the slice call: a fixed launch count)
+  for (int j = 0; j < np; j++) {
+    const SlicePiece& p = P.pieces[j];
+    const zipnn_b200_slice_item& it = items[p.item];
+    const size_t mb = plan_piece_meta_bytes(it, p), sb = plan_piece_scratch_bytes(it, p);
+    const uint64_t kc = p.c1 - p.c0;
+    DecodeCfg& cfg = cfgs[j];
+    const int rc = fill_decode_cfg(cfg, it.d_body, it.body_len, it.num_buf, it.bits_mode, it.chunk, it.orig, (uint8_t*)it.d_out + p.out_off,
+                                   meta + at, mb, true, kc, scratch + sat, sb);
+    if (rc) return rc;
+    // a piece that is a whole tensor decodes without the window, as in the batch call
+    const bool whole = p.base == 0 && p.rows == 1 && p.len == it.orig;
+    if (!whole) {
+      cfg.box_base = p.base;
+      cfg.box_rows = p.rows;
+      cfg.box_pitch = p.pitch;
+      cfg.box_len = p.len;
+      cfg.box_step_rows = kBoxStep / p.pitch;
+      cfg.box_step_cols = kBoxStep % p.pitch;
+      cfg.box_fast = ((p.base | p.pitch | p.len) & 15) == 0;
+      cfg.c0 = p.c0;
+    }
+    chunk_start[j + 1] = chunk_start[j] + kc;
+    item_start[j + 1] = item_start[j] + 4ull * it.num_buf * kc;
+    tile_start[j + 1] = tile_start[j] + kc * ((it.chunk + kMergeTile - 1) / kMergeTile);
+    max_ovf = std::max<uint64_t>(max_ovf, cfg.ovf_slots);
+    at += mb;
+    sat += sb;
+  }
+  // error word, every piece's control block, and the index (entries of items that turn out raw or RLE stay empty)
+  ZB_CUDA(cudaMemsetAsync(meta, 0, P.plan_bytes, st));
+  ZB_CUDA(cudaMemcpyAsync(meta + P.base_off, P.seg_base.data(), sizeof(uint64_t) * P.seg_base.size(), cudaMemcpyHostToDevice, st));
+  PlanState s;
+  memset(&s, 0, sizeof(s));
+  s.X.seg = (SegEntry*)(meta + P.index_off);
+  s.X.base = (const uint64_t*)(meta + P.base_off);
+  s.coded = P.seg_base[np] / kSegPerItem;
+  s.mode = P.replay ? kSyncReplay : kSyncDecode;
+  {
+    int rc = batch_prepare(cfgs, starts, np, meta, max_ovf, st, s.B, s.grid);
+    if (!rc) rc = batch_decode(s.B, s.grid, st, P.replay ? kSyncRecord : kSyncDecode, &s.X);
+    if (!rc) rc = batch_errors(s.B, st);
+    if (!rc) rc = read_ctrl_error(meta, st);
+    if (rc) return rc;
+  }
+  s.magic = kPlanMagic;
+  memcpy(plan->opaque, &s, sizeof(s));
+  return ZIPNN_B200_OK;
+}
+
+int zipnn_b200_decode_plan_index(const zipnn_b200_decode_plan* plan, size_t* index_bytes, size_t* coded_items) {
+  PlanState s;
+  if (!plan_state(plan, s) || !index_bytes || !coded_items) return ZIPNN_B200_E_ARG;
+  *coded_items = s.mode == kSyncReplay ? s.coded : 0;
+  *index_bytes = *coded_items * kSegPerItem * sizeof(SegEntry);
+  return ZIPNN_B200_OK;
+}
+
+int zipnn_b200_decode_plan_run(const zipnn_b200_decode_plan* plan, void* cuda_stream) {
+  PlanState s;
+  if (!plan_state(plan, s)) return ZIPNN_B200_E_ARG;
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  const int rc = batch_decode(s.B, s.grid, st, s.mode, &s.X);
+  return rc ? rc : batch_errors(s.B, st);
+}
+
+int zipnn_b200_decode_plan_status(const zipnn_b200_decode_plan* plan, void* cuda_stream) {
+  PlanState s;
+  if (!plan_state(plan, s)) return ZIPNN_B200_E_ARG;
+  return read_ctrl_error(s.B.error_out, (cudaStream_t)cuda_stream);
 }
 
 int zipnn_b200_split(const void* d_in, size_t n, int num_buf, int bits_mode, void* d_planes, size_t stride,

@@ -1,0 +1,170 @@
+"""`DecodePlan` -- decode the same compressed tensors again and again with no host work per decode.
+
+A plan is made once from a list of CUDA torch-format ZipNN streams: their headers are parsed (one synchronising
+device-to-host copy for all of them), the outputs are laid out in one buffer, and `zipnn_b200_decode_plan_create`
+validates the streams, builds everything that depends only on them and decodes once, recording where every segment
+of the per-bitstream-CTA decoder starts.  `run()` then only enqueues the decode kernels, which decode each segment
+once from its recorded start, on the current CUDA stream (a fixed number of launches, capturable in a CUDA graph) and
+rewrites the same output tensors.  This is what keeps weights compressed in HBM (resident.py): a module's weights
+are decoded just before it runs.
+
+Lifetime rules (include/zipnn_b200.h): the streams must not change while the plan lives (the plan keeps references
+to them); plans that share a scratch buffer must run ordered on one stream; plans that share an output buffer
+overwrite each other's outputs.
+"""
+from __future__ import annotations
+
+import ctypes as C
+
+import torch
+
+from . import _native
+from .util_header import EnumFormat
+from .util_torch import torch_dtype_of_code
+from .zipnn import HEADER_LEN, HUF_MAX_BLOCK, ZipNN, _cuda_stream_handle
+
+_HEAD = HEADER_LEN + 1 + 9 * 255   # the 32-byte header and the longest packed shape (as decompress peeks)
+_ALIGN = 16
+
+
+def _round(n: int, a: int) -> int:
+    return (n + a - 1) // a * a
+
+
+class _Stream:
+    """What the header of one torch-format stream says: where the body starts, the decoded bytes and layout."""
+
+    def __init__(self, stream: torch.Tensor, head: bytes):
+        z = ZipNN(input_format="torch")
+        if len(head) < HEADER_LEN:
+            raise ValueError("Header should start with ZN")
+        after = z._retrieve_header(head)
+        if z.input_format != EnumFormat.TORCH.value or head[9] != 0 or z.is_streaming:
+            raise ValueError("DecodePlan takes torch-format streams without delta compression or streaming frames")
+        if stream.numel() < after:
+            raise RuntimeError("corrupt ZipNN stream: truncated header")
+        self.stream = stream
+        self.after = after
+        self.num_buf = z._num_buf_of_dtype()
+        self.bits_mode, self.bytes_mode = z._bit_reorder, z._byte_reorder
+        self.chunk = z.compression_chunk if self.num_buf != 1 else min(HUF_MAX_BLOCK, z.compression_chunk)
+        self.nbytes = z.original_len
+        self.dtype = torch_dtype_of_code(z.dtype)
+        self.shape = tuple(z.shape_bytes)
+
+
+def _parse(streams) -> list:
+    streams = [s for s in streams]
+    for s in streams:
+        if not (isinstance(s, torch.Tensor) and s.is_cuda and s.dtype == torch.uint8 and s.dim() == 1 and s.is_contiguous()):
+            raise ValueError("DecodePlan takes flat contiguous CUDA uint8 streams")
+    if len({s.device for s in streams}) > 1:
+        raise ValueError("DecodePlan takes streams on one device")
+    if not streams:
+        return []
+    heads = torch.cat([s[:_HEAD] for s in streams]).cpu().numpy().tobytes()   # one synchronising copy
+    out, at = [], 0
+    for s in streams:
+        k = min(s.numel(), _HEAD)
+        out.append(_Stream(s, heads[at: at + k]))
+        at += k
+    return out
+
+
+def _offsets(parsed) -> tuple:
+    offs, at = [], 0
+    for p in parsed:
+        offs.append(at)
+        at = _round(at + p.nbytes, _ALIGN)
+    return offs, at
+
+
+def _items(parsed, offs, out_ptr: int):
+    arr = (_native.SliceItem * max(1, len(parsed)))()
+    for it, p, o in zip(arr, parsed, offs):
+        it.d_body, it.body_len = p.stream.data_ptr() + p.after, p.stream.numel() - p.after
+        it.num_buf, it.bits_mode, it.bytes_mode = p.num_buf, p.bits_mode, p.bytes_mode
+        it.chunk, it.orig = p.chunk, p.nbytes
+        it.base, it.rows, it.pitch, it.len = 0, 1, p.nbytes, p.nbytes
+        it.d_out = out_ptr + o
+    return arr
+
+
+def _sizes(parsed) -> tuple:
+    """-> (out bytes, plan bytes, scratch bytes)."""
+    offs, out_bytes = _offsets(parsed)
+    arr = _items(parsed, offs, 1 << 12)   # (any aligned non-null address: sizing reads no output)
+    pb, sb = C.c_size_t(0), C.c_size_t(0)
+    # (synchronising: reads the streams' type rows to size the segment index)
+    _native.check(_native.lib().zipnn_b200_decode_plan_size(arr, len(parsed), _cuda_stream_handle(), C.byref(pb), C.byref(sb)))
+    return out_bytes, pb.value, sb.value
+
+
+def _raise_status(rc: int) -> None:
+    if rc == _native.E_CORRUPT:
+        raise _native.ZipNNNativeError(rc, "Thread processing failed: corrupt ZipNN stream")
+    _native.check(rc)
+
+
+class DecodePlan:
+    """Decode `streams` (CUDA uint8 torch-format ZipNN streams on one device, as `ZipNN(input_format="torch")
+    .compress` or `compress_batch` return them) into `.outputs` now and on every `run()`.
+
+    out:     optional CUDA uint8 buffer of at least `DecodePlan.sizes(streams)[0]` bytes that receives the outputs
+             (at 16-byte aligned offsets); allocated when not given.
+    scratch: optional CUDA uint8 buffer of at least `DecodePlan.sizes(streams)[1]` bytes, 256-byte aligned, for the
+             plane pools of a run; allocated when not given.  Plans whose runs are ordered on one stream may share it.
+    Raises like `ZipNN.decompress` when a stream is corrupt or unsupported.
+    """
+
+    @staticmethod
+    def sizes(streams) -> tuple:
+        """-> (out_bytes, scratch_bytes) a plan of these streams needs, so that callers can share buffers."""
+        out_bytes, _, scratch_bytes = _sizes(_parse(streams))
+        return out_bytes, scratch_bytes
+
+    def __init__(self, streams, out: torch.Tensor = None, scratch: torch.Tensor = None):
+        _native.require_cuda()
+        parsed = _parse(streams)
+        dev = parsed[0].stream.device if parsed else torch.device("cuda", torch.cuda.current_device())
+        with torch.cuda.device(dev):
+            out_bytes, plan_bytes, scratch_bytes = _sizes(parsed)
+            if out is None:
+                out = torch.empty(max(out_bytes, 1), dtype=torch.uint8, device=dev)
+            if scratch is None:
+                scratch = torch.empty(max(scratch_bytes, 1), dtype=torch.uint8, device=dev)
+            for name, buf, need, align in (("out", out, out_bytes, _ALIGN), ("scratch", scratch, scratch_bytes, 256)):
+                if not (buf.is_cuda and buf.device == dev and buf.dtype == torch.uint8 and buf.is_contiguous()):
+                    raise ValueError(f"{name} must be a contiguous CUDA uint8 tensor on the streams' device")
+                if buf.numel() < need or buf.data_ptr() % align:
+                    raise ValueError(f"{name} needs {need} bytes, {align}-byte aligned")
+            self._meta = torch.empty(plan_bytes, dtype=torch.uint8, device=dev)
+            offs, _ = _offsets(parsed)
+            arr = _items(parsed, offs, out.data_ptr())
+            self._plan = _native.DecodePlanStruct()
+            rc = _native.lib().zipnn_b200_decode_plan_create(arr, len(parsed), self._meta.data_ptr(), plan_bytes, scratch.data_ptr(),
+                                                              scratch_bytes, C.byref(self._plan), _cuda_stream_handle())
+        _raise_status(rc)
+        self._streams = [p.stream for p in parsed]   # the plan reads them on every run
+        self._out, self._scratch = out, scratch
+        self.device = dev
+        self.outputs = [out[o: o + p.nbytes].view(p.dtype).reshape(p.shape) for p, o in zip(parsed, offs)]
+        index_bytes, coded = C.c_size_t(0), C.c_size_t(0)
+        _native.check(_native.lib().zipnn_b200_decode_plan_index(C.byref(self._plan), C.byref(index_bytes), C.byref(coded)))
+        self.coded_items = coded.value
+        self.nbytes = {"plan": plan_bytes, "scratch": scratch_bytes, "index": index_bytes.value, "out": out_bytes,
+                       "streams": sum(p.stream.numel() for p in parsed), "dense": sum(p.nbytes for p in parsed)}
+        self._run = _native.lib().zipnn_b200_decode_plan_run
+        self._ref = C.byref(self._plan)
+
+    def run(self) -> list:
+        """Enqueue the decode on the current CUDA stream (launches only) and return `.outputs`."""
+        rc = self._run(self._ref, torch.cuda.current_stream(self.device).cuda_stream)
+        if rc:
+            _native.check(rc)
+        return self.outputs
+
+    def check(self) -> None:
+        """Synchronise the current stream and raise if a run so far found an error."""
+        with torch.cuda.device(self.device):
+            _raise_status(_native.lib().zipnn_b200_decode_plan_status(C.byref(self._plan), _cuda_stream_handle()))
