@@ -9,7 +9,7 @@ from .safetensors_io import (SafeOpen, compress_safetensors_file, decompress_saf
                              decompress_safetensors_tensor, load_file, save_file, zipnn_safetensors)
 from .slicing import CompressedSlice
 from .plan import DecodePlan
-from .resident import compress_module, decompress_module
+from .resident import compress_module, decompress_module, load_module, save_module
 
 
 from .hf import zipnn_hf
@@ -17,4 +17,5 @@ from .hf import zipnn_hf
 
 __all__ = ["ZipNN", "zipnn_safetensors", "SafeOpen", "compress_safetensors_file",
            "decompress_safetensors_file", "decompress_safetensors_tensor", "load_file", "save_file", "DecodePipe",
-           "zipnn_hf", "CompressedSlice", "DecodePlan", "compress_module", "decompress_module"]
+           "zipnn_hf", "CompressedSlice", "DecodePlan", "compress_module", "decompress_module",
+           "load_module", "save_module"]

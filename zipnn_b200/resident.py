@@ -19,13 +19,22 @@ Rules:
     the selection stays dense, as does one whose stream is not smaller than its bytes;
   * `state_dict()` does not see compressed parameters; `decompress_module(model)` restores them as dense
     `Parameter`s, bit for bit, and removes the hooks and plans.
+
+`load_module(model, files)` reaches the same state straight from safetensors / .znn.safetensors files, with no dense
+copy of the compressed weights on the GPU, and `save_module(model, file)` writes a compressed model back to a
+.znn.safetensors file from its streams, with no decode.
 """
 from __future__ import annotations
 
+import os
+import traceback
+
 import torch
 
-from .plan import DecodePlan
-from .zipnn import ZipNN
+from .plan import _HEAD, DecodePlan, _Stream
+from .safetensors_io import _FileRange, _cuda_device, compress_groups, file_entries, save_coded
+from .util_safetensors import COMPRESSION_METHOD
+from .zipnn import DecodePipe, ZipNN
 
 _DTYPES = (torch.bfloat16, torch.float16, torch.float32, torch.float8_e4m3fn, torch.float8_e5m2)
 _ATTR = "_zipnn_resident"
@@ -78,7 +87,7 @@ class _Resident:
         self.entries = []     # (module, plan, [(name, index into the plan's outputs)], [hook handles])
         self.params = {}      # parameter index -> (requires_grad, dtype, shape, [(module, name)] where it was bound)
         self.stream_of = {}   # parameter index -> its stream (a view of `streams`)
-        self.streams = None   # the one buffer that holds every stream
+        self.streams = []     # the buffers that hold the streams (one per load group)
         self.order = {}       # id(module) -> (module, its parameter names in their original order)
 
 
@@ -100,6 +109,69 @@ def _unbind(names):
     return hook
 
 
+_EMPTY_REPORT = {"dense_bytes": 0, "stream_bytes": 0, "plan_bytes": 0, "index_bytes": 0, "scratch_bytes": 0, "out_bytes": 0,
+                 "params": 0, "modules": 0}
+
+
+def _pack(streams: dict, dev) -> tuple:
+    """{group index: CUDA uint8 stream} -> (one tight buffer holding them at 16-byte aligned offsets, {index: its
+    view}); the sources are only read."""
+    offs, at = {}, 0
+    for i, s in streams.items():
+        offs[i] = at
+        at = (at + s.numel() + 15) // 16 * 16
+    buf = torch.empty(max(at, 1), dtype=torch.uint8, device=dev)
+    views = {}
+    for i, s in streams.items():
+        views[i] = buf[offs[i]: offs[i] + s.numel()]
+        views[i].copy_(s)
+    return buf, views
+
+
+def _resident_state(modules, groups, streams: dict, buffers: list, dev) -> tuple:
+    """The back half of compress_module and load_module: streams {group index: CUDA stream} -> per selected module
+    one DecodePlan over its parameters' streams, all sharing one output and one scratch buffer.  Raises like
+    `decompress` on a corrupt stream; nothing outside is touched until `_commit`.  -> (_Resident, report)."""
+    where = {id(groups[i][0]): i for i in streams}
+    per_module = []
+    for m in modules:
+        names = [(n, where[id(p)]) for n, p in _own_params(m) if id(p) in where]
+        if names:
+            per_module.append((m, names))
+    sizes = [DecodePlan.sizes([streams[i] for _, i in names]) for _, names in per_module]
+    out = torch.empty(max([s[0] for s in sizes] + [1]), dtype=torch.uint8, device=dev)
+    scratch = torch.empty(max([s[1] for s in sizes] + [1]), dtype=torch.uint8, device=dev)
+    state = _Resident()
+    state.streams = buffers
+    plan_bytes = index_bytes = 0
+    for m, names in per_module:
+        plan = DecodePlan([streams[i] for _, i in names], out=out, scratch=scratch)
+        plan_bytes += plan.nbytes["plan"]
+        index_bytes += plan.nbytes["index"]
+        state.entries.append((m, plan, [(n, k) for k, (n, _) in enumerate(names)], []))
+    dense = 0
+    for i in streams:
+        p, owners = groups[i]
+        dense += p.numel() * p.element_size()
+        state.params[i] = (p.requires_grad, p.dtype, tuple(p.shape), owners)
+    state.stream_of = dict(streams)
+    return state, {"dense_bytes": dense, "stream_bytes": sum(s.numel() for s in streams.values()), "plan_bytes": plan_bytes,
+                   "index_bytes": index_bytes, "scratch_bytes": scratch.numel(), "out_bytes": out.numel(),
+                   "params": len(streams), "modules": len(per_module)}
+
+
+def _commit(module: torch.nn.Module, state: _Resident) -> None:
+    """Hooks on, compressed parameters out: after this the model runs from its streams."""
+    for m, plan, local, hooks in state.entries:
+        hooks += [m.register_forward_pre_hook(_pre_hook(plan, local)), m.register_forward_hook(_unbind(local), always_call=True)]
+    # the dense parameters go: nothing here keeps their storage alive
+    for _, _, _, owners in state.params.values():
+        for o, n in owners:
+            state.order.setdefault(id(o), (o, list(o._parameters)))
+            del o._parameters[n]
+    setattr(module, _ATTR, state)
+
+
 def compress_module(module: torch.nn.Module, modules=None) -> dict:
     """Compress the weights of `modules` (default: every submodule that directly owns bf16 / fp16 / fp32 / fp8
     parameters) into streams kept in HBM, decoded just before each module's forward.  All parameters are compressed
@@ -115,64 +187,18 @@ def compress_module(module: torch.nn.Module, modules=None) -> dict:
     params = [p for p, _ in groups]
     if not params:
         setattr(module, _ATTR, None)
-        return {"dense_bytes": 0, "stream_bytes": 0, "plan_bytes": 0, "index_bytes": 0, "scratch_bytes": 0, "out_bytes": 0,
-                "params": 0, "modules": 0}
+        return dict(_EMPTY_REPORT)
     if not all(p.is_cuda for p in params) or len({p.device for p in params}) > 1:
         raise ValueError("compress_module: the selected parameters must lie on one CUDA device")
     dev = params[0].device
-    with torch.no_grad():
-        coded = ZipNN(input_format="torch").compress_batch([p.detach() for p in params])
-    keep = [i for i, (p, s) in enumerate(zip(params, coded)) if s.numel() < p.numel() * p.element_size()]
+    with torch.no_grad():   # the .znn files' method byte: the streams are the ones save_file writes, byte for byte
+        coded = ZipNN(input_format="torch", method=COMPRESSION_METHOD).compress_batch([p.detach() for p in params])
     # the streams move into one tight buffer; the batch's output buffer (sized by the bound) is dropped
-    offs, at = [], 0
-    for i in keep:
-        offs.append(at)
-        at = (at + coded[i].numel() + 15) // 16 * 16
-    buf = torch.empty(max(at, 1), dtype=torch.uint8, device=dev)
-    streams = {}
-    for i, o in zip(keep, offs):
-        n = coded[i].numel()
-        buf[o: o + n].copy_(coded[i])
-        streams[i] = buf[o: o + n]
-    del coded
-    # per module, the streams of its parameters
-    where = {id(params[i]): i for i in keep}
-    per_module = []
-    for m in modules:
-        names = [(n, where[id(p)]) for n, p in _own_params(m) if id(p) in where]
-        if names:
-            per_module.append((m, names))
-    sizes = [DecodePlan.sizes([streams[i] for _, i in names]) for _, names in per_module]
-    out = torch.empty(max([s[0] for s in sizes] + [1]), dtype=torch.uint8, device=dev)
-    scratch = torch.empty(max([s[1] for s in sizes] + [1]), dtype=torch.uint8, device=dev)
-    state = _Resident()
-    state.streams = buf
-    plan_bytes = index_bytes = 0
-    for m, names in per_module:
-        idx = [i for _, i in names]
-        plan = DecodePlan([streams[i] for i in idx], out=out, scratch=scratch)
-        plan_bytes += plan.nbytes["plan"]
-        index_bytes += plan.nbytes["index"]
-        local = [(n, k) for k, (n, _) in enumerate(names)]
-        state.entries.append((m, plan, local, [m.register_forward_pre_hook(_pre_hook(plan, local)),
-                                               m.register_forward_hook(_unbind(local), always_call=True)]))
-    # the dense parameters go: nothing here keeps their storage alive
-    dense = 0
-    restore = {}
-    for i in keep:
-        p, owners = groups[i]
-        dense += p.numel() * p.element_size()
-        restore[i] = (p.requires_grad, p.dtype, tuple(p.shape), owners)
-        for o, n in owners:
-            state.order.setdefault(id(o), (o, list(o._parameters)))
-            del o._parameters[n]
-    state.params = restore
-    state.stream_of = {i: streams[i] for i in keep}
-    del params, groups
-    setattr(module, _ATTR, state)
-    return {"dense_bytes": dense, "stream_bytes": sum(s.numel() for s in state.stream_of.values()), "plan_bytes": plan_bytes,
-            "index_bytes": index_bytes, "scratch_bytes": scratch.numel(), "out_bytes": out.numel(), "params": len(keep),
-            "modules": len(per_module)}
+    buf, streams = _pack({i: s for i, (p, s) in enumerate(zip(params, coded)) if s.numel() < p.numel() * p.element_size()}, dev)
+    del coded, params
+    state, report = _resident_state(modules, groups, streams, [buf], dev)
+    _commit(module, state)
+    return report
 
 
 def decompress_module(module: torch.nn.Module) -> None:
@@ -213,3 +239,305 @@ def decompress_module(module: torch.nn.Module) -> None:
         params.update(reordered)
     state.entries.clear()
     delattr(module, _ATTR)
+
+
+def state_names(module: torch.nn.Module) -> list:
+    """`module`'s full dense state in `state_dict()` order, compressed parameters at their owners' names (where
+    `decompress_module` would put them back): [(name, owner module, attribute, kind, key)], kind "param" (a dense
+    Parameter), "resident" (a compressed one) or "buffer" (a persistent buffer); every name of one tensor has the
+    same key."""
+    state = getattr(module, _ATTR, None)
+    resident = {}
+    if state is not None:
+        for i, (_, _, _, owners) in state.params.items():
+            for o, n in owners:
+                resident[(id(o), n)] = i
+    out = []
+
+    def walk(m, prefix):
+        names = list(m._parameters)
+        if state is not None and id(m) in state.order:
+            first = state.order[id(m)][1]
+            names = first + [n for n in names if n not in first]
+        for n in names:
+            p = m._parameters.get(n)
+            if p is not None:
+                out.append((prefix + n, m, n, "param", id(p)))
+            elif (id(m), n) in resident:
+                out.append((prefix + n, m, n, "resident", ("resident", resident[(id(m), n)])))
+        for n, b in m._buffers.items():
+            if b is not None and n not in m._non_persistent_buffers_set:
+                out.append((prefix + n, m, n, "buffer", id(b)))
+        for n, c in m._modules.items():
+            if c is not None:
+                walk(c, prefix + n + ".")
+
+    walk(module, "")
+    return out
+
+
+def first_names(entries) -> tuple:
+    """`state_names` -> (the first name of every tensor, the later names of tied tensors)."""
+    seen, first, later = set(), [], []
+    for e in entries:
+        (later if e[4] in seen else first).append(e)
+        seen.add(e[4])
+    return first, later
+
+
+class LoadPlan:
+    """What `load_module` does with each key, decided from the module and the files' headers alone."""
+
+    def __init__(self, modules, groups):
+        self.modules, self.groups = modules, groups   # as `select` gives them
+        self.streams = []   # (group index, FileEntry): compressed entries that stay compressed, read as they are
+        self.compress = []  # (group index, FileEntry): plain floating-point entries, compressed on the device
+        self.dense = []     # (FileEntry, [(module, attribute)], kind, requires_grad): read (and decoded) to dense
+        self.moves = []     # (module, name): non-persistent buffers, moved to the device
+        self.kinds = {}     # every state name -> "stream", "compress", "dense" or "alias" (not read)
+
+
+def _stream_header(e) -> _Stream:
+    """The header of a compressed entry, checked as DecodePlan checks it, read from the file (no device work)."""
+    with open(e.file, "rb") as f:
+        f.seek(e.offset)
+        head = f.read(min(e.nbytes, _HEAD))
+    return _Stream(torch.empty(e.nbytes, dtype=torch.uint8, device="meta"), head)
+
+
+def _files(filenames) -> list:
+    if isinstance(filenames, (str, os.PathLike)):
+        return [os.fspath(filenames)]
+    return [os.fspath(f) for f in filenames]
+
+
+def plan_load(module: torch.nn.Module, filenames, modules=None) -> LoadPlan:
+    """The checks and choices of `load_module`, from the files' headers: ValueError naming the keys for a missing or
+    unexpected key, a dtype or shape that differs, a non-persistent buffer on the meta device, and for a module that
+    is already compressed."""
+    if getattr(module, _ATTR, None) is not None:
+        raise ValueError("load_module: this module is already compressed")
+    found = file_entries(_files(filenames))
+    modules, groups = select(module, modules)
+    plan = LoadPlan(modules, groups)
+    group_of = {id(p): gi for gi, (p, _) in enumerate(groups)}
+    by_key = {}
+    for name, m, attr, kind, key in state_names(module):
+        by_key.setdefault(key, []).append((name, m, attr, kind))
+    missing = [names[0][0] for names in by_key.values() if not any(n in found for n, _, _, _ in names)]
+    known = {n for names in by_key.values() for n, _, _, _ in names}
+    unexpected = sorted(k for k in found if k not in known)
+    if missing or unexpected:
+        raise ValueError(f"load_module: keys the files lack: {missing}; keys the module lacks: {unexpected}")
+    meta = []
+    for prefix, m in module.named_modules():
+        for n in m._non_persistent_buffers_set:
+            b = m._buffers.get(n)
+            if b is not None:
+                if b.is_meta:
+                    meta.append(prefix + ("." if prefix else "") + n)
+                else:
+                    plan.moves.append((m, n))
+    if meta:
+        raise ValueError(f"load_module: non-persistent buffers on the meta device (no file holds them): {meta}")
+    wrong = []
+    for key, names in by_key.items():
+        name, m, attr, kind = next(n for n in names if n[0] in found)
+        for n in names:
+            plan.kinds[n[0]] = "alias"
+        e = found[name]
+        t = m._parameters[attr] if kind == "param" else m._buffers[attr]
+        if e.dtype != t.dtype or e.shape != tuple(t.shape):
+            wrong.append(f"{name}: {e.dtype} {list(e.shape)} in the file, {t.dtype} {list(t.shape)} in the module")
+            continue
+        if e.compressed:
+            try:
+                s = _stream_header(e)
+            except (ValueError, RuntimeError) as err:
+                wrong.append(f"{name}: {err}")
+                continue
+            if s.dtype != e.dtype or s.shape != e.shape or s.nbytes != t.numel() * t.element_size():
+                wrong.append(f"{name}: its stream holds {s.dtype} {list(s.shape)}, the metadata says {e.dtype} {list(e.shape)}")
+                continue
+        gi = group_of.get(key) if kind == "param" else None
+        if gi is not None and e.compressed:
+            plan.streams.append((gi, e))
+            plan.kinds[name] = "stream"
+        elif gi is not None and e.floating and not e.znn_file:   # a .znn file stored it raw: it does not compress
+            plan.compress.append((gi, e))
+            plan.kinds[name] = "compress"
+        else:
+            plan.dense.append((e, [(n[1], n[2]) for n in names], kind, kind == "param" and t.requires_grad))
+            plan.kinds[name] = "dense"
+    if wrong:
+        raise ValueError(f"load_module: dtype or shape differs (no casting): {wrong}")
+    plan.streams.sort(key=lambda g: g[0])
+    plan.compress.sort(key=lambda g: g[0])
+    return plan
+
+
+def _load_device(plan: LoadPlan, dev) -> tuple:
+    """Every device step of load_module; the module is not touched.  -> (_Resident or None, report, dense tensors of
+    plan.dense, {group index: dense tensor} of plain entries that did not compress, moved buffers of plan.moves)."""
+    pipe = DecodePipe(dev)
+    fds = {}
+
+    def fd(fn):
+        if fn not in fds:
+            fds[fn] = os.open(fn, os.O_RDONLY)
+        return fds[fn]
+
+    def upload(dst, e):   # file bytes -> device through the pipe's pinned slab ring
+        if e.nbytes:
+            pipe._upload(dst, e.nbytes, lambda d, a, b: pipe._fill_from_file(d, fd(e.file), e.offset + a), cur)
+
+    try:
+        with torch.cuda.device(dev), torch.no_grad():
+            cur = torch.cuda.current_stream()
+            # compressed entries of selected parameters: one buffer, each stream at a 16-byte aligned offset (the
+            # plans' recorded segment starts depend on the address modulo 16), never decoded but by plan create
+            buffers, streams, at, offs = [], {}, 0, []
+            for _, e in plan.streams:
+                offs.append(at)
+                at = (at + e.nbytes + 15) // 16 * 16
+            if plan.streams:
+                buffers.append(torch.empty(at, dtype=torch.uint8, device=dev))
+                for (gi, e), o in zip(plan.streams, offs):
+                    streams[gi] = buffers[0][o: o + e.nbytes]
+                    upload(streams[gi], e)
+            # plain floating-point entries of selected parameters: compressed a group at a time, compress_module's rule
+            entries = [(gi, _FileRange(fd(e.file), e.offset, e.nbytes, e.dtype, e.shape)) for gi, e in plan.compress]
+            stayed = {}
+            for g in compress_groups(entries, dev):
+                small = {}
+                for k, i in enumerate(g.grp):
+                    gi = entries[i][0]
+                    if g.streams[k].numel() < entries[i][1].nbytes:
+                        small[gi] = g.streams[k]
+                    else:
+                        stayed[gi] = g.flats[k].clone()
+                if small:
+                    buf, views = _pack(small, dev)
+                    buffers.append(buf)
+                    streams.update(views)
+                del g, small
+            # everything else becomes dense; compressed entries through the batched decode, one call per run of
+            # entries that lie back to back in a file (a call reads the span from its first to its last entry)
+            dense, runs = [None] * len(plan.dense), {}
+            for j, (e, _, _, _) in enumerate(plan.dense):
+                if e.compressed:
+                    runs.setdefault(e.file, []).append(j)
+                else:
+                    dense[j] = torch.empty(e.shape, dtype=e.dtype, device=dev)
+                    upload(dense[j].view(-1).view(torch.uint8), e)
+            for fn, js in runs.items():
+                js.sort(key=lambda j: plan.dense[j][0].offset)
+                run = []
+                for j in js + [None]:
+                    e = plan.dense[j][0] if j is not None else None
+                    if run and (e is None or plan.dense[run[-1]][0].offset + plan.dense[run[-1]][0].nbytes != e.offset):
+                        got = pipe.submit_file_batch(fd(fn), [(plan.dense[r][0].offset, plan.dense[r][0].nbytes) for r in run])
+                        for r, t in zip(run, got):
+                            er = plan.dense[r][0]
+                            dense[r] = t if t is not None else pipe.submit_file(fd(fn), er.offset, er.nbytes)
+                        run = []
+                    if j is not None:
+                        run.append(j)
+            pipe.finish()
+            moved = [m._buffers[n].to(dev) for m, n in plan.moves]
+            if plan.groups:
+                state, report = _resident_state(plan.modules, plan.groups, dict(sorted(streams.items())), buffers, dev)
+            else:
+                state, report = None, dict(_EMPTY_REPORT)
+        return state, report, dense, stayed, moved
+    finally:
+        pipe.release()
+        for f in fds.values():
+            os.close(f)
+
+
+def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None) -> dict:
+    """Load a checkpoint into `module` with the weights of `modules` kept compressed on `device`: the state
+    `compress_module` leaves (same selection rules, hooks, plans and report), reached without a dense copy of those
+    weights on the GPU.
+
+    filenames: one path or a list of paths, the shards of one checkpoint, .safetensors and .znn.safetensors mixed (the
+    index JSON is not read).  The module's parameters and buffers may be on the meta device, the CPU or `device`.
+
+    Keys follow `load_state_dict(strict=True)`: every key of the module's dense `state_dict()` must be in the files
+    and every key of the files in the module, but for tied parameters: one name of a tied parameter is enough (as
+    `save_module`, `safetensors.torch.save_model` and Hugging Face checkpoints store them); if several are present the
+    first in `state_dict()` order is read and the others are not.  Dtypes and shapes must match (no casting); for a
+    compressed entry both the `znn_compressed_vectors` metadata and the stream's header are checked.  Each violation,
+    a non-persistent buffer on the meta device and an already compressed module raise ValueError naming the keys,
+    from the headers, before any device allocation.
+
+    Where each entry goes:
+      * a compressed entry of a selected parameter: its stream is read from the file (through DecodePipe's pinned slab
+        ring) into one device buffer at a 16-byte aligned offset and stays compressed;
+      * a plain floating-point entry of a selected parameter (plain .safetensors files): compressed on the device in
+        groups of SAVE_GROUP_BYTES input bytes; it stays compressed when its stream is smaller, else dense;
+      * everything else (unselected parameters, ones tied to an unselected owner, entries a .znn file stored raw,
+        non-float tensors, buffers): a dense tensor on `device`; compressed ones through the batched decode.  A
+        parameter becomes a new Parameter with the old one's requires_grad, shared by every owner of a tied one.
+      Non-persistent buffers move to `device`.
+
+    Atomic: the module is changed only after every plan exists (plan create finds a corrupt stream and raises as
+    `decompress` does); on any error the module keeps its tensors, hooks and attributes and the device memory this
+    call allocated is released.
+
+    Device memory: what stays (streams, plans, shared scratch and output buffer, dense tensors) plus transients -- the
+    plans' header peeks (up to 2.3 KB per stream), and for compressed entries that become dense their compressed bytes
+    and the batched decode's workspace; plain entries add one group at a time: its input, its streams' bound and the
+    compress workspace.  A model loaded from .znn files never has its compressed weights dense on the device.
+
+    -> the report of `compress_module`."""
+    dev = _cuda_device(device)
+    if dev is None:
+        raise ValueError(f"load_module: {device!r} is not a CUDA device")
+    if dev.index is None:
+        dev = torch.device("cuda", torch.cuda.current_device())
+    plan = plan_load(module, filenames, modules)
+    try:
+        state, report, dense, stayed, moved = _load_device(plan, dev)
+    except BaseException as e:
+        traceback.clear_frames(e.__traceback__)   # the frames' locals would keep the call's device memory alive
+        raise
+
+    def assign(owners, kind, requires_grad, t):
+        if kind == "param":
+            t = torch.nn.Parameter(t, requires_grad=requires_grad)
+        for o, n in owners:
+            (o._parameters if kind == "param" else o._buffers)[n] = t
+
+    for (_, owners, kind, requires_grad), t in zip(plan.dense, dense):
+        assign(owners, kind, requires_grad, t)
+    for gi, t in stayed.items():
+        p, owners = plan.groups[gi]
+        assign(owners, "param", p.requires_grad, t)
+    for (m, n), b in zip(plan.moves, moved):
+        m._buffers[n] = b
+    if state is None:
+        setattr(module, _ATTR, None)
+    else:
+        _commit(module, state)
+    return report
+
+
+def save_module(module: torch.nn.Module, filename, metadata=None) -> None:
+    """Write `module`'s full state -- its dense `state_dict()` and its compressed parameters at their owners' names --
+    as a .znn.safetensors file, one name per tied parameter (the first in `state_dict()` order).
+
+    Compressed parameters are written from their streams (one device-to-host copy, no decode or encode); dense
+    floating-point tensors are compressed as `save_file` compresses them, adding at most one compress group to the
+    device memory.  The file is byte for byte `save_file` of the dense model's state dict without the later tied names
+    (with `save_file`'s caveat: at most one metadata key)."""
+    state = getattr(module, _ATTR, None)
+    tensors, coded = {}, {}
+    for name, m, attr, kind, key in first_names(state_names(module))[0]:
+        if kind == "resident":
+            _, dtype, shape, _ = state.params[key[1]]
+            coded[name] = (state.stream_of[key[1]], dtype, shape)
+        else:
+            tensors[name] = (m._parameters if kind == "param" else m._buffers)[attr].detach()
+    save_coded(tensors, coded, filename, metadata)

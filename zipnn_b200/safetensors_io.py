@@ -23,7 +23,7 @@ from safetensors.torch import save_file as _save_file
 from .slicing import CompressedSlice
 from .util_header import EnumFormat
 from .util_patch import multi_process_patcher
-from .util_safetensors import (COMPRESSED_DTYPE, COMPRESSION_METHOD, build_compressed_tensor_info,
+from .util_safetensors import (COMPRESSED_DTYPE, COMPRESSION_METHOD, METADATA_KEY, build_compressed_tensor_info,
                                get_compressed_tensors_metadata, set_compressed_tensors_metadata)
 from .util_torch import zipnn_is_floating_point
 from .zipnn import DecodePipe, ZipNN
@@ -39,16 +39,72 @@ def decompress_safetensors_tensor(tensor: torch.Tensor, device=None) -> torch.Te
     return znn.decompress(tensor.contiguous())
 
 
-def _safetensors_index(filename) -> dict:
-    """{tensor name: (absolute file offset, byte length)} from the safetensors header
+def _safetensors_header(filename) -> tuple:
+    """-> (file offset of the data, the header's JSON dict) of a safetensors file
     (8-byte little-endian length, JSON with `data_offsets` relative to the end of the header)."""
     import json
     with open(filename, "rb") as f:
         hlen = int.from_bytes(f.read(8), "little")
         meta = json.loads(f.read(hlen))
-    base = 8 + hlen
+    return 8 + hlen, meta
+
+
+def _safetensors_index(filename) -> dict:
+    """{tensor name: (absolute file offset, byte length)} from the safetensors header."""
+    base, meta = _safetensors_header(filename)
     return {k: (base + v["data_offsets"][0], v["data_offsets"][1] - v["data_offsets"][0])
             for k, v in meta.items() if k != "__metadata__"}
+
+
+class FileEntry:
+    """One tensor of a safetensors / .znn.safetensors file, from the header alone: `nbytes` at `offset` of `file`,
+    the tensor's dtype and shape (for a compressed entry those of `znn_compressed_vectors`, not of its uint8
+    stream), whether it is compressed, and whether the file is a .znn file (one with that metadata key)."""
+
+    def __init__(self, file, offset, nbytes, dtype, shape, compressed, znn_file):
+        self.file, self.offset, self.nbytes, self.dtype, self.shape = file, offset, nbytes, dtype, tuple(shape)
+        self.compressed, self.znn_file = compressed, znn_file
+
+    @property
+    def floating(self) -> bool:
+        return self.dtype in _FLOAT_DTYPES
+
+
+def file_entries(filenames) -> dict:
+    """{name: FileEntry} over the headers of several files, the shards of one checkpoint (no tensor data is read).
+    ValueError for a name found in two files or a dtype the header names that torch lacks."""
+    import json
+    from safetensors.torch import _getdtype
+    out, dups, bad = {}, [], []
+    for fn in filenames:
+        base, meta = _safetensors_header(fn)
+        file_meta = meta.get("__metadata__") or {}
+        comp = get_compressed_tensors_metadata(file_meta)
+        znn = METADATA_KEY in file_meta
+        for k, v in meta.items():
+            if k == "__metadata__":
+                continue
+            if k in out:
+                dups.append(k)
+                continue
+            a, b = v["data_offsets"]
+            info = comp.get(k)
+            try:
+                if info is not None:
+                    dtype, shape = getattr(torch, info["dtype"]), json.loads(info["shape"])
+                    if not isinstance(dtype, torch.dtype):
+                        raise AttributeError(info["dtype"])
+                else:
+                    dtype, shape = _getdtype(v["dtype"]), v["shape"]
+            except (AttributeError, KeyError, TypeError, ValueError):
+                bad.append(k)
+                continue
+            out[k] = FileEntry(fn, base + a, b - a, dtype, shape, info is not None, znn)
+    if dups:
+        raise ValueError(f"keys found in more than one file: {sorted(set(dups))}")
+    if bad:
+        raise ValueError(f"keys with a dtype or shape this reader does not know: {bad}")
+    return out
 
 
 class SafeOpen:
@@ -211,6 +267,7 @@ def _plan_groups(sizes, budget: int) -> list:
 # safetensors dtype names of the floating-point types (anything else is stored as it is)
 _ST_DTYPES = {"F64": "float64", "F32": "float32", "F16": "float16", "BF16": "bfloat16", "F8_E4M3": "float8_e4m3fn",
               "F8_E5M2": "float8_e5m2"}
+_FLOAT_DTYPES = frozenset(getattr(torch, v) for v in _ST_DTYPES.values())
 
 
 class _FileRange:
@@ -232,40 +289,54 @@ def _pread_into(fd: int, mv, off: int) -> None:
         mv, off = mv[got:], off + got
 
 
-def _compress_entries(entries, device, timings=None):
-    """Floating-point entries [(name, CPU/CUDA tensor or _FileRange)] -> ({name: CPU tensor}, infos,
-    compressed bytes, original bytes), the choices `compress_safetensors_file` makes per tensor (a stream
-    that is not smaller keeps the original bytes).  Groups of SAVE_GROUP_BYTES: host bytes are staged in
-    pinned memory (file ranges read with pread) and copied with one host-to-device copy per group, a group
-    is one `ZipNN.compress_batch` call, and every stream is copied back into pinned memory.
-    `timings` (a dict): seconds per phase, added up -- stage, h2d, kernels, d2h (device phases by events)."""
-    from .zipnn import _pinned_empty
+def _cuda_index(device) -> torch.device:
     dev = torch.device(device)
     if dev.type == "cuda" and dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
-    out, infos = {}, {}
-    comp_len = og_len = 0
+    return dev
+
+
+def _align256(v: int) -> int:
+    return (v + 255) // 256 * 256
+
+
+class _Group:
+    """One compressed group of `compress_groups`: `grp` indices into its entries, `flats` the inputs on the device,
+    `streams` their streams (views of the batch's output buffer, sized by the bound), `stage` / `place` the pinned
+    staging buffer and each staged entry's offset in it, `events` [before h2d, after h2d, after the kernels]."""
+
+    def __init__(self, grp, flats, streams, stage, place, events):
+        self.grp, self.flats, self.streams, self.stage, self.place, self.events = grp, flats, streams, stage, place, events
+
+
+def compress_groups(entries, device, timings=None):
+    """Floating-point entries [(key, CPU/CUDA tensor or _FileRange)] -> one `_Group` per group of SAVE_GROUP_BYTES
+    input bytes, compressed on `device` but not synchronised.  Host bytes are staged in pinned memory (file ranges
+    read with pread) and copied with one host-to-device copy per group; a group is one `ZipNN.compress_batch` call.
+    A group's device memory (its inputs, the streams' bound, the workspace) is released when the consumer moves on
+    to the next one, so that one group at a time is on the device.  `timings` (a dict): seconds of staging, added up."""
+    from .zipnn import _pinned_empty
+    dev = _cuda_index(device)
     sizes = [_entry_bytes(src) for _, src in entries]
-    groups = _plan_groups(sizes, SAVE_GROUP_BYTES)
-    align = lambda v: (v + 255) // 256 * 256  # noqa: E731
-    with torch.cuda.device(dev):
-        stream = torch.cuda.current_stream()
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
-        for grp in groups:
-            t0 = time.perf_counter()
-            host = [i for i in grp if not (isinstance(entries[i][1], torch.Tensor) and entries[i][1].is_cuda)]
-            at, place = 0, {}
-            for i in host:
-                place[i] = at
-                at += align(sizes[i])
-            stage = _pinned_empty(at)
-            for i in host:
-                src, a = entries[i][1], place[i]
-                if isinstance(src, _FileRange):
-                    _pread_into(src.fd, memoryview(stage.numpy())[a: a + src.nbytes], src.offset)
-                elif sizes[i]:
-                    stage[a: a + sizes[i]].copy_(src.detach().contiguous().reshape(-1).view(torch.uint8))
-            t1 = time.perf_counter()
+    for grp in _plan_groups(sizes, SAVE_GROUP_BYTES):
+        t0 = time.perf_counter()
+        host = [i for i in grp if not (isinstance(entries[i][1], torch.Tensor) and entries[i][1].is_cuda)]
+        at, place = 0, {}
+        for i in host:
+            place[i] = at
+            at += _align256(sizes[i])
+        stage = _pinned_empty(at)
+        for i in host:
+            src, a = entries[i][1], place[i]
+            if isinstance(src, _FileRange):
+                _pread_into(src.fd, memoryview(stage.numpy())[a: a + src.nbytes], src.offset)
+            elif sizes[i]:
+                stage[a: a + sizes[i]].copy_(src.detach().contiguous().reshape(-1).view(torch.uint8))
+        if timings is not None:
+            timings["stage"] = timings.get("stage", 0.0) + (time.perf_counter() - t0)
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream()
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
             ev[0].record(stream)
             d_stage = stage[:at].to(dev, non_blocking=True) if host else None
             ev[1].record(stream)
@@ -279,37 +350,56 @@ def _compress_entries(entries, device, timings=None):
                     flats.append(s.view(dt).view(shape) if sizes[i] else torch.empty(shape, dtype=dt, device=dev))
                 else:
                     flats.append(src)
-            znn = ZipNN(input_format="torch", method=COMPRESSION_METHOD)
-            streams = znn.compress_batch(flats)
+            streams = ZipNN(input_format="torch", method=COMPRESSION_METHOD).compress_batch(flats)
             ev[2].record(stream)
-            lens = [s.numel() for s in streams]
-            keep = [k for k, i in enumerate(grp) if lens[k] < sizes[i]]
+        yield _Group(grp, flats, streams, stage, place, ev)
+        del flats, streams, d_stage   # before the next group is allocated
+
+
+def _compress_entries(entries, device, timings=None):
+    """Floating-point entries [(name, CPU/CUDA tensor or _FileRange)] -> ({name: CPU tensor}, infos,
+    compressed bytes, original bytes), the choices `compress_safetensors_file` makes per tensor (a stream
+    that is not smaller keeps the original bytes).  The groups of `compress_groups`; every stream is copied
+    back into pinned memory.
+    `timings` (a dict): seconds per phase, added up -- stage, h2d, kernels, d2h (device phases by events)."""
+    from .zipnn import _pinned_empty
+    dev = _cuda_index(device)
+    out, infos = {}, {}
+    comp_len = og_len = 0
+    sizes = [_entry_bytes(src) for _, src in entries]
+    for g in compress_groups(entries, dev, timings):
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream()
+            lens = [s.numel() for s in g.streams]
+            keep = [k for k, i in enumerate(g.grp) if lens[k] < sizes[i]]
             at, hplace = 0, {}
             for k in keep:
                 hplace[k] = at
-                at += align(lens[k])
+                at += _align256(lens[k])
             hout = _pinned_empty(at)
             for k in keep:
-                hout[hplace[k]: hplace[k] + lens[k]].copy_(streams[k], non_blocking=True)
-            ev[3].record(stream)
+                hout[hplace[k]: hplace[k] + lens[k]].copy_(g.streams[k], non_blocking=True)
+            done = torch.cuda.Event(enable_timing=True)
+            done.record(stream)
             stream.synchronize()
-            for k, i in enumerate(grp):
-                name, src = entries[i]
-                og_len += sizes[i]
-                if k in hplace:
-                    comp_len += lens[k]
-                    out[name] = hout[hplace[k]: hplace[k] + lens[k]]
-                    infos[name] = build_compressed_tensor_info(flats[k])
-                else:   # not smaller: the original bytes
-                    comp_len += sizes[i]
-                    if isinstance(src, _FileRange):
-                        out[name] = stage[place[i]: place[i] + sizes[i]].clone().view(src.dtype).view(src.shape)
-                    else:
-                        out[name] = src.cpu()
-            if timings is not None:
-                timings["stage"] = timings.get("stage", 0.0) + (t1 - t0)
-                for key, a, b in (("h2d", 0, 1), ("kernels", 1, 2), ("d2h", 2, 3)):
-                    timings[key] = timings.get(key, 0.0) + ev[a].elapsed_time(ev[b]) / 1e3
+        for k, i in enumerate(g.grp):
+            name, src = entries[i]
+            og_len += sizes[i]
+            if k in hplace:
+                comp_len += lens[k]
+                out[name] = hout[hplace[k]: hplace[k] + lens[k]]
+                infos[name] = build_compressed_tensor_info(g.flats[k])
+            else:   # not smaller: the original bytes
+                comp_len += sizes[i]
+                if isinstance(src, _FileRange):
+                    out[name] = g.stage[g.place[i]: g.place[i] + sizes[i]].clone().view(src.dtype).view(src.shape)
+                else:
+                    out[name] = src.cpu()
+        if timings is not None:
+            ev = g.events + [done]
+            for key, a, b in (("h2d", 0, 1), ("kernels", 1, 2), ("d2h", 2, 3)):
+                timings[key] = timings.get(key, 0.0) + ev[a].elapsed_time(ev[b]) / 1e3
+        del g
     return out, infos, comp_len, og_len
 
 
@@ -357,6 +447,13 @@ def save_file(tensors, filename, metadata=None) -> None:
     byte for byte what `safetensors.torch.save_file` of the tensors followed by `compress_safetensors_file`
     writes.  Floating-point tensors are compressed on the GPU (CPU ones are staged in pinned memory and
     copied over), many per kernel launch; the file is written by `safetensors.torch.save_file`."""
+    save_coded(tensors, {}, filename, metadata)
+
+
+def save_coded(tensors, coded, filename, metadata=None) -> None:
+    """`save_file` of `tensors` plus entries that are already compressed: `coded` = {name: (CUDA uint8 stream,
+    dtype, shape)}, written as they are (one device-to-host copy each, no decode or encode)."""
+    from .zipnn import _pinned_empty
     _check_like_safetensors(tensors)
     plain, floats = {}, []
     for name in sorted(tensors):   # the order a reader of the plain file lists them in, which the metadata JSON follows
@@ -365,12 +462,27 @@ def save_file(tensors, filename, metadata=None) -> None:
             floats.append((name, t))
         else:
             plain[name] = t.cpu()
-    devices = {t.device for _, t in floats if t.is_cuda}
+    devices = {t.device for _, t in floats if t.is_cuda} | {s.device for s, _, _ in coded.values()}
     if len(devices) > 1:
         raise ValueError(f"save_file compresses on one GPU, but the tensors are on {sorted(map(str, devices))}: "
                          "move them to one device (or to the CPU) first")
-    out, infos, _, _ = _compress_entries(floats, devices.pop() if devices else torch.device("cuda"))
+    dev = devices.pop() if devices else torch.device("cuda")
+    out, infos, _, _ = _compress_entries(floats, dev)
     plain.update(out)
+    if coded:
+        at, place = 0, {}
+        for name, (s, _, _) in coded.items():
+            place[name] = at
+            at += _align256(s.numel())
+        hout = _pinned_empty(at)
+        with torch.cuda.device(dev):
+            for name, (s, _, _) in coded.items():
+                hout[place[name]: place[name] + s.numel()].copy_(s, non_blocking=True)
+            torch.cuda.current_stream().synchronize()
+        for name, (s, dtype, shape) in coded.items():
+            plain[name] = hout[place[name]: place[name] + s.numel()]
+            infos[name] = build_compressed_tensor_info(torch.empty(shape, dtype=dtype, device="meta"))
+        infos = {k: infos[k] for k in sorted(infos)}
     _write_compressed(plain, infos, metadata, filename)
 
 
