@@ -186,6 +186,16 @@ int zipnn_b200_decode_plan_create(const zipnn_b200_slice_item* items, int n, voi
 int zipnn_b200_decode_plan_run(const zipnn_b200_decode_plan* plan, void* cuda_stream);
 int zipnn_b200_decode_plan_status(const zipnn_b200_decode_plan* plan, void* cuda_stream);
 int zipnn_b200_decode_plan_index(const zipnn_b200_decode_plan* plan, size_t* index_bytes, size_t* coded_items);
+/* _run_shifted: the decode of _run as ONE kernel launch (no copy, memset or synchronisation: capturable in a CUDA
+ * graph) of at most max_ctas CTAs, with every item's output at d_out + out_shift instead of d_out.  Each target
+ * must be allocated and as large as the item's output; out_shift must be a multiple of 16 (else E_ARG).
+ * max_ctas <= 0: as many CTAs as fit on the device at once; larger values are capped to that.  With few CTAs the
+ * decode leaves the other SMs to concurrent work (a decode of the next layer's weights next to this layer's GEMMs).
+ * Plans without a segment index (ZIPNN_B200_PLAN_REPLAY=0 at create) return E_UNSUPPORTED.  Errors reach the
+ * word _status reads.  Lifetime and scratch rules are _run's: runs of one plan, and runs of plans that share a
+ * scratch buffer, must be ordered on one stream, whichever of _run and _run_shifted enqueues them. */
+int zipnn_b200_decode_plan_run_shifted(const zipnn_b200_decode_plan* plan, int64_t out_shift, int max_ctas,
+                                       void* cuda_stream);
 
 /* ---- stage 1 alone ------------------------------------------------------------ */
 /* d_planes: num_buf planes of `stride` bytes each; plane g receives byte g of every element

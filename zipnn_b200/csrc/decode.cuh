@@ -1743,6 +1743,37 @@ __device__ __forceinline__ void decode_overflow_body(const DecodeCfg& cfg, uint8
   }
 }
 
+// The same for CTA `cta` of `ncta` (at most ovf_slots): it owns plane slot max_slots + cta and takes queued chunks cta,
+// cta + ncta, ...  (k_plan_replay_persistent, whose grid is not the overflow grid.  A copy rather than a parameter of
+// decode_overflow_body: the parameter changes the code the existing launches compile to.)
+template <int G, bool W>
+__device__ __forceinline__ void decode_overflow_part(const DecodeCfg& cfg, uint8_t* __restrict__ out, DecodeSmem& S, PlaneSrc (&src)[G], uint32_t cta,
+                                                     uint32_t ncta) {
+  const uint32_t n = cfg.ctrl->overflow_count;
+  const uint32_t pslot = cfg.max_slots + cta;
+  const uint32_t tiles_per_chunk = (cfg.chunk + kMergeTile - 1) / kMergeTile;
+  for (uint32_t i = cta; i < n; i += ncta) {
+    const uint64_t c = cfg.olist[i];
+    if (threadIdx.x < 32) {
+      const int lane = threadIdx.x, slot = lane >> 2, stream = lane & 3;
+      ItemDesc d;
+      d.kind = kRaw;
+      d.src_off = 0;
+      d.src_len = d.dec_len = 0;
+      bool active = false;
+      if (slot < G) {
+        d = cfg.items[(uint64_t)slot * cfg.K + c];
+        active = (d.kind == kHuf);
+      }
+      planar_decode_item(S, cfg, d, active, slot, stream, cfg.planes + ((uint64_t)pslot * G + (slot < G ? slot : 0)) * cfg.pstride);
+    }
+    __threadfence_block();
+    __syncthreads();  // the planes are complete
+    for (uint32_t tile = 0; tile < tiles_per_chunk; tile++) regroup_tile<G, W>(cfg, out, c, tile, pslot, src);
+    __syncthreads();  // ... and read, before the next chunk overwrites them
+  }
+}
+
 template <int G>
 __global__ void __launch_bounds__(kMergeThreads) k_decode_overflow(DecodeCfg cfg, uint8_t* __restrict__ out) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];

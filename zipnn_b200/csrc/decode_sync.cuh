@@ -673,6 +673,142 @@ __global__ void __launch_bounds__(kSyncThreads) k_huf_decode_sync_plan(BatchCfg 
   }
 }
 
+// ---- a plan's whole decode half in one launch of any number of CTAs, into its outputs moved by out_shift ----
+// The four launches of a plan run (k_huf_decode_sync_plan<kSyncReplay>, k_regroup_batch, k_decode_overflow_batch,
+// k_batch_errors) each fill every SM, so a run on a side stream next to a GEMM takes every SM it can get and its
+// kernels drain one after another.  This kernel does the same work with however many CTAs it is given:
+//   * one claim counter hands out the coded bitstreams (flat index over item_start, as k_huf_decode_sync_plan), then
+//     the regroup tiles (flat index over tile_start, as k_regroup_batch);
+//   * a tile reads the plane pool the bitstreams wrote, so it waits until every bitstream is done: the done counter,
+//     incremented after a fence once per bitstream index, read with an acquire load;
+//   * the overflow chunks (general chunks past the slot pool) go to CTAs 0 .. min(ovf_slots, grid) - 1 of every tensor,
+//     each on its own plane slot max_slots + blockIdx.x, as k_decode_overflow_batch does;
+//   * the last CTA to finish ORs the tensors' error words into the plan's (as k_batch_errors) and zeroes the counters.
+// No deadlock at any co-residency: a CTA waits only once the claim counter has passed every bitstream, so every
+// bitstream it waits for is held by a CTA that is running and never waits before it finishes that bitstream.  One
+// CTA alone decodes every bitstream before its first tile.
+// The counters live in the plan's first 256-byte block behind the error word (the batch workspace header, see
+// batch_prepare); they are zero after create and after every run, so a run is one launch: no memset, capturable in
+// a graph.  Runs that share the counters (one plan) or the plane pool (a shared scratch) must be ordered on one stream.
+struct PlanCounters {
+  uint32_t error;            // BatchCfg::error_out
+  uint32_t finished;         // CTAs past their last unit
+  unsigned long long claim;  // next unit: bitstream indexes [0, items), then tile indexes
+  unsigned long long done;   // bitstream indexes finished
+};
+static_assert(sizeof(PlanCounters) <= 256, "the counters share the error word's 256-byte block");
+constexpr size_t kPlanReplaySmemBytes = kSyncSmemBytes > sizeof(DecodeSmem) ? kSyncSmemBytes : sizeof(DecodeSmem);
+
+// The dispatchers of the batch kernels with the output as an argument (the persistent replay moves it).
+template <bool W>
+__device__ __forceinline__ void sync_replay_to(const DecodeCfg& cfg, uint8_t* __restrict__ out, SyncShared& S, const SyncCarve& cv, uint64_t work,
+                                               SegEntry* seg) {
+  if (cfg.G == 1) sync_process<1, W, kSyncReplay>(cfg, out, S, cv.lut, cv.lut_s, work, seg);
+  else if (cfg.G == 2) sync_process<2, W, kSyncReplay>(cfg, out, S, cv.lut, cv.lut_s, work, seg);
+  else sync_process<4, W, kSyncReplay>(cfg, out, S, cv.lut, cv.lut_s, work, seg);
+}
+template <bool W>
+__device__ __forceinline__ void regroup_tile_to(const DecodeCfg& cfg, uint8_t* __restrict__ out, uint64_t c, uint32_t tile, PlaneSrc (&src)[4]) {
+  if (cfg.G == 1) regroup_tile<1, W>(cfg, out, c, tile, cfg.slot[c], reinterpret_cast<PlaneSrc (&)[1]>(src));
+  else if (cfg.G == 2) regroup_tile<2, W>(cfg, out, c, tile, cfg.slot[c], reinterpret_cast<PlaneSrc (&)[2]>(src));
+  else regroup_tile<4, W>(cfg, out, c, tile, cfg.slot[c], src);
+}
+template <bool W>
+__device__ __forceinline__ void decode_overflow_to(const DecodeCfg& cfg, uint8_t* __restrict__ out, DecodeSmem& S, PlaneSrc (&src)[4], uint32_t cta,
+                                                   uint32_t ncta) {
+  if (cfg.G == 1) decode_overflow_part<1, W>(cfg, out, S, reinterpret_cast<PlaneSrc (&)[1]>(src), cta, ncta);
+  else if (cfg.G == 2) decode_overflow_part<2, W>(cfg, out, S, reinterpret_cast<PlaneSrc (&)[2]>(src), cta, ncta);
+  else decode_overflow_part<4, W>(cfg, out, S, src, cta, ncta);
+}
+
+// The overflow chunks of every tensor: they decode into their own plane slots, so they need no other CTA's work.
+__device__ __forceinline__ void plan_overflow(const BatchCfg& B, int64_t out_shift, DecodeSmem& D, PlaneSrc (&src)[4]) {
+  for (uint32_t t = 0; t < B.n; t++) {
+    const DecodeCfg& cfg = B.cfgs[t];
+    const uint32_t ncta = min(cfg.ovf_slots, gridDim.x);
+    if (blockIdx.x >= ncta || cfg.ctrl->overflow_count == 0) continue;  // (uniform)
+    __syncthreads();  // the shared memory's previous use is over
+    if (cfg.box_len) decode_overflow_to<true>(cfg, cfg.out + out_shift, D, src, blockIdx.x, ncta);
+    else decode_overflow_to<false>(cfg, cfg.out + out_shift, D, src, blockIdx.x, ncta);
+  }
+}
+
+// 157 registers without spills (-Xptxas -v), so one CTA per SM: the claim loop, the replay decoder, the boxed and
+// unboxed regroup and the overflow decoder together.  Bounded to 128 (two per SM) it spills ~100 bytes, to 80 (three,
+// as k_huf_decode_sync_plan) 632; at one per SM a whole-device run takes 2.5x the four-launch run (DESIGN §3.9).
+__global__ void __launch_bounds__(kSyncThreads, 1) k_plan_replay_persistent(BatchCfg B, SegIndex X, int64_t out_shift) {
+  static_assert(kSyncThreads == kMergeThreads, "bitstreams, tiles and overflow chunks share the CTA");
+  extern __shared__ __align__(1024) unsigned char smem_raw[];
+  __shared__ PlaneSrc src[4];
+  __shared__ unsigned long long s_unit;
+  __shared__ int s_last;
+  PlanCounters* ctr = reinterpret_cast<PlanCounters*>(B.error_out);
+  const SyncCarve cv = sync_carve(smem_raw);
+  SyncShared& S = *cv.S;
+  const uint64_t items = B.item_start[B.n];
+  const uint64_t units = items + B.tile_start[B.n];
+  for (;;) {
+    __syncthreads();  // the previous unit's shared state and s_unit are dead
+    if (threadIdx.x == 0) s_unit = atomicAdd(&ctr->claim, 1ull);
+    __syncthreads();
+    const uint64_t w = s_unit;
+    if (w >= units) break;
+    if (w < items) {
+      const uint32_t t = batch_find(B.item_start, B.n, w);
+      const DecodeCfg& cfg = B.cfgs[t];
+      const uint64_t work = w - B.item_start[t];
+      if (work < 4ull * cfg.ctrl->huf_count) {  // (uniform) the bound counts every item, only the coded ones are queued
+        SegEntry* seg = X.seg + X.base[t] + work * kSyncThreads;
+        if (cfg.box_len) sync_replay_to<true>(cfg, cfg.out + out_shift, S, cv, work, seg);
+        else sync_replay_to<false>(cfg, cfg.out + out_shift, S, cv, work, seg);
+      }
+      __syncthreads();  // every thread's stores of this bitstream are issued
+      if (threadIdx.x == 0) {
+        __threadfence();
+        atomicAdd(&ctr->done, 1ull);
+      }
+      continue;
+    }
+    if (threadIdx.x == 0) {
+      unsigned long long d;
+      for (;;) {
+        asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(d) : "l"(&ctr->done) : "memory");
+        if (d >= items) break;
+        __nanosleep(200);
+      }
+    }
+    __syncthreads();  // every bitstream is done: the plane pool is complete
+    const uint64_t tw = w - items;
+    const uint32_t t = batch_find(B.tile_start, B.n, tw);
+    const DecodeCfg& cfg = B.cfgs[t];
+    const uint32_t tiles_per_chunk = (cfg.chunk + kMergeTile - 1) / kMergeTile;
+    const uint64_t local = tw - B.tile_start[t];
+    if (local >= (uint64_t)cfg.ctrl->regroup_count * tiles_per_chunk) continue;  // (uniform)
+    const uint64_t c = cfg.rlist[local / tiles_per_chunk];
+    const uint32_t tile = (uint32_t)(local % tiles_per_chunk);
+    if (cfg.box_len) regroup_tile_to<true>(cfg, cfg.out + out_shift, c, tile, src);
+    else regroup_tile_to<false>(cfg, cfg.out + out_shift, c, tile, src);
+  }
+  plan_overflow(B, out_shift, *reinterpret_cast<DecodeSmem*>(smem_raw), src);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    s_last = atomicAdd(&ctr->finished, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!s_last) return;
+  // every other CTA is past its last unit and its fence: their error bits are visible, the counters unused
+  __threadfence();
+  uint32_t e = 0;
+  for (uint32_t t = threadIdx.x; t < B.n; t += blockDim.x) e |= *(volatile uint32_t*)&B.cfgs[t].ctrl->error;
+  if (e) atomicOr(&ctr->error, e);
+  if (threadIdx.x == 0) {
+    ctr->claim = 0;
+    ctr->done = 0;
+    ctr->finished = 0;
+  }
+}
+
 // one warp per coded item of every tensor of a batch (flat index over item_start / 4)
 __global__ void __launch_bounds__(kParseWarps * 32) k_parse_tables_batch(BatchCfg B) {
   __shared__ ParseSmem P[kParseWarps];

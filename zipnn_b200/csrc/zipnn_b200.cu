@@ -1092,6 +1092,29 @@ int zipnn_b200_decode_plan_run(const zipnn_b200_decode_plan* plan, void* cuda_st
   return rc ? rc : batch_errors(s.B, st);
 }
 
+int zipnn_b200_decode_plan_run_shifted(const zipnn_b200_decode_plan* plan, int64_t out_shift, int max_ctas, void* cuda_stream) {
+  PlanState s;
+  if (!plan_state(plan, s) || (out_shift & 15)) return ZIPNN_B200_E_ARG;
+  if (s.mode != kSyncReplay) return ZIPNN_B200_E_UNSUPPORTED;
+  static bool attr_done = false;
+  if (!attr_done) {
+    ZB_CUDA(cudaFuncSetAttribute(k_plan_replay_persistent, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPlanReplaySmemBytes));
+    attr_done = true;
+  }
+  static const int nb = [] {
+    int v = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_plan_replay_persistent, kSyncThreads, kPlanReplaySmemBytes) != cudaSuccess || v < 1) v = 1;
+    return v;
+  }();
+  // more CTAs than units (or than the overflow CTAs a tensor may use) would only claim nothing
+  const uint64_t limit = (uint64_t)nb * sm_count_cached();
+  const uint64_t useful = std::max<uint64_t>(std::max<uint64_t>(1, s.grid.items + s.grid.tiles), s.grid.max_ovf);
+  const uint64_t ctas = std::min<uint64_t>(max_ctas <= 0 ? limit : std::min<uint64_t>((uint64_t)max_ctas, limit), useful);
+  k_plan_replay_persistent<<<(unsigned)ctas, kSyncThreads, kPlanReplaySmemBytes, (cudaStream_t)cuda_stream>>>(s.B, s.X, out_shift);
+  ZB_LAUNCHED();
+  return ZIPNN_B200_OK;
+}
+
 int zipnn_b200_decode_plan_status(const zipnn_b200_decode_plan* plan, void* cuda_stream) {
   PlanState s;
   if (!plan_state(plan, s)) return ZIPNN_B200_E_ARG;

@@ -155,7 +155,9 @@ class DecodePlan:
         self.nbytes = {"plan": plan_bytes, "scratch": scratch_bytes, "index": index_bytes.value, "out": out_bytes,
                        "streams": sum(p.stream.numel() for p in parsed), "dense": sum(p.nbytes for p in parsed)}
         self._run = _native.lib().zipnn_b200_decode_plan_run
+        self._run_shifted = _native.lib().zipnn_b200_decode_plan_run_shifted
         self._ref = C.byref(self._plan)
+        self._offs = [(o, p.nbytes, p.dtype, p.shape) for p, o in zip(parsed, offs)]
 
     def run(self) -> list:
         """Enqueue the decode on the current CUDA stream (launches only) and return `.outputs`."""
@@ -163,6 +165,30 @@ class DecodePlan:
         if rc:
             _native.check(rc)
         return self.outputs
+
+    def views(self, out: torch.Tensor) -> list:
+        """The outputs' views of another buffer `out` (same offsets, dtypes and shapes as `.outputs`); ValueError
+        unless `out` is a contiguous CUDA uint8 tensor on the plan's device, 16-byte aligned, of at least
+        `nbytes["out"]` bytes."""
+        if not (isinstance(out, torch.Tensor) and out.is_cuda and out.device == self.device and out.dtype == torch.uint8
+                and out.dim() == 1 and out.is_contiguous()):
+            raise ValueError("run_into takes a flat contiguous CUDA uint8 tensor on the plan's device")
+        if out.numel() < self.nbytes["out"] or out.data_ptr() % _ALIGN:
+            raise ValueError(f"run_into needs {self.nbytes['out']} bytes, {_ALIGN}-byte aligned")
+        return [out[o: o + n].view(dt).reshape(sh) for o, n, dt, sh in self._offs]
+
+    def run_into(self, out: torch.Tensor, max_ctas: int = 0) -> list:
+        """Enqueue the decode on the current CUDA stream as ONE kernel launch of at most `max_ctas` CTAs (0: as many
+        as fit on the device) with the outputs in `out` instead of the create-time buffer, and return their views
+        of `out` (as `views(out)`).  Runs of one plan, and of plans sharing a scratch buffer, must stay ordered on
+        one stream, whichever of `run` and `run_into` enqueues them.  Needs a plan with a segment index (the
+        default)."""
+        views = self.views(out)
+        rc = self._run_shifted(self._ref, out.data_ptr() - self._out.data_ptr(), int(max_ctas),
+                               torch.cuda.current_stream(self.device).cuda_stream)
+        if rc:
+            _native.check(rc)
+        return views
 
     def check(self) -> None:
         """Synchronise the current stream and raise if a run so far found an error."""

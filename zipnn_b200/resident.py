@@ -17,6 +17,9 @@ Rules:
     selected;
   * a parameter shared by several modules (tied weights) is stored once; a parameter also owned by a module outside
     the selection stays dense, as does one whose stream is not smaller than its bytes;
+  * with `prefetch=True` the next module's weights are decoded on a side stream while the current module computes
+    (prefetch.py); to capture a CUDA graph, capture the root module's forward, not a submodule's: the root's
+    forward hook is what joins the side stream;
   * `state_dict()` does not see compressed parameters; `decompress_module(model)` restores them as dense
     `Parameter`s, bit for bit, and removes the hooks and plans.
 
@@ -31,6 +34,7 @@ import traceback
 
 import torch
 
+from . import prefetch as _prefetch
 from .plan import _HEAD, DecodePlan, _Stream
 from .safetensors_io import _FileRange, _cuda_device, compress_groups, file_entries, save_coded
 from .util_safetensors import COMPRESSION_METHOD
@@ -89,6 +93,7 @@ class _Resident:
         self.stream_of = {}   # parameter index -> its stream (a view of `streams`)
         self.streams = []     # the buffers that hold the streams (one per load group)
         self.order = {}       # id(module) -> (module, its parameter names in their original order)
+        self.prefetch = None  # prefetch=True: (Prefetcher, slot 1 buffer, root hook handles)
 
 
 def _pre_hook(plan, names):
@@ -97,6 +102,17 @@ def _pre_hook(plan, names):
             raise RuntimeError(f"{type(mod).__name__} holds compressed weights and runs only under torch.no_grad() or "
                                "torch.inference_mode() (its decoded weights live in a shared buffer)")
         outs = plan.run()
+        for name, k in names:
+            object.__setattr__(mod, name, outs[k])
+    return hook
+
+
+def _pre_hook_prefetch(sched, key, names, views):
+    def hook(mod, args):
+        if torch.is_grad_enabled():
+            raise RuntimeError(f"{type(mod).__name__} holds compressed weights and runs only under torch.no_grad() or "
+                               "torch.inference_mode() (its decoded weights live in a shared buffer)")
+        outs = views[sched.before(key)]
         for name, k in names:
             object.__setattr__(mod, name, outs[k])
     return hook
@@ -160,10 +176,23 @@ def _resident_state(modules, groups, streams: dict, buffers: list, dev) -> tuple
                    "params": len(streams), "modules": len(per_module)}
 
 
-def _commit(module: torch.nn.Module, state: _Resident) -> None:
+def _commit(module: torch.nn.Module, state: _Resident, prefetch: bool = False) -> None:
     """Hooks on, compressed parameters out: after this the model runs from its streams."""
-    for m, plan, local, hooks in state.entries:
-        hooks += [m.register_forward_pre_hook(_pre_hook(plan, local)), m.register_forward_hook(_unbind(local), always_call=True)]
+    sched = None
+    if prefetch and state.entries:
+        plans = [plan for _, plan, _, _ in state.entries]
+        slot1 = torch.empty_like(plans[0]._out)
+        slots = [plans[0]._out, slot1]
+        sched = _prefetch.Prefetcher(_prefetch.CudaOps(plans[0].device, plans, slots, _prefetch.prefetch_ctas()))
+        roots = [module.register_forward_pre_hook(lambda mod, args: sched.root_begin(), prepend=True),
+                 module.register_forward_hook(lambda mod, args, output: sched.root_end(), always_call=True)]
+        state.prefetch = (sched, slot1, roots)
+    for key, (m, plan, local, hooks) in enumerate(state.entries):
+        if sched is None:
+            pre = _pre_hook(plan, local)
+        else:
+            pre = _pre_hook_prefetch(sched, key, local, [plan.views(b) for b in sched.ops.slots])
+        hooks += [m.register_forward_pre_hook(pre), m.register_forward_hook(_unbind(local), always_call=True)]
     # the dense parameters go: nothing here keeps their storage alive
     for _, _, _, owners in state.params.values():
         for o, n in owners:
@@ -172,7 +201,7 @@ def _commit(module: torch.nn.Module, state: _Resident) -> None:
     setattr(module, _ATTR, state)
 
 
-def compress_module(module: torch.nn.Module, modules=None) -> dict:
+def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = False) -> dict:
     """Compress the weights of `modules` (default: every submodule that directly owns bf16 / fp16 / fp32 / fp8
     parameters) into streams kept in HBM, decoded just before each module's forward.  All parameters are compressed
     in one `compress_batch` call and must be on one CUDA device.
@@ -180,7 +209,10 @@ def compress_module(module: torch.nn.Module, modules=None) -> dict:
     -> {"dense_bytes", "stream_bytes", "plan_bytes", "index_bytes", "scratch_bytes", "out_bytes", "params",
         "modules"}: bytes of the parameters now compressed, of their streams, of the plans' memory, of the segment
     index (the recorded segment starts, part of the plans' memory), of the shared plane scratch and of the shared output buffer
-    (the size of the largest module's decoded weights)."""
+    (the size of the largest module's decoded weights).
+
+    prefetch=True: decode each module's weights on a side stream while the module before it computes (prefetch.py),
+    into a second output buffer of the shared one's size; the report gains "prefetch_out_bytes", that buffer's bytes."""
     if getattr(module, _ATTR, None) is not None:
         raise ValueError("compress_module: this module is already compressed")
     modules, groups = select(module, modules)
@@ -197,7 +229,13 @@ def compress_module(module: torch.nn.Module, modules=None) -> dict:
     buf, streams = _pack({i: s for i, (p, s) in enumerate(zip(params, coded)) if s.numel() < p.numel() * p.element_size()}, dev)
     del coded, params
     state, report = _resident_state(modules, groups, streams, [buf], dev)
-    _commit(module, state)
+    _commit(module, state, prefetch)
+    return _with_prefetch(report, state, prefetch)
+
+
+def _with_prefetch(report: dict, state, prefetch: bool) -> dict:
+    if prefetch:
+        report = dict(report, prefetch_out_bytes=state.prefetch[1].numel() if state is not None and state.prefetch else 0)
     return report
 
 
@@ -210,6 +248,13 @@ def decompress_module(module: torch.nn.Module) -> None:
             delattr(module, _ATTR)
             return
         raise ValueError("decompress_module: this module was not compressed by compress_module")
+    if state.prefetch is not None:
+        sched, _, roots = state.prefetch
+        torch.cuda.current_stream(sched.ops.dev).wait_stream(sched.ops.side)
+        for h in roots:
+            h.remove()
+        sched.ops.slots = None   # slot 1 goes with the state
+        state.prefetch = None
     for _, _, _, hooks in state.entries:
         for h in hooks:
             h.remove()
@@ -456,7 +501,7 @@ def _load_device(plan: LoadPlan, dev) -> tuple:
             os.close(f)
 
 
-def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None) -> dict:
+def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None, prefetch: bool = False) -> dict:
     """Load a checkpoint into `module` with the weights of `modules` kept compressed on `device`: the state
     `compress_module` leaves (same selection rules, hooks, plans and report), reached without a dense copy of those
     weights on the GPU.
@@ -491,6 +536,8 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None)
     and the batched decode's workspace; plain entries add one group at a time: its input, its streams' bound and the
     compress workspace.  A model loaded from .znn files never has its compressed weights dense on the device.
 
+    prefetch: as for `compress_module`.
+
     -> the report of `compress_module`."""
     dev = _cuda_device(device)
     if dev is None:
@@ -520,8 +567,8 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None)
     if state is None:
         setattr(module, _ATTR, None)
     else:
-        _commit(module, state)
-    return report
+        _commit(module, state, prefetch)
+    return _with_prefetch(report, state, prefetch)
 
 
 def save_module(module: torch.nn.Module, filename, metadata=None) -> None:
