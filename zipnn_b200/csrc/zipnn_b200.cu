@@ -796,7 +796,7 @@ int slice_pieces(const zipnn_b200_slice_item& it, int i, uint64_t limit, std::ve
   };
   auto run = [&](uint64_t b, uint64_t e, uint64_t off) {  // bytes [b, e) to output offset off (16-byte aligned)
     const uint64_t unit = std::max<uint64_t>(chunk, 16);
-    // units per piece; at least one, also when limit * chunk < 16 (chunks under 8 bytes with a small limit), where
+    // units per piece; at least one, also when limit * chunk < 32 (chunks under 16 bytes with a small limit), where
     // such a piece covers more than `limit` chunks (its tables are sized by its own chunk range)
     const uint64_t per = limit * chunk / unit;
     const uint64_t step = per > 1 ? per - 1 : 1;
