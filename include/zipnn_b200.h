@@ -209,7 +209,13 @@ int zipnn_b200_regroup(const void* d_planes, size_t stride, size_t n, int num_bu
 /* ---- host buffers (the call the reference's Python layer makes) ----------------- */
 /* Same contracts with HOST pointers: the library stages through pinned memory, copies
  * H2D, runs the kernels and copies the result D2H, all inside the call.  `h_out` must hold
- * zipnn_b200_compress_bound(...) bytes (compress) or `orig` bytes (decompress). */
+ * zipnn_b200_compress_bound(...) bytes (compress) or `orig` bytes (decompress).
+ * Every return, errors included, means the call no longer reads `h_in` / `h_body` or writes
+ * `h_out`: the buffers may be freed or reused at once.
+ * Compress: large inputs are compressed slab by slab and may be accepted with a smaller
+ * `out_cap` than the bound (E_CAPACITY when the stream does not fit).  Nothing is written at or
+ * past `out_cap`, but bytes in [*out_len, out_cap) may be overwritten: groups behind the first
+ * are copied out early to where they would sit if every group in front of them stayed raw. */
 int zipnn_b200_compress_host(const void* h_in, size_t n, const void* h_hdr, size_t hdr_len, int num_buf,
                              int bits_mode, int bytes_mode, size_t chunk, float threshold, void* h_out,
                              size_t out_cap, size_t* out_len);

@@ -581,6 +581,8 @@ class DecodePipe:
             from concurrent.futures import ThreadPoolExecutor
             DecodePipe._shared_pool = ThreadPoolExecutor(max_workers=nthreads)
         self._pool = DecodePipe._shared_pool if nthreads > 1 else None
+        # only slabs of the current size: SLAB_BYTES may have changed since they were cached
+        DecodePipe._slab_cache[:] = [sl for sl in DecodePipe._slab_cache if sl.numel() == self.SLAB_BYTES]
         for j in range(stage_buffers):
             if DecodePipe._slab_cache:
                 self._stage[j] = DecodePipe._slab_cache.pop()
