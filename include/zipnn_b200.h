@@ -49,6 +49,7 @@ extern "C" {
 #define ZIPNN_B200_E_CUDA 4       /* a CUDA runtime call failed; see zipnn_b200_last_cuda_error  */
 #define ZIPNN_B200_E_UNSUPPORTED 5 /* valid stream using a table log of 12 (never produced by
                                      the reference encoder, which asks for 11)                   */
+#define ZIPNN_B200_E_INDEX 6      /* a decode plan gather met an id outside [0, rows)            */
 
 int zipnn_b200_version(void);                 /* 0x000200 = 0.2.0 */
 const char* zipnn_b200_strerror(int status);
@@ -196,6 +197,30 @@ int zipnn_b200_decode_plan_index(const zipnn_b200_decode_plan* plan, size_t* ind
  * scratch buffer, must be ordered on one stream, whichever of _run and _run_shifted enqueues them. */
 int zipnn_b200_decode_plan_run_shifted(const zipnn_b200_decode_plan* plan, int64_t out_shift, int max_ctas,
                                        void* cuda_stream);
+/* _gather: rows of item `item` (a whole tensor) looked up by ids on the device, decoding only the chunks they touch.
+ * The item's decoded bytes are rows of row_bytes bytes; for t in [0, n_ids): d_out[t*row_bytes, +row_bytes) =
+ * row d_ids[t] (int32 or int64 ids: id_bytes 4 or 8, aligned to their size).  No alignment is asked of d_out.
+ * Launches only (no copy, memset or synchronisation: capturable in a CUDA graph, replayable with new ids in d_ids):
+ * 1 + 2 * passes launches, passes = ceil(min(n_ids * span, K) / slots), where span = floor((row_bytes + chunk - 2) /
+ * chunk) + 1 (at most K) is the most chunks a row can touch, K the item's chunks, and slots what scratch_bytes holds.
+ * So the count depends on n_ids and the buffers, never on the id values.  n_ids == 0 launches nothing.
+ * An id outside [0, rows) (negative included) reads nothing and its row of d_out is zeroed; it sets ZIPNN_B200_E_INDEX
+ * in the plan's error word, which _status returns (after E_CORRUPT, E_UNSUPPORTED and E_CAPACITY) from then on: the
+ * word is sticky for the plan's life, like every error of its runs.
+ * d_scratch (256-byte aligned, scratch_bytes from _gather_scratch_size for some slot count >= 1; more slots mean
+ * fewer passes) holds nothing between calls: like the plan scratch, calls that share it must be ordered on one
+ * stream, and it may be the scratch of plan runs ordered on that stream.  The plan's own scratch is not used, so a
+ * gather may run next to a _run_shifted of the same plan on another stream.
+ * Host-side rejections launch and write nothing: E_ARG for id_bytes other than 4 or 8, row_bytes 0 or not dividing
+ * the item's bytes, a NULL d_ids, d_out or d_scratch (n_ids > 0), misaligned ids or scratch, a scratch smaller than
+ * one slot, an item index out of range, or a plan whose create failed; E_UNSUPPORTED for an item that is a box, is
+ * empty or was split into several pieces (over 16384 chunks), and for a plan without a segment index.
+ * _gather_scratch_size: the scratch bytes of `slots` slots (capped to K; slots >= 1), same checks. */
+int zipnn_b200_decode_plan_gather_scratch_size(const zipnn_b200_decode_plan* plan, int item, size_t row_bytes,
+                                               size_t slots, size_t* out);
+int zipnn_b200_decode_plan_gather(const zipnn_b200_decode_plan* plan, int item, size_t row_bytes, const void* d_ids,
+                                  size_t n_ids, int id_bytes, void* d_out, void* d_scratch, size_t scratch_bytes,
+                                  void* cuda_stream);
 
 /* ---- stage 1 alone ------------------------------------------------------------ */
 /* d_planes: num_buf planes of `stride` bytes each; plane g receives byte g of every element

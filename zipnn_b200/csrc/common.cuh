@@ -32,7 +32,8 @@ struct ItemDesc {
 enum : uint32_t { kRaw = 0, kRle = 1, kHuf = 2 };
 
 // error bits kept in Ctrl::error
-enum : uint32_t { kErrCorrupt = 1u, kErrUnsupported = 2u, kErrWorkspace = 4u };
+// (kErrIndex: a gather met an id outside [0, rows); raised in a decode plan's error word only)
+enum : uint32_t { kErrCorrupt = 1u, kErrUnsupported = 2u, kErrWorkspace = 4u, kErrIndex = 8u };
 
 // ---- sign-bit rotation (reference data_manipulation_dtype16.c:10-20,145-155;
 //      data_manipulation_dtype32.c:39-49,275-285) ----------------------------------

@@ -366,10 +366,12 @@ struct SegEntry {
 };
 static_assert(sizeof(SegEntry) == 8, "8 bytes per segment: 8 KiB per coded item");
 // W: `out` is the box of cfg (box_store16) instead of the whole tensor.
+// GA (the gather, gather.cuh): every chunk, fused ones included, copies its quarter plane to the chunk's planes at
+// `gplanes` (G planes of cfg.pstride bytes) instead of the pool; the merge is left to the gather.
 static_assert(kSyncThreads * 16 == kBoxStep, "the merge advances the box cursor by kBoxStep");
-template <int G, bool W = false, int M = kSyncDecode>
+template <int G, bool W = false, int M = kSyncDecode, bool GA = false>
 __device__ __forceinline__ void sync_process(const DecodeCfg& cfg, uint8_t* __restrict__ out, SyncShared& S, uint16_t* lut_tab, uint32_t lut_s,
-                                             uint64_t work, SegEntry* segs = nullptr) {
+                                             uint64_t work, SegEntry* segs = nullptr, uint8_t* gplanes = nullptr) {
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const uint64_t K = cfg.K;
   {
@@ -543,7 +545,7 @@ __device__ __forceinline__ void sync_process(const DecodeCfg& cfg, uint8_t* __re
     else sync_emit(b, lut, from, n, S.plane, off);
     __syncthreads();
     // ---- quarter plane -> elements, or -> the chunk's workspace plane ----
-    if (mode == kModeFused) {
+    if (mode == kModeFused && !GA) {
       // fused chunks: the coded plane is the top byte plane, dec_len % 128 == 0, every other plane raw or RLE
       if (tid < G - 1) {
         const ItemDesc t = cfg.items[(uint64_t)tid * K + c];
@@ -601,7 +603,7 @@ __device__ __forceinline__ void sync_process(const DecodeCfg& cfg, uint8_t* __re
         }
       }
     } else {
-      uint8_t* dst = cfg.planes + ((uint64_t)cfg.slot[c] * G + g) * cfg.pstride + out_off;
+      uint8_t* dst = GA ? gplanes + (uint64_t)g * cfg.pstride + out_off : cfg.planes + ((uint64_t)cfg.slot[c] * G + g) * cfg.pstride + out_off;
       if (((uintptr_t)dst & 3) == 0) {
         const uint32_t nw = count >> 2;
         for (uint32_t i = tid; i < nw; i += kSyncThreads) reinterpret_cast<uint32_t*>(dst)[i] = reinterpret_cast<const uint32_t*>(S.plane)[i];

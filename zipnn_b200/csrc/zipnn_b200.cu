@@ -12,12 +12,14 @@
 #include <cstring>
 #include <mutex>
 #include <numeric>
+#include <unordered_map>
 #include <vector>
 
 #include "common.cuh"
 #include "decode.cuh"
 #include "decode_sync.cuh"
 #include "encode.cuh"
+#include "gather.cuh"
 #include "stage1.cuh"
 
 using namespace zb;
@@ -294,6 +296,7 @@ int read_ctrl_error(void* d_ws, cudaStream_t st) {
   if (err & kErrCorrupt) return ZIPNN_B200_E_CORRUPT;
   if (err & kErrUnsupported) return ZIPNN_B200_E_UNSUPPORTED;
   if (err & kErrWorkspace) return ZIPNN_B200_E_CAPACITY;
+  if (err & kErrIndex) return ZIPNN_B200_E_INDEX;
   return ZIPNN_B200_OK;
 }
 
@@ -311,6 +314,7 @@ const char* zipnn_b200_strerror(int s) {
     case ZIPNN_B200_E_CORRUPT: return "corrupt ZipNN stream";
     case ZIPNN_B200_E_CUDA: return "CUDA runtime error";
     case ZIPNN_B200_E_UNSUPPORTED: return "unsupported stream feature (Huffman table log 12)";
+    case ZIPNN_B200_E_INDEX: return "gather id out of range";
     default: return "unknown status";
   }
 }
@@ -925,7 +929,24 @@ struct PlanState {
   SegIndex X;
   uint64_t coded;  // coded items the segment index has room for
   int32_t mode;    // kSyncReplay, or kSyncDecode for a plan without an index
+  uint32_t gen;    // create's number: which host record (g_plan_items) describes this plan's items
 };
+// What a gather needs to know of each item on the host, without reading the device: recorded by create under the
+// plan memory's address (a later create at the same address replaces the record; `gen` tells a stale plan apart).
+struct GatherItem {
+  int piece;          // the item's one piece, -1 when it has none or several (empty, or split) or is a box
+  int G;
+  uint32_t chunk;
+  uint64_t K, orig;
+  uint64_t seg_base;  // the piece's first segment index entry
+};
+struct PlanItems {
+  uint32_t gen;
+  std::vector<GatherItem> items;
+};
+std::mutex g_plan_mu;
+std::unordered_map<uintptr_t, PlanItems> g_plan_items;  // by plan memory address
+uint32_t g_plan_gen = 0;
 static_assert(sizeof(PlanState) <= sizeof(zipnn_b200_decode_plan), "the plan state must fit the ABI's opaque struct");
 size_t plan_piece_meta_bytes(const zipnn_b200_slice_item& it, const SlicePiece& p) {
   return round_up(dec_ws_layout(it.orig, it.num_buf, it.chunk, p.c1 - p.c0).planes_off, 256);
@@ -1071,6 +1092,27 @@ int zipnn_b200_decode_plan_create(const zipnn_b200_slice_item* items, int n, voi
     if (!rc) rc = read_ctrl_error(meta, st);
     if (rc) return rc;
   }
+  {
+    PlanItems rec;
+    rec.items.resize((size_t)n);
+    for (int i = 0; i < n; i++) {
+      const zipnn_b200_slice_item& it = items[i];
+      rec.items[i] = GatherItem{-1, it.num_buf, (uint32_t)it.chunk, num_chunks(it.orig, it.chunk), it.orig, 0};
+    }
+    for (int j = 0; j < np; j++) {
+      const SlicePiece& p = P.pieces[j];
+      const zipnn_b200_slice_item& it = items[p.item];
+      GatherItem& g = rec.items[p.item];
+      const bool whole = p.base == 0 && p.rows == 1 && p.len == it.orig;
+      g.piece = whole && g.piece == -1 ? j : -2;   // (-2: a box or a split item; the pieces of an item are consecutive)
+      g.seg_base = P.seg_base[j];
+    }
+    for (GatherItem& g : rec.items)
+      if (g.piece < 0) g.piece = -1;
+    std::lock_guard<std::mutex> lk(g_plan_mu);
+    s.gen = rec.gen = ++g_plan_gen;
+    g_plan_items[(uintptr_t)d_plan] = std::move(rec);
+  }
   s.magic = kPlanMagic;
   memcpy(plan->opaque, &s, sizeof(s));
   return ZIPNN_B200_OK;
@@ -1119,6 +1161,123 @@ int zipnn_b200_decode_plan_status(const zipnn_b200_decode_plan* plan, void* cuda
   PlanState s;
   if (!plan_state(plan, s)) return ZIPNN_B200_E_ARG;
   return read_ctrl_error(s.B.error_out, (cudaStream_t)cuda_stream);
+}
+
+// ---- gathers: rows of one whole-tensor item, decoded from the chunks the ids touch (gather.cuh) ----------------
+// Scratch: [256 B: touched-chunk count][list u32 K][pos u32 K][inv u32 G*K][slots x G planes of pstride bytes].
+namespace {
+struct GatherLayout {
+  size_t list_off, pos_off, inv_off, planes_off;
+  uint64_t pstride;
+};
+GatherLayout gather_layout(const GatherItem& gi) {
+  GatherLayout L;
+  L.list_off = 256;
+  L.pos_off = round_up(L.list_off + 4 * gi.K, 256);
+  L.inv_off = round_up(L.pos_off + 4 * gi.K, 256);
+  L.planes_off = round_up(L.inv_off + 4 * (size_t)gi.G * gi.K, 256);
+  L.pstride = dec_ws_layout(gi.orig, gi.G, gi.chunk, 0).pstride;
+  return L;
+}
+// Chunks a row of `row_bytes` may touch, wherever it starts: floor((chunk - 1 + row_bytes - 1) / chunk) + 1, at most K.
+uint64_t gather_span(uint64_t row_bytes, uint64_t chunk, uint64_t K) { return std::min<uint64_t>(K, (row_bytes + chunk - 2) / chunk + 1); }
+// The host-side checks shared by both calls.
+int gather_item(const zipnn_b200_decode_plan* plan, int item, size_t row_bytes, PlanState& s, GatherItem& gi) {
+  if (!plan_state(plan, s)) return ZIPNN_B200_E_ARG;
+  {
+    std::lock_guard<std::mutex> lk(g_plan_mu);
+    const auto it = g_plan_items.find((uintptr_t)s.B.error_out);
+    if (it == g_plan_items.end() || it->second.gen != s.gen) return ZIPNN_B200_E_ARG;
+    if (item < 0 || (size_t)item >= it->second.items.size()) return ZIPNN_B200_E_ARG;
+    gi = it->second.items[(size_t)item];
+  }
+  if (gi.piece < 0 || s.mode != kSyncReplay) return ZIPNN_B200_E_UNSUPPORTED;
+  if (row_bytes == 0 || gi.orig % row_bytes) return ZIPNN_B200_E_ARG;
+  return ZIPNN_B200_OK;
+}
+}  // namespace
+
+int zipnn_b200_decode_plan_gather_scratch_size(const zipnn_b200_decode_plan* plan, int item, size_t row_bytes, size_t slots, size_t* out) {
+  if (!out || slots == 0) return ZIPNN_B200_E_ARG;
+  PlanState s;
+  GatherItem gi;
+  const int rc = gather_item(plan, item, row_bytes, s, gi);
+  if (rc) return rc;
+  const GatherLayout L = gather_layout(gi);
+  *out = L.planes_off + std::min<uint64_t>(slots, gi.K) * gi.G * L.pstride;
+  return ZIPNN_B200_OK;
+}
+
+int zipnn_b200_decode_plan_gather(const zipnn_b200_decode_plan* plan, int item, size_t row_bytes, const void* d_ids, size_t n_ids, int id_bytes,
+                                  void* d_out, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (id_bytes != 4 && id_bytes != 8) return ZIPNN_B200_E_ARG;
+  PlanState s;
+  GatherItem gi;
+  {
+    const int rc = gather_item(plan, item, row_bytes, s, gi);
+    if (rc) return rc;
+  }
+  if (n_ids == 0) return ZIPNN_B200_OK;
+  if (!d_ids || !d_out || !d_scratch || ((uintptr_t)d_ids % (uintptr_t)id_bytes) || ((uintptr_t)d_scratch & 255)) return ZIPNN_B200_E_ARG;
+  if (n_ids > (1ull << 40)) return ZIPNN_B200_E_ARG;
+  const GatherLayout L = gather_layout(gi);
+  const uint64_t slot_bytes = (uint64_t)gi.G * L.pstride;
+  const uint64_t slots = std::min<uint64_t>(scratch_bytes < L.planes_off ? 0 : (scratch_bytes - L.planes_off) / slot_bytes, gi.K);
+  if (slots == 0) return ZIPNN_B200_E_ARG;
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  uint8_t* ws = (uint8_t*)d_scratch;
+  GatherCfg g;
+  g.cfg = s.B.cfgs + gi.piece;
+  g.seg = s.X.seg + gi.seg_base;
+  g.error = s.B.error_out;
+  g.ids = d_ids;
+  g.n = n_ids;
+  g.id8 = id_bytes == 8;
+  g.G = gi.G;
+  g.K = gi.K;
+  g.orig = gi.orig;
+  g.rows = gi.orig / row_bytes;
+  g.row_bytes = row_bytes;
+  g.span = gather_span(row_bytes, gi.chunk, gi.K);
+  g.chunk = gi.chunk;
+  g.slots = (uint32_t)slots;
+  g.out = (uint8_t*)d_out;
+  g.count = (uint32_t*)ws;
+  g.list = (uint32_t*)(ws + L.list_off);
+  g.pos = (uint32_t*)(ws + L.pos_off);
+  g.inv = (uint32_t*)(ws + L.inv_off);
+  g.planes = ws + L.planes_off;
+  g.pstride = L.pstride;
+  // passes: the distinct chunks are at most min(n * span, K), `slots` per pass (a bound of n alone, not of the ids)
+  const uint64_t most = n_ids > gi.K / g.span ? gi.K : std::min<uint64_t>(gi.K, n_ids * g.span);
+  const uint64_t passes = (most + slots - 1) / slots;
+  static bool attr_done = false;
+  if (!attr_done) {
+    ZB_CUDA(cudaFuncSetAttribute(k_gather_decode, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPlanReplaySmemBytes));
+    attr_done = true;
+  }
+  static const int nb = [] {
+    int v = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_gather_decode, kSyncThreads, kPlanReplaySmemBytes) != cudaSuccess || v < 1) v = 1;
+    return v;
+  }();
+  const int sms = sm_count_cached();
+  const unsigned inv_blocks = (unsigned)std::max<uint64_t>(1, ((uint64_t)gi.G * gi.K + kGatherIndexThreads - 1) / kGatherIndexThreads);
+  k_gather_index<<<1 + inv_blocks, kGatherIndexThreads, 0, st>>>(g);
+  ZB_LAUNCHED();
+  const unsigned dec_blocks = (unsigned)std::min<uint64_t>(slots * 4 * gi.G, (uint64_t)nb * sms);
+  const uint64_t units = n_ids * ((row_bytes + 15) / 16 + 1);
+  const unsigned row_blocks = (unsigned)std::min<uint64_t>((units + 255) / 256, (uint64_t)sms * 16);
+  for (uint64_t p = 0; p < passes; p++) {
+    k_gather_decode<<<dec_blocks, kSyncThreads, kPlanReplaySmemBytes, st>>>(g, (uint32_t)p);
+    ZB_LAUNCHED();
+    dispatch_G(gi.G, [&](auto gg) -> int {
+      k_gather_rows<decltype(gg)::value><<<row_blocks, 256, 0, st>>>(g, (uint32_t)p);
+      return 0;
+    });
+    ZB_LAUNCHED();
+  }
+  return ZIPNN_B200_OK;
 }
 
 int zipnn_b200_split(const void* d_in, size_t n, int num_buf, int bits_mode, void* d_planes, size_t stride,

@@ -25,6 +25,7 @@ from .zipnn import HEADER_LEN, HUF_MAX_BLOCK, ZipNN, _cuda_stream_handle
 
 _HEAD = HEADER_LEN + 1 + 9 * 255   # the 32-byte header and the longest packed shape (as decompress peeks)
 _ALIGN = 16
+GATHER_SLOTS = 64   # chunk slots of gather's default scratch: 16 MiB for 256 KiB chunks
 
 
 def _round(n: int, a: int) -> int:
@@ -103,6 +104,8 @@ def _sizes(parsed) -> tuple:
 def _raise_status(rc: int) -> None:
     if rc == _native.E_CORRUPT:
         raise _native.ZipNNNativeError(rc, "Thread processing failed: corrupt ZipNN stream")
+    if rc == _native.E_INDEX:
+        raise IndexError("zipnn_b200: a gather of this plan met an id outside [0, rows) (its rows were zeroed)")
     _native.check(rc)
 
 
@@ -156,11 +159,15 @@ class DecodePlan:
                        "streams": sum(p.stream.numel() for p in parsed), "dense": sum(p.nbytes for p in parsed)}
         self._run = _native.lib().zipnn_b200_decode_plan_run
         self._run_shifted = _native.lib().zipnn_b200_decode_plan_run_shifted
+        self._gather = _native.lib().zipnn_b200_decode_plan_gather
         self._ref = C.byref(self._plan)
         self._offs = [(o, p.nbytes, p.dtype, p.shape) for p, o in zip(parsed, offs)]
+        self._gather_scratch = None   # gather's default scratch, grown on demand
 
     def run(self) -> list:
         """Enqueue the decode on the current CUDA stream (launches only) and return `.outputs`."""
+        if self._out is None:
+            raise RuntimeError("DecodePlan: the output buffer was released (release_out); only gather runs")
         rc = self._run(self._ref, torch.cuda.current_stream(self.device).cuda_stream)
         if rc:
             _native.check(rc)
@@ -170,6 +177,8 @@ class DecodePlan:
         """The outputs' views of another buffer `out` (same offsets, dtypes and shapes as `.outputs`); ValueError
         unless `out` is a contiguous CUDA uint8 tensor on the plan's device, 16-byte aligned, of at least
         `nbytes["out"]` bytes."""
+        if self._out is None:
+            raise RuntimeError("DecodePlan: the output buffer was released (release_out); only gather runs")
         if not (isinstance(out, torch.Tensor) and out.is_cuda and out.device == self.device and out.dtype == torch.uint8
                 and out.dim() == 1 and out.is_contiguous()):
             raise ValueError("run_into takes a flat contiguous CUDA uint8 tensor on the plan's device")
@@ -189,6 +198,66 @@ class DecodePlan:
         if rc:
             _native.check(rc)
         return views
+
+    def release_out(self) -> None:
+        """Drop the plan's reference to its output buffer (the one create decoded into), for a plan that only
+        gathers: `run`, `run_into` and `views` raise RuntimeError from then on, `outputs` is None."""
+        self._out, self.outputs = None, None
+
+    def _gather_row(self, k: int) -> tuple:
+        if not 0 <= k < len(self._offs):
+            raise IndexError(f"DecodePlan has {len(self._offs)} outputs, not {k + 1}")
+        _, n, dt, sh = self._offs[k]
+        if len(sh) == 0 or sh[0] == 0:
+            raise ValueError("gather takes rows along dim 0 of a non-empty output with at least one dimension")
+        return n // sh[0], dt, sh
+
+    def gather_scratch_bytes(self, k: int, slots: int) -> int:
+        """Bytes of a gather scratch for output `k` with `slots` chunk slots (capped to the output's chunks): each
+        gather pass decodes up to `slots` chunks, so more slots mean fewer launches and more memory."""
+        row, _, _ = self._gather_row(k)
+        out = C.c_size_t(0)
+        _native.check(_native.lib().zipnn_b200_decode_plan_gather_scratch_size(self._ref, k, row, int(slots), C.byref(out)))
+        return out.value
+
+    def gather(self, k: int, ids: torch.Tensor, out: torch.Tensor = None, scratch: torch.Tensor = None) -> torch.Tensor:
+        """Rows of output `k` along dim 0, as `outputs[k][ids]` would give them, decoded from the chunks the ids
+        touch and no others (zipnn_b200_decode_plan_gather): enqueued on the current CUDA stream, launches only,
+        the ids never read on the host, so it can be captured in a CUDA graph and replayed with new ids.
+
+        ids:     CUDA int32 or int64 tensor of any shape on the plan's device.
+        out:     optional contiguous tensor of shape `ids.shape + outputs[k].shape[1:]` and the output's dtype.
+        scratch: optional 256-byte aligned CUDA uint8 buffer of at least `gather_scratch_bytes(k, 1)` bytes; its slot
+                 count sets the passes.  It holds nothing between calls: calls (and plan runs) that share it must
+                 be ordered on one stream.  Default: a buffer of GATHER_SLOTS slots kept by the plan.
+        -> out.  An id outside [0, rows) gets a zero row and makes `check()` raise IndexError (from then on: the
+        plan's error word is sticky).  Works without the plan's output buffer (`release_out`)."""
+        row, dt, sh = self._gather_row(k)
+        if not (isinstance(ids, torch.Tensor) and ids.is_cuda and ids.device == self.device and ids.dtype in (torch.int32, torch.int64)):
+            raise ValueError("gather takes CUDA int32 or int64 ids on the plan's device")
+        ids_c = ids.contiguous()
+        shape = tuple(ids.shape) + tuple(sh[1:])
+        if out is None:
+            out = torch.empty(shape, dtype=dt, device=self.device)
+        elif not (isinstance(out, torch.Tensor) and out.is_cuda and out.device == self.device and out.dtype == dt
+                  and tuple(out.shape) == shape and out.is_contiguous()):
+            raise ValueError(f"gather's out must be a contiguous {dt} CUDA tensor of shape {shape} on the plan's device")
+        n = ids_c.numel()
+        if n == 0:
+            return out
+        if scratch is None:
+            need = self.gather_scratch_bytes(k, GATHER_SLOTS)
+            if self._gather_scratch is None or self._gather_scratch.numel() < need:
+                self._gather_scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
+            scratch = self._gather_scratch
+        elif not (isinstance(scratch, torch.Tensor) and scratch.is_cuda and scratch.device == self.device
+                  and scratch.dtype == torch.uint8 and scratch.is_contiguous()):
+            raise ValueError("gather's scratch must be a contiguous CUDA uint8 tensor on the plan's device")
+        rc = self._gather(self._ref, k, row, ids_c.data_ptr(), n, ids_c.element_size(), out.data_ptr(), scratch.data_ptr(),
+                          scratch.numel(), torch.cuda.current_stream(self.device).cuda_stream)
+        if rc:
+            _native.check(rc)
+        return out
 
     def check(self) -> None:
         """Synchronise the current stream and raise if a run so far found an error."""

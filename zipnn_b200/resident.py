@@ -20,6 +20,9 @@ Rules:
   * with `prefetch=True` the next module's weights are decoded on a side stream while the current module computes
     (prefetch.py); to capture a CUDA graph, capture the root module's forward, not a submodule's: the root's
     forward hook is what joins the side stream;
+  * with `gather=True` a selected `torch.nn.Embedding` (its class's own forward, no max_norm) looks its rows up
+    straight from the stream (`DecodePlan.gather`: only the chunks the ids touch are decoded) and is never decoded
+    whole; its output is an ordinary tensor the caller owns;
   * `state_dict()` does not see compressed parameters; `decompress_module(model)` restores them as dense
     `Parameter`s, bit for bit, and removes the hooks and plans.
 
@@ -94,6 +97,10 @@ class _Resident:
         self.streams = []     # the buffers that hold the streams (one per load group)
         self.order = {}       # id(module) -> (module, its parameter names in their original order)
         self.prefetch = None  # prefetch=True: (Prefetcher, slot 1 buffer, root hook handles)
+        self.gathers = []     # gather=True: (embedding module, plan, index into the plan's outputs, own plan?)
+        self.scratch = None   # the plans' shared scratch
+        self.gather_scratch = None  # the gathers' scratch: the plans' one, or a buffer of its own (prefetch)
+        self.gather_plan_bytes = 0  # memory of the plans that only serve gathers
 
 
 def _pre_hook(plan, names):
@@ -118,6 +125,22 @@ def _pre_hook_prefetch(sched, key, names, views):
     return hook
 
 
+def gathers(module: torch.nn.Module) -> bool:
+    """Does `gather=True` look `module` up by a gather instead of decoding its weight whole?  A torch.nn.Embedding
+    (or subclass) whose class does not override forward and that has no max_norm (which renormalises the weight)."""
+    return isinstance(module, torch.nn.Embedding) and type(module).forward is torch.nn.Embedding.forward and module.max_norm is None
+
+
+def _gather_forward(mod, state, plan, k):
+    # padding_idx, scale_grad_by_freq and sparse only shape gradients, which a compressed module never has
+    def forward(input):
+        if torch.is_grad_enabled():
+            raise RuntimeError(f"{type(mod).__name__} holds compressed weights and runs only under torch.no_grad() or "
+                               "torch.inference_mode()")
+        return plan.gather(k, input, scratch=state.gather_scratch)
+    return forward
+
+
 def _unbind(names):
     def hook(mod, args, output):
         for name, _ in names:
@@ -127,6 +150,20 @@ def _unbind(names):
 
 _EMPTY_REPORT = {"dense_bytes": 0, "stream_bytes": 0, "plan_bytes": 0, "index_bytes": 0, "scratch_bytes": 0, "out_bytes": 0,
                  "params": 0, "modules": 0}
+
+
+def split_gathers(per_module, gather: bool) -> tuple:
+    """[(module, [(name, stream index)])] -> (modules decoded whole, [(embedding, stream index)] looked up by gathers,
+    the gathers' stream indexes no whole-decoded module holds: each needs a plan of its own)."""
+    whole, looked = [], []
+    for m, names in per_module:
+        if gather and gathers(m) and [n for n, _ in names] == ["weight"]:
+            looked.append((m, names[0][1]))
+        else:
+            whole.append((m, names))
+    held = {i for _, names in whole for _, i in names}
+    own = list(dict.fromkeys(i for _, i in looked if i not in held))
+    return whole, looked, own
 
 
 def _pack(streams: dict, dev) -> tuple:
@@ -144,27 +181,50 @@ def _pack(streams: dict, dev) -> tuple:
     return buf, views
 
 
-def _resident_state(modules, groups, streams: dict, buffers: list, dev) -> tuple:
+def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: bool = False) -> tuple:
     """The back half of compress_module and load_module: streams {group index: CUDA stream} -> per selected module
     one DecodePlan over its parameters' streams, all sharing one output and one scratch buffer.  Raises like
-    `decompress` on a corrupt stream; nothing outside is touched until `_commit`.  -> (_Resident, report)."""
+    `decompress` on a corrupt stream; nothing outside is touched until `_commit`.  -> (_Resident, report).
+
+    gather=True: embeddings (`gathers`) get no output space.  One whose weight a whole-decoded module also holds (a
+    tied lm_head) gathers through that module's plan; any other gets a plan of its own, created first, into a
+    transient buffer that is freed before the shared output buffer exists (so the peak stays that of gather=False)."""
     where = {id(groups[i][0]): i for i in streams}
     per_module = []
     for m in modules:
         names = [(n, where[id(p)]) for n, p in _own_params(m) if id(p) in where]
         if names:
             per_module.append((m, names))
-    sizes = [DecodePlan.sizes([streams[i] for _, i in names]) for _, names in per_module]
-    out = torch.empty(max([s[0] for s in sizes] + [1]), dtype=torch.uint8, device=dev)
-    scratch = torch.empty(max([s[1] for s in sizes] + [1]), dtype=torch.uint8, device=dev)
+    whole, looked, own = split_gathers(per_module, gather)
+    sizes = [DecodePlan.sizes([streams[i] for _, i in names]) for _, names in whole]
+    own_sizes = [DecodePlan.sizes([streams[i]]) for i in own]
+    out = None if own else torch.empty(max([s[0] for s in sizes] + [1]), dtype=torch.uint8, device=dev)
+    scratch = torch.empty(max([s[1] for s in sizes + own_sizes] + [1]), dtype=torch.uint8, device=dev)
     state = _Resident()
     state.streams = buffers
+    state.scratch = scratch
     plan_bytes = index_bytes = 0
-    for m, names in per_module:
+    by_stream = {}   # stream index -> (plan, output index) a gather reads
+    for i, (out_bytes, _) in zip(own, own_sizes):
+        transient = torch.empty(max(out_bytes, 1), dtype=torch.uint8, device=dev)
+        plan = DecodePlan([streams[i]], out=transient, scratch=scratch)
+        plan.release_out()
+        del transient
+        by_stream[i] = (plan, 0)
+        state.gather_plan_bytes += plan.nbytes["plan"]
+        index_bytes += plan.nbytes["index"]
+    if out is None:
+        out = torch.empty(max([s[0] for s in sizes] + [1]), dtype=torch.uint8, device=dev)
+    for m, names in whole:
         plan = DecodePlan([streams[i] for _, i in names], out=out, scratch=scratch)
         plan_bytes += plan.nbytes["plan"]
         index_bytes += plan.nbytes["index"]
         state.entries.append((m, plan, [(n, k) for k, (n, _) in enumerate(names)], []))
+        for k, (_, i) in enumerate(names):
+            by_stream.setdefault(i, (plan, k))
+    for m, i in looked:
+        plan, k = by_stream[i]
+        state.gathers.append((m, plan, k, i in own))
     dense = 0
     for i in streams:
         p, owners = groups[i]
@@ -187,6 +247,16 @@ def _commit(module: torch.nn.Module, state: _Resident, prefetch: bool = False) -
         roots = [module.register_forward_pre_hook(lambda mod, args: sched.root_begin(), prepend=True),
                  module.register_forward_hook(lambda mod, args, output: sched.root_end(), always_call=True)]
         state.prefetch = (sched, slot1, roots)
+    if state.gathers:
+        # the plans' scratch, whose runs share the forward's stream; with prefetch those runs move to the side stream,
+        # so the gathers get a buffer of their own.  One slot at least.
+        need = max(plan.gather_scratch_bytes(k, 1) for _, plan, k, _ in state.gathers)
+        if prefetch or need > state.scratch.numel():
+            state.gather_scratch = torch.empty(max(need, state.scratch.numel()), dtype=torch.uint8, device=state.scratch.device)
+        else:
+            state.gather_scratch = state.scratch
+        for m, plan, k, _ in state.gathers:
+            m.__dict__["forward"] = _gather_forward(m, state, plan, k)
     for key, (m, plan, local, hooks) in enumerate(state.entries):
         if sched is None:
             pre = _pre_hook(plan, local)
@@ -201,7 +271,7 @@ def _commit(module: torch.nn.Module, state: _Resident, prefetch: bool = False) -
     setattr(module, _ATTR, state)
 
 
-def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = False) -> dict:
+def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = False, gather: bool = False) -> dict:
     """Compress the weights of `modules` (default: every submodule that directly owns bf16 / fp16 / fp32 / fp8
     parameters) into streams kept in HBM, decoded just before each module's forward.  All parameters are compressed
     in one `compress_batch` call and must be on one CUDA device.
@@ -212,7 +282,15 @@ def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = Fals
     (the size of the largest module's decoded weights).
 
     prefetch=True: decode each module's weights on a side stream while the module before it computes (prefetch.py),
-    into a second output buffer of the shared one's size; the report gains "prefetch_out_bytes", that buffer's bytes."""
+    into a second output buffer of the shared one's size; the report gains "prefetch_out_bytes", that buffer's bytes.
+
+    gather=True: a selected embedding whose weight is compressed (`gathers`) runs its forward as
+    `DecodePlan.gather` and is never decoded whole.  A tied lm_head keeps its whole decode and the embedding gathers
+    through the same plan; an untied one gets a plan of its own.  Embeddings take no room in the shared output buffer
+    ("out_bytes": the largest module decoded whole), and their plans are not in "plan_bytes" (their indexes are in
+    "index_bytes").  The gathers use the plans' scratch (they run on the forward's stream, as the plans do), or with
+    prefetch=True a buffer of its own.  The report gains "gather_modules" and "gather_bytes": memory that exists only
+    for gathers, i.e. the plans of their own plus a scratch of their own."""
     if getattr(module, _ATTR, None) is not None:
         raise ValueError("compress_module: this module is already compressed")
     modules, groups = select(module, modules)
@@ -228,14 +306,18 @@ def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = Fals
     # the streams move into one tight buffer; the batch's output buffer (sized by the bound) is dropped
     buf, streams = _pack({i: s for i, (p, s) in enumerate(zip(params, coded)) if s.numel() < p.numel() * p.element_size()}, dev)
     del coded, params
-    state, report = _resident_state(modules, groups, streams, [buf], dev)
+    state, report = _resident_state(modules, groups, streams, [buf], dev, gather)
     _commit(module, state, prefetch)
-    return _with_prefetch(report, state, prefetch)
+    return _with_prefetch(report, state, prefetch, gather)
 
 
-def _with_prefetch(report: dict, state, prefetch: bool) -> dict:
+def _with_prefetch(report: dict, state, prefetch: bool, gather: bool = False) -> dict:
     if prefetch:
         report = dict(report, prefetch_out_bytes=state.prefetch[1].numel() if state is not None and state.prefetch else 0)
+    if gather:
+        own = state is not None and state.gather_scratch is not None and state.gather_scratch is not state.scratch
+        report = dict(report, gather_modules=len(state.gathers) if state is not None else 0,
+                      gather_bytes=(state.gather_plan_bytes + (state.gather_scratch.numel() if own else 0)) if state is not None else 0)
     return report
 
 
@@ -258,6 +340,8 @@ def decompress_module(module: torch.nn.Module) -> None:
     for _, _, _, hooks in state.entries:
         for h in hooks:
             h.remove()
+    for m, _, _, _ in state.gathers:
+        m.__dict__.pop("forward", None)
     # each module's plan decodes into the shared buffer once more; its parameters are copied out of it, so the
     # model needs its dense size plus that buffer, not twice its dense size
     dense = {}
@@ -269,6 +353,11 @@ def decompress_module(module: torch.nn.Module) -> None:
                 i = idx_of[id(s_)]
                 if i not in dense:
                     dense[i] = outs[k].clone()
+        for m, plan, k, _ in state.gathers:   # an embedding of its own plan: every row, gathered
+            i = idx_of[id(plan._streams[k])]
+            if i not in dense:
+                rows = state.params[i][2][0]
+                dense[i] = plan.gather(k, torch.arange(rows, device=plan.device), scratch=state.gather_scratch)
     for i, t in dense.items():
         requires_grad, _, _, owners = state.params[i]
         p = torch.nn.Parameter(t, requires_grad=requires_grad)
@@ -283,6 +372,7 @@ def decompress_module(module: torch.nn.Module) -> None:
         params.clear()
         params.update(reordered)
     state.entries.clear()
+    state.gathers.clear()
     delattr(module, _ATTR)
 
 
@@ -421,7 +511,7 @@ def plan_load(module: torch.nn.Module, filenames, modules=None) -> LoadPlan:
     return plan
 
 
-def _load_device(plan: LoadPlan, dev) -> tuple:
+def _load_device(plan: LoadPlan, dev, gather: bool = False) -> tuple:
     """Every device step of load_module; the module is not touched.  -> (_Resident or None, report, dense tensors of
     plan.dense, {group index: dense tensor} of plain entries that did not compress, moved buffers of plan.moves)."""
     pipe = DecodePipe(dev)
@@ -491,7 +581,7 @@ def _load_device(plan: LoadPlan, dev) -> tuple:
             pipe.finish()
             moved = [m._buffers[n].to(dev) for m, n in plan.moves]
             if plan.groups:
-                state, report = _resident_state(plan.modules, plan.groups, dict(sorted(streams.items())), buffers, dev)
+                state, report = _resident_state(plan.modules, plan.groups, dict(sorted(streams.items())), buffers, dev, gather)
             else:
                 state, report = None, dict(_EMPTY_REPORT)
         return state, report, dense, stayed, moved
@@ -501,7 +591,8 @@ def _load_device(plan: LoadPlan, dev) -> tuple:
             os.close(f)
 
 
-def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None, prefetch: bool = False) -> dict:
+def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None, prefetch: bool = False,
+                gather: bool = False) -> dict:
     """Load a checkpoint into `module` with the weights of `modules` kept compressed on `device`: the state
     `compress_module` leaves (same selection rules, hooks, plans and report), reached without a dense copy of those
     weights on the GPU.
@@ -536,7 +627,7 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None,
     and the batched decode's workspace; plain entries add one group at a time: its input, its streams' bound and the
     compress workspace.  A model loaded from .znn files never has its compressed weights dense on the device.
 
-    prefetch: as for `compress_module`.
+    prefetch, gather: as for `compress_module`.
 
     -> the report of `compress_module`."""
     dev = _cuda_device(device)
@@ -546,7 +637,7 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None,
         dev = torch.device("cuda", torch.cuda.current_device())
     plan = plan_load(module, filenames, modules)
     try:
-        state, report, dense, stayed, moved = _load_device(plan, dev)
+        state, report, dense, stayed, moved = _load_device(plan, dev, gather)
     except BaseException as e:
         traceback.clear_frames(e.__traceback__)   # the frames' locals would keep the call's device memory alive
         raise
@@ -568,7 +659,7 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None,
         setattr(module, _ATTR, None)
     else:
         _commit(module, state, prefetch)
-    return _with_prefetch(report, state, prefetch)
+    return _with_prefetch(report, state, prefetch, gather)
 
 
 def save_module(module: torch.nn.Module, filename, metadata=None) -> None:
