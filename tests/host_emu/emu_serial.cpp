@@ -2,8 +2,16 @@
 // TEST ONLY: lets `pytest -m "not gpu"` fuzz the single-thread device routines
 // (tree build, table header encode/decode) against the oracle without a GPU.
 // It is not part of the product library and is never loaded by zipnn_b200.
+#include <cstdint>
+
+// Count every branch of the table build a crafted histogram reaches (huf_serial.cuh, enum HufTrace).
+static thread_local uint32_t g_trace[64];
+#define ZB_HUF_TRACE(id) (++g_trace[(id)])
+
 #include "../../zipnn_b200/csrc/huf_serial.cuh"
 #include <cstring>
+
+static_assert(zb::kTrCount <= 64, "trace counters");
 
 extern "C" {
 
@@ -21,6 +29,18 @@ int emu_table_from_counts(const uint32_t* count, uint32_t n, uint8_t* nb, uint16
   if (h > 0) memcpy(hdr, T.hdr, (size_t)h);
   return h;
 }
+
+// The branches reached since the last call (trace[kTrCount]), then zeroed.  Returns kTrCount.
+int emu_trace_take(uint32_t* trace) {
+  for (int i = 0; i < zb::kTrCount; i++) {
+    trace[i] = g_trace[i];
+    g_trace[i] = 0;
+  }
+  return zb::kTrCount;
+}
+
+// zb::huf_early_out: 0 = raw, 1 = one symbol, 2 = build the table.
+int emu_early_out(uint32_t largest, uint32_t plen) { return zb::huf_early_out(largest, plen); }
 
 // zb::huf_block_decision: 0 = raw, 1 = RLE, else the coded block's size.
 uint32_t emu_block_decision(int rle, const uint32_t* bits, int hsize, uint32_t plen, uint64_t cap, double thr) {

@@ -252,21 +252,15 @@ __device__ void warp_block_decision(TableWarp& S, const uint16_t* __restrict__ h
   }
   __syncwarp();
   uint32_t stored = 0;  // huf_block_decision: 0 = raw, 1 = RLE, else the coded block's size
-  bool huf = false;
-  if (plen == 0 || plen > (uint32_t)kHufBlockMax) {
-    // empty plane, or HUF_compress rejects > 128 KiB (huf_compress.c:658) -> raw
-  } else if (largest == plen) {
+  const int early = huf_early_out(largest, plen);
+  if (early == 1) {
     stored = huf_block_decision(true, nullptr, 0, plen, cap, thr);  // RLE block of 1 byte (huf_compress.c:673)
     if (stored && lane == 0) {
       save->hdr[0] = (uint8_t)max_sym;
       save->hsize = 0;
     }
-  } else if (largest <= (plen >> 7) + 4) {
-    // heuristic "probably not compressible" (huf_compress.c:674)
-  } else {
-    huf = true;
   }
-  if (huf) {
+  if (early == 2) {
     // ---- order the present symbols: count descending, symbol ascending ----
     TreeScratch& T = S.tree;
     uint8_t* nz = S.nzsym;

@@ -22,9 +22,39 @@
 #define ZB_HD
 #endif
 
+// ZB_HUF_TRACE(id): a hook at each branch of the table build that real weights rarely take.  Empty here, so the
+// library is compiled as if it were not there; the host test shim (tests/host_emu) defines it as a counter to show
+// that its crafted histograms reach every branch.
+#ifndef ZB_HUF_TRACE
+#define ZB_HUF_TRACE(id) ((void)0)
+#endif
+
 namespace zb {
 
-constexpr int kHufLogMax = 12;      // largest table log the format allows
+// Branch ids for ZB_HUF_TRACE.
+enum HufTrace {
+  kTrLimit = 0,          // huf_limit_depth: the tree is deeper than the limit
+  kTrLimitBelow11,       //   ... and the limit is below 11 (a small plane)
+  kTrRepayBreakTotal,    //   repay loop: the rank above costs at most twice the rank below (highTotal <= lowTotal)
+  kTrRepayBreakNoLow,    //   repay loop: the rank below is empty
+  kTrRepayStepUp,        //   no symbol left in the chosen rank: step up to the next non-empty one
+  kTrRepayLargest,       //   the promoted symbol was the largest one: its rank is reset
+  kTrRepayRankEmptied,   //   the chosen rank ran out of symbols
+  kTrOvershootNoRank1,   //   overshoot fix-up with no symbol one bit under the limit
+  kTrOvershootRank1,     //   overshoot fix-up with one
+  kTrHufLogFloor,        // fse_pick_log for the Huffman table: the floor of the alphabet size raised the log
+  kTrFseLogFloor,        // fse_pick_log for the weight tANS: same
+  kTrNormalizeSlow,      // fse_normalize fell back to fse_normalize_slow
+  kTrPackDistinct,       // huf_pack_weights: every weight at most once -> 0
+  kTrPackRle,            // huf_pack_weights: all weights equal -> 1
+  kTrTableFse,           // huf_write_table: tANS-coded weights
+  kTrTableNibbleLost,    //   raw nibbles although tANS produced a header (it did not pay: hSize >= maxSymbolValue / 2)
+  kTrTableNibble,        //   raw nibbles
+  kTrTableRaw,           //   no description: the block is stored raw
+  kTrCount
+};
+
+constexpr int kHufLogMax = 12;     // largest table log the format allows
 constexpr int kHufLogDefault = 11;  // what HUF_compress() asks for
 constexpr int kHufBlockMax = 128 * 1024;
 
@@ -78,7 +108,10 @@ ZB_HD inline int fse_pick_log(int want, uint32_t n, uint32_t max_sym, int minus)
   int lg = want;
   int need = fse_min_log(n, max_sym);
   if (by_src < lg) lg = by_src;
-  if (need > lg) lg = need;
+  if (need > lg) {
+    ZB_HUF_TRACE(minus == 1 ? kTrHufLogFloor : kTrFseLogFloor);
+    lg = need;
+  }
   if (lg < 5) lg = 5;
   if (lg > 12) lg = 12;
   return lg;
@@ -197,7 +230,10 @@ ZB_HD inline int fse_normalize(int16_t* norm, int lg, const uint32_t* count, uin
       left -= p;
     }
   }
-  if (-left >= (norm[largest] >> 1)) return fse_normalize_slow(norm, lg, count, total, max_sym);
+  if (-left >= (norm[largest] >> 1)) {
+    ZB_HUF_TRACE(kTrNormalizeSlow);
+    return fse_normalize_slow(norm, lg, count, total, max_sym);
+  }
   norm[largest] = (int16_t)(norm[largest] + left);
   return 0;
 }
@@ -338,8 +374,14 @@ ZB_HD inline int huf_pack_weights(uint8_t* dst, const uint8_t* w, int n, FseEnc&
   uint32_t top = 0;
   for (int s = 0; s <= max_w; s++)
     if (E.count[s] > top) top = E.count[s];
-  if (top == (uint32_t)n) return 1;
-  if (top == 1) return 0;
+  if (top == (uint32_t)n) {
+    ZB_HUF_TRACE(kTrPackRle);
+    return 1;
+  }
+  if (top == 1) {
+    ZB_HUF_TRACE(kTrPackDistinct);
+    return 0;
+  }
   const int lg = fse_pick_log(6, (uint32_t)n, (uint32_t)max_w, 2);
   if (fse_normalize(E.norm, lg, E.count, (uint32_t)n, max_w) != 0) return -1;
   int h = fse_write_ncount(dst, E.norm, max_w, lg);
@@ -385,6 +427,8 @@ struct TreeScratch {
 ZB_HD inline int huf_limit_depth(TreeScratch& T, int last, int max_nb) {
   const int deepest = T.depth[last];
   if (deepest <= max_nb) return deepest;
+  ZB_HUF_TRACE(kTrLimit);
+  if (max_nb < kHufLogDefault) ZB_HUF_TRACE(kTrLimitBelow11);
   const uint32_t kNone = 0xF0F0F0F0u;
   int debt = 0;
   const int base = 1 << (deepest - max_nb);
@@ -412,28 +456,43 @@ ZB_HD inline int huf_limit_depth(TreeScratch& T, int last, int max_nb) {
     for (; dec > 1; dec--) {
       uint32_t hi = rank_last[dec], lo = rank_last[dec - 1];
       if (hi == kNone) continue;
-      if (lo == kNone) break;
-      if (T.cnt[hi] <= 2 * T.cnt[lo]) break;
+      if (lo == kNone) {
+        ZB_HUF_TRACE(kTrRepayBreakNoLow);
+        break;
+      }
+      if (T.cnt[hi] <= 2 * T.cnt[lo]) {
+        ZB_HUF_TRACE(kTrRepayBreakTotal);
+        break;
+      }
     }
-    while (dec <= kHufLogMax && rank_last[dec] == kNone) dec++;
+    while (dec <= kHufLogMax && rank_last[dec] == kNone) {
+      ZB_HUF_TRACE(kTrRepayStepUp);
+      dec++;
+    }
     debt -= 1 << (dec - 1);
     if (rank_last[dec - 1] == kNone) rank_last[dec - 1] = rank_last[dec];
     T.depth[rank_last[dec]]++;
     if (rank_last[dec] == 0) {
+      ZB_HUF_TRACE(kTrRepayLargest);
       rank_last[dec] = kNone;
     } else {
       rank_last[dec]--;
-      if (T.depth[rank_last[dec]] != max_nb - dec) rank_last[dec] = kNone;
+      if (T.depth[rank_last[dec]] != max_nb - dec) {
+        ZB_HUF_TRACE(kTrRepayRankEmptied);
+        rank_last[dec] = kNone;
+      }
     }
   }
   while (debt < 0) {
     if (rank_last[1] == kNone) {
+      ZB_HUF_TRACE(kTrOvershootNoRank1);
       while (T.depth[n] == max_nb) n--;
       T.depth[n + 1]--;
       rank_last[1] = (uint32_t)(n + 1);
       debt++;
       continue;
     }
+    ZB_HUF_TRACE(kTrOvershootRank1);
     T.depth[rank_last[1] + 1]--;
     rank_last[1]++;
     debt++;
@@ -513,10 +572,16 @@ ZB_HD inline int huf_write_table(TreeScratch& T, const uint8_t* nb, int max_sym,
   int h = huf_pack_weights(T.hdr + 1, T.weight, max_sym, T.fse);
   if (h < 0) return -1;
   if (h > 1 && h < max_sym / 2) {
+    ZB_HUF_TRACE(kTrTableFse);
     T.hdr[0] = (uint8_t)h;
     return h + 1;
   }
-  if (max_sym > 128) return -1;
+  if (max_sym > 128) {
+    ZB_HUF_TRACE(kTrTableRaw);
+    return -1;
+  }
+  if (h > 1) ZB_HUF_TRACE(kTrTableNibbleLost);
+  ZB_HUF_TRACE(kTrTableNibble);
   T.hdr[0] = (uint8_t)(128 + (max_sym - 1));
   T.weight[max_sym] = 0;
   for (int s = 0; s < max_sym; s += 2) T.hdr[(s / 2) + 1] = (uint8_t)((T.weight[s] << 4) + T.weight[s + 1]);
@@ -526,6 +591,16 @@ ZB_HD inline int huf_write_table(TreeScratch& T, const uint8_t* nb, int max_sym,
 // ---------------------------------------------------------------------------------
 // Block decision: what the reference stores for one byte plane of plen bytes.
 // ---------------------------------------------------------------------------------
+// The early-outs of HUF_compress that need the histogram alone (huf_compress.c:658, 673-674); largest = the count of
+// the plane's most frequent byte.  0 = stored raw, 1 = one symbol (RLE), 2 = build the table.
+ZB_HD inline int huf_early_out(uint32_t largest, uint32_t plen) {
+  if (plen == 0 || plen > (uint32_t)kHufBlockMax) return 0;
+  if (largest == plen) return 1;
+  if (largest <= (plen >> 7) + 4) return 0;  // "probably not compressible"
+  return 2;
+}
+
+
 // HUF_compress into a destination of cap bytes (huf_compress.c:637-724), then the threshold of
 // zipnn_core.c:371-373.  The caller has already applied the early-outs that need the histogram:
 // rle = every byte of the plane is equal (huf_compress.c:673); otherwise the plane passed the
