@@ -222,6 +222,40 @@ int zipnn_b200_decode_plan_gather(const zipnn_b200_decode_plan* plan, int item, 
                                   size_t n_ids, int id_bytes, void* d_out, void* d_scratch, size_t scratch_bytes,
                                   void* cuda_stream);
 
+/* _matvec: y = x W^T (+ bias) for a few rows of x, straight from the coded bitstreams of item `item`: the dense W is
+ * never written or read back.  W is the item's decoded tensor, row-major [out_features][in_features] of `dtype`
+ * (out_features = the item's elements / in_features); x is n_tokens rows of in_features elements, x_stride elements
+ * apart; y is n_tokens rows of out_features elements, y_stride apart; x, y and the optional d_bias (out_features
+ * elements, or NULL) have the weight's dtype.  Products and sums are fp32; each y is rounded once.
+ * Launches: 2 whatever n_tokens and the shapes are -- the plan run's per-bitstream replay decoder, whose fused merge
+ * multiplies each 16 bytes it forms with x instead of storing them and writes one fp32 partial sum per (block of the
+ * tensor, row it touches, token) to d_scratch, and a reduction that adds each row's partial sums in ascending element
+ * order.  No atomics on floats, no copy, memset or synchronisation: capturable in a CUDA graph, replayable with new x,
+ * and two calls with the same inputs give the same bits.  n_tokens == 0 launches nothing.
+ * Eligible items (else E_UNSUPPORTED, and the caller decodes the item as before): a whole tensor in one piece (not a
+ * box, not empty, at most 16384 chunks) of a plan with a segment index; num_buf equal to the dtype's size;
+ * in_features * element size a multiple of 16; every chunk in the fused decode mode (one coded plane, the top byte
+ * plane; chunk length a multiple of 512) -- what float weights produce.  The first _matvec or _matvec_scratch_size call
+ * for an item reads its chunk modes from the device and synchronises cuda_stream (the null stream for _scratch_size);
+ * later calls do not.
+ * Host-side rejections launch and write nothing: E_ARG for n_tokens above ZIPNN_B200_MATVEC_MAX_TOKENS, a dtype other
+ * than the three below, in_features 0 or not dividing the item's elements, an item index out of range, a plan whose
+ * create failed, and with n_tokens > 0: a NULL d_x, d_y or d_scratch, d_x not 16-byte aligned, x_stride * element size
+ * not a multiple of 16 or a stride shorter than its row (n_tokens > 1), d_y or d_bias not aligned to the element,
+ * d_scratch not 256-byte aligned, scratch_bytes below _matvec_scratch_size.
+ * d_scratch holds nothing between calls: calls that share it must be ordered on one stream, and it may be the plan
+ * scratch of runs ordered on that stream.  The plan's own scratch and outputs are not touched, so a matvec may run next
+ * to a _run_shifted of the same plan on another stream.  Decode errors reach the word _status reads. */
+#define ZIPNN_B200_MATVEC_MAX_TOKENS 8
+#define ZIPNN_B200_MATVEC_BF16 0
+#define ZIPNN_B200_MATVEC_FP16 1
+#define ZIPNN_B200_MATVEC_FP32 2
+int zipnn_b200_decode_plan_matvec_scratch_size(const zipnn_b200_decode_plan* plan, int item, int dtype,
+                                               size_t in_features, size_t n_tokens, size_t* out);
+int zipnn_b200_decode_plan_matvec(const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features,
+                                  const void* d_x, size_t x_stride, size_t n_tokens, const void* d_bias, void* d_y,
+                                  size_t y_stride, void* d_scratch, size_t scratch_bytes, void* cuda_stream);
+
 /* ---- stage 1 alone ------------------------------------------------------------ */
 /* d_planes: num_buf planes of `stride` bytes each; plane g receives byte g of every element
  * of the (optionally rotated) input.  Lengths as in the reference: n/num_buf, the first

@@ -365,13 +365,53 @@ struct SegEntry {
   uint32_t n;     // symbols in the segment
 };
 static_assert(sizeof(SegEntry) == 8, "8 bytes per segment: 8 KiB per coded item");
+// 16 bytes of a fused chunk's elements at byte `o` of the quarter that starts at plane byte `out_off`, into r[0..3]:
+// the coded plane from shared memory, the other planes (S.src: raw bytes of the stream or an RLE fill) interleaved
+// with it, the sign bit un-rotated when `rot`.  o is a multiple of 16.  Shared by the store loop of sync_process and
+// the matvec (matvec.cuh) as a macro: as a function, even a force-inlined one, it changes the register allocation of
+// k_huf_decode_sync<2>, and the decoders' machine code is kept byte for byte what it was.
+#define ZB_FUSED_VECTOR(G, S, out_off, o, rot, r)                                                             \
+  do {                                                                                                        \
+    if (G == 1) {                                                                                             \
+      smem_plane_words<4>(S.plane, o, r);                                                                     \
+    } else if (G == 2) {                                                                                      \
+      uint32_t a[2], e2[2];                                                                                   \
+      load_plane_words<2>(S.src[0], out_off + (o >> 1), a);                                                   \
+      smem_plane_words<2>(S.plane, o >> 1, e2);                                                               \
+      r[0] = __byte_perm(a[0], e2[0], 0x5140);                                                                \
+      r[1] = __byte_perm(a[0], e2[0], 0x7362);                                                                \
+      r[2] = __byte_perm(a[1], e2[1], 0x5140);                                                                \
+      r[3] = __byte_perm(a[1], e2[1], 0x7362);                                                                \
+    } else {                                                                                                  \
+      uint32_t p0[1], p1[1], p2[1], p3[1];                                                                    \
+      load_plane_words<1>(S.src[0], out_off + (o >> 2), p0);                                                  \
+      load_plane_words<1>(S.src[1 % 3], out_off + (o >> 2), p1);                                              \
+      load_plane_words<1>(S.src[2 % 3], out_off + (o >> 2), p2);                                              \
+      smem_plane_words<1>(S.plane, o >> 2, p3);                                                               \
+      const uint32_t t0 = __byte_perm(p0[0], p1[0], 0x5140), t1 = __byte_perm(p2[0], p3[0], 0x5140);          \
+      const uint32_t t2 = __byte_perm(p0[0], p1[0], 0x7362), t3 = __byte_perm(p2[0], p3[0], 0x7362);          \
+      r[0] = __byte_perm(t0, t1, 0x5410);                                                                     \
+      r[1] = __byte_perm(t0, t1, 0x7632);                                                                     \
+      r[2] = __byte_perm(t2, t3, 0x5410);                                                                     \
+      r[3] = __byte_perm(t2, t3, 0x7632);                                                                     \
+    }                                                                                                         \
+    if (rot) {                                                                                                \
+      _Pragma("unroll") for (int i = 0; i < 4; i++) r[i] = unrot_word<G>(r[i]);                               \
+    }                                                                                                         \
+  } while (0)
+
 // W: `out` is the box of cfg (box_store16) instead of the whole tensor.
 // GA (the gather, gather.cuh): every chunk, fused ones included, copies its quarter plane to the chunk's planes at
 // `gplanes` (G planes of cfg.pstride bytes) instead of the pool; the merge is left to the gather.
+// MV (the matvec, matvec.cuh): a fused chunk's elements are not stored: `mv->quarter` multiplies them with the
+// activations as they are formed; chunks of any other mode are left alone (the host admits none).
+struct NoMatvec {
+  static constexpr bool on = false;
+};
 static_assert(kSyncThreads * 16 == kBoxStep, "the merge advances the box cursor by kBoxStep");
-template <int G, bool W = false, int M = kSyncDecode, bool GA = false>
+template <int G, bool W = false, int M = kSyncDecode, bool GA = false, class MV = NoMatvec>
 __device__ __forceinline__ void sync_process(const DecodeCfg& cfg, uint8_t* __restrict__ out, SyncShared& S, uint16_t* lut_tab, uint32_t lut_s,
-                                             uint64_t work, SegEntry* segs = nullptr, uint8_t* gplanes = nullptr) {
+                                             uint64_t work, SegEntry* segs = nullptr, uint8_t* gplanes = nullptr, const MV* mv = nullptr) {
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const uint64_t K = cfg.K;
   {
@@ -561,6 +601,10 @@ __device__ __forceinline__ void sync_process(const DecodeCfg& cfg, uint8_t* __re
         S.src[tid] = s;
       }
       __syncthreads();
+      if constexpr (MV::on) {
+        mv->template quarter<G>(S, c, stream, out_off, count, (cfg.bits_mode == 1) && (G > 1));
+        return;
+      }
       uint8_t* out_q = out + c * (uint64_t)cfg.chunk + (uint64_t)out_off * G;
       const bool rot = (cfg.bits_mode == 1) && (G > 1);
       const uint32_t obytes = count * (uint32_t)G;
@@ -568,33 +612,7 @@ __device__ __forceinline__ void sync_process(const DecodeCfg& cfg, uint8_t* __re
       if (W) bc = box_cursor(cfg, c * (uint64_t)cfg.chunk + (uint64_t)out_off * G + (uint32_t)tid * 16u);
       for (uint32_t o = (uint32_t)tid * 16u; o < obytes; o += kSyncThreads * 16u) {
         uint32_t r[4];
-        if (G == 1) {
-          smem_plane_words<4>(S.plane, o, r);
-        } else if (G == 2) {
-          uint32_t a[2], e2[2];
-          load_plane_words<2>(S.src[0], out_off + (o >> 1), a);
-          smem_plane_words<2>(S.plane, o >> 1, e2);
-          r[0] = __byte_perm(a[0], e2[0], 0x5140);
-          r[1] = __byte_perm(a[0], e2[0], 0x7362);
-          r[2] = __byte_perm(a[1], e2[1], 0x5140);
-          r[3] = __byte_perm(a[1], e2[1], 0x7362);
-        } else {
-          uint32_t p0[1], p1[1], p2[1], p3[1];
-          load_plane_words<1>(S.src[0], out_off + (o >> 2), p0);
-          load_plane_words<1>(S.src[1 % 3], out_off + (o >> 2), p1);
-          load_plane_words<1>(S.src[2 % 3], out_off + (o >> 2), p2);
-          smem_plane_words<1>(S.plane, o >> 2, p3);
-          const uint32_t t0 = __byte_perm(p0[0], p1[0], 0x5140), t1 = __byte_perm(p2[0], p3[0], 0x5140);
-          const uint32_t t2 = __byte_perm(p0[0], p1[0], 0x7362), t3 = __byte_perm(p2[0], p3[0], 0x7362);
-          r[0] = __byte_perm(t0, t1, 0x5410);
-          r[1] = __byte_perm(t0, t1, 0x7632);
-          r[2] = __byte_perm(t2, t3, 0x5410);
-          r[3] = __byte_perm(t2, t3, 0x7632);
-        }
-        if (rot) {
-#pragma unroll
-          for (int i = 0; i < 4; i++) r[i] = unrot_word<G>(r[i]);
-        }
+        ZB_FUSED_VECTOR(G, S, out_off, o, rot, r);
         if (W) {
           box_store16(cfg, out, bc, r);
           box_advance(cfg, bc);
@@ -602,7 +620,7 @@ __device__ __forceinline__ void sync_process(const DecodeCfg& cfg, uint8_t* __re
           *reinterpret_cast<uint4*>(out_q + o) = make_uint4(r[0], r[1], r[2], r[3]);
         }
       }
-    } else {
+    } else if constexpr (!MV::on) {
       uint8_t* dst = GA ? gplanes + (uint64_t)g * cfg.pstride + out_off : cfg.planes + ((uint64_t)cfg.slot[c] * G + g) * cfg.pstride + out_off;
       if (((uintptr_t)dst & 3) == 0) {
         const uint32_t nw = count >> 2;

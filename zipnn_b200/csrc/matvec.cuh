@@ -1,0 +1,231 @@
+// matvec.cuh -- y = x W^T for a few rows of x, with W a whole-tensor item of a decode plan that is never written dense.
+//
+// y[t][o] = sum_i x[t][i] * W[o][i] (+ bias[o]), t < n_tokens <= kMatvecMaxTokens, W row-major [out][in] of bf16, fp16
+// or fp32, every chunk of it in fused mode (the host checks).  Two launches per call, whatever the shapes are:
+//
+//   k_matvec         sync_process in replay mode, one CTA per coded bitstream as in a plan run: tables, stream staging,
+//                    segment index and the fused merge (ZB_FUSED_VECTOR) are the plan run's.  Where the run stores the 16
+//                    bytes it formed, `MatvecEp::quarter` multiplies them with the activations.
+//   k_matvec_reduce  one thread per (token, output row) adds the row's partial sums in ascending element order, adds the
+//                    bias, rounds once to the output type and stores.
+//
+// Thread mapping.  The run's store loop gives thread t the vectors t, t + 256, ...: fine for stores, but it scatters a
+// row of W over all threads, so every row would end in a CTA-wide reduction.  Here a warp owns a contiguous BLOCK of
+// the quarter plane (an eighth of it, rounded up to whole 32-vector steps) and its lanes take consecutive vectors:
+// the quarter plane in shared memory and x in L2 are read coalesced, a row's sum stays in per-lane fp32 accumulators
+// across steps, and it ends in one butterfly of shuffles when the warp leaves the row.  With in_features a multiple of
+// 32 vectors (every llama shape) a step lies in one row and the row test is uniform; a step that straddles rows (small
+// or odd in_features) walks its rows one by one, each lane adding to the row its vector is in.
+//
+// Partial sums.  A block is identified by (chunk, bitstream, warp) and covers a fixed element range, so the rows it
+// touches are known from the shapes alone: at most rs = (block elements + in - 2) / in + 1 of them.  The warp writes one
+// fp32 per (row, token) to part[((block * rs) + row - block's first row) * n_tokens + t]: every slot the reduce reads
+// is written by exactly one warp in every call, nothing is accumulated in memory, no atomics and no memset, and the
+// order of every addition is fixed by the shapes: two calls with the same inputs give the same bits.
+#pragma once
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
+#include "decode_sync.cuh"
+
+namespace zb {
+
+constexpr int kMatvecMaxTokens = 8;
+enum : int { kMvBf16 = 0, kMvFp16 = 1, kMvFp32 = 2 };
+__host__ __device__ constexpr int matvec_esize(int dt) { return dt == kMvFp32 ? 4 : 2; }
+
+struct MatvecCfg {
+  const DecodeCfg* cfg;   // the item's piece, in plan memory
+  SegEntry* seg;          // the piece's segment index
+  uint32_t* error;        // the plan's error word
+  const void* x;
+  const void* bias;       // or nullptr
+  void* y;
+  float* part;            // the partial sums (scratch)
+  uint64_t in, out;       // features
+  uint64_t xs, ys;        // row strides of x and y, in elements
+  uint64_t ce, total, K;  // elements of a full chunk and of the tensor; chunks
+  uint32_t esize, nt, rs; // element bytes, tokens, slots (rows) per block
+  uint32_t step_rows, step_cols;  // one 32-vector step as whole rows + columns
+};
+
+// Elements of a block of a chunk with n elements: a quarter's vectors split over 8 warps, in whole 32-vector steps.
+__host__ __device__ inline uint64_t matvec_block_elems(uint64_t n, uint32_t esize) {
+  const uint64_t epv = 16 / esize, nv = (n / 4) / epv;
+  return ((nv + 255) / 256) * 32 * epv;
+}
+// Rows of `in` elements that `be` consecutive elements can touch, wherever they start.
+__host__ __device__ inline uint64_t matvec_block_rows(uint64_t be, uint64_t in, uint64_t out) {
+  const uint64_t r = (be + in - 2) / in + 1;
+  return r < out ? r : out;
+}
+// The block that holds element e: its number and its element range [start, end).
+struct MatvecBlock {
+  uint64_t id, start, end;
+};
+__device__ __forceinline__ MatvecBlock matvec_block_of(const MatvecCfg& m, uint64_t e) {
+  const uint64_t c = e / m.ce;
+  const uint64_t n = c == m.K - 1 ? m.total - c * m.ce : m.ce;
+  const uint64_t q = n / 4, be = matvec_block_elems(n, m.esize);
+  const uint64_t r = e - c * m.ce, s = r / q, w = (r - s * q) / be;
+  MatvecBlock b;
+  b.id = (c * 4 + s) * 8 + w;
+  b.start = c * m.ce + s * q + w * be;
+  b.end = min(b.start + be, c * m.ce + (s + 1) * q);
+  return b;
+}
+
+template <int DT, int EPV>
+__device__ __forceinline__ void matvec_floats(const uint32_t (&r)[4], float (&f)[EPV]) {
+#pragma unroll
+  for (int i = 0; i < 4; i++) {
+    if constexpr (DT == kMvBf16) {
+      f[2 * i] = __uint_as_float(r[i] << 16);
+      f[2 * i + 1] = __uint_as_float(r[i] & 0xFFFF0000u);
+    } else if constexpr (DT == kMvFp16) {
+      const float2 v = __half22float2(*reinterpret_cast<const __half2*>(&r[i]));
+      f[2 * i] = v.x;
+      f[2 * i + 1] = v.y;
+    } else {
+      f[i] = __uint_as_float(r[i]);
+    }
+  }
+}
+
+// NT: the accumulators a lane holds, n_tokens rounded up to a power of two.  Tokens past n_tokens repeat the last one
+// and are not stored: 3 and 5 to 7 tokens pay for 4 and 8.  A uniform `t < n_tokens` exit from the token loop was
+// measured instead: it keeps the loads of the tokens from being issued together, and 8 tokens took 1.3 to 1.5 times as long.
+template <int DT, int NT>
+struct MatvecEp {
+  static constexpr bool on = true;
+  static constexpr int EPV = 16 / matvec_esize(DT);
+  MatvecCfg m;
+
+  __device__ __forceinline__ void flush(float (&acc)[NT], float* slot, int lane) const {
+#pragma unroll
+    for (int t = 0; t < NT; t++) {
+      float v = acc[t];
+#pragma unroll
+      for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if (lane == t && (uint32_t)t < m.nt) slot[t] = v;
+      acc[t] = 0.f;
+    }
+  }
+
+  // The quarter plane of bitstream `stream` of chunk c is in S.plane (count elements from plane byte out_off).
+  template <int G>
+  __device__ __forceinline__ void quarter(const SyncShared& S, uint64_t c, int stream, uint32_t out_off, uint32_t count, bool rot) const {
+    static_assert(G == matvec_esize(DT), "one byte plane per byte of the element");
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint32_t nv = count / EPV;
+    const uint32_t vpw = ((nv + 255u) >> 8) << 5;
+    const uint32_t v0 = (uint32_t)wid * vpw, v1 = min(nv, v0 + vpw);
+    if (v0 >= v1) return;  // (warp-uniform) a short last chunk leaves the upper warps without a block
+    const uint64_t in = m.in;
+    const uint64_t e0 = c * m.ce + out_off + (uint64_t)v0 * EPV;
+    uint64_t row0 = e0 / in, col0 = e0 - row0 * in;  // of the step's first element: the same in every lane
+    float* const slots = m.part + ((c * 4 + (uint32_t)stream) * 8 + (uint32_t)wid) * m.rs * m.nt;  // the block's, from its first row
+    const uint64_t first = row0;
+    const uint8_t* const xb = reinterpret_cast<const uint8_t*>(m.x);
+    float acc[NT];
+#pragma unroll
+    for (int t = 0; t < NT; t++) acc[t] = 0.f;
+    uint64_t cur = row0;
+    for (uint32_t v = v0; v < v1; v += 32) {
+      const uint32_t nvalid = min(32u, v1 - v);
+      const bool valid = (uint32_t)lane < nvalid;
+      uint64_t lrow = row0, lcol = col0 + (uint32_t)lane * EPV;
+      uint64_t last = row0;
+      if (col0 + 32u * EPV > in) {  // (uniform) the step straddles rows
+        const uint64_t q = lcol / in;
+        lrow += q;
+        lcol -= q * in;
+        last += (col0 + nvalid * EPV - 1) / in;
+      }
+      float p[NT];
+#pragma unroll
+      for (int t = 0; t < NT; t++) p[t] = 0.f;
+      if (valid) {
+        uint32_t r[4];
+        const uint32_t o = (v + (uint32_t)lane) * 16u;
+        ZB_FUSED_VECTOR(G, S, out_off, o, rot, r);
+        float w[EPV];
+        matvec_floats<DT, EPV>(r, w);
+#pragma unroll
+        for (int t = 0; t < NT; t++) {
+          const uint64_t tt = min((uint32_t)t, m.nt - 1u);
+          const uint4 xv = __ldg(reinterpret_cast<const uint4*>(xb + (tt * m.xs + lcol) * matvec_esize(DT)));
+          const uint32_t xr[4] = {xv.x, xv.y, xv.z, xv.w};
+          float xf[EPV];
+          matvec_floats<DT, EPV>(xr, xf);
+          float s = 0.f;
+#pragma unroll
+          for (int i = 0; i < EPV; i++) s = fmaf(w[i], xf[i], s);
+          p[t] = s;
+        }
+      }
+      for (uint64_t rr = row0; rr <= last; rr++) {
+        if (rr != cur) {
+          flush(acc, slots + (cur - first) * m.nt, lane);
+          cur = rr;
+        }
+        if (lrow == rr) {
+#pragma unroll
+          for (int t = 0; t < NT; t++) acc[t] += p[t];
+        }
+      }
+      row0 += m.step_rows;
+      col0 += m.step_cols;
+      if (col0 >= in) {
+        col0 -= in;
+        row0++;
+      }
+    }
+    flush(acc, slots + (cur - first) * m.nt, lane);
+  }
+};
+
+// One CTA per coded bitstream of the item (every chunk is fused: its one coded item is the top byte plane).
+template <int DT, int NT>
+__global__ void __launch_bounds__(kSyncThreads, 3) k_matvec(MatvecCfg m) {
+  extern __shared__ __align__(1024) unsigned char smem_raw[];
+  const SyncCarve cv = sync_carve(smem_raw);
+  SyncShared& S = *cv.S;
+  const DecodeCfg& cfg = *m.cfg;
+  const MatvecEp<DT, NT> ep{m};
+  const uint64_t works = 4ull * cfg.ctrl->huf_count;
+  for (uint64_t work = blockIdx.x; work < works; work += gridDim.x) {
+    __syncthreads();  // the previous bitstream's shared state is dead
+    sync_process<matvec_esize(DT), false, kSyncReplay, false, MatvecEp<DT, NT>>(cfg, nullptr, S, cv.lut, cv.lut_s, work, m.seg + work * kSyncThreads,
+                                                                                nullptr, &ep);
+  }
+}
+
+template <int DT>
+__global__ void __launch_bounds__(256) k_matvec_reduce(MatvecCfg m) {
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    const uint32_t e = *(volatile uint32_t*)&m.cfg->ctrl->error;  // a decode error of this call
+    if (e) atomicOr(m.error, e);
+  }
+  const uint64_t idx = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (idx >= m.out * m.nt) return;
+  const uint64_t t = idx / m.out, o = idx - t * m.out;
+  float s = 0.f;
+  for (uint64_t e = o * m.in; e < (o + 1) * m.in;) {
+    const MatvecBlock b = matvec_block_of(m, e);
+    s += m.part[((b.id * m.rs) + o - b.start / m.in) * m.nt + t];
+    e = b.end;
+  }
+  if (DT == kMvBf16) {
+    if (m.bias) s += __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(m.bias)[o]);
+    reinterpret_cast<__nv_bfloat16*>(m.y)[t * m.ys + o] = __float2bfloat16_rn(s);
+  } else if (DT == kMvFp16) {
+    if (m.bias) s += __half2float(reinterpret_cast<const __half*>(m.bias)[o]);
+    reinterpret_cast<__half*>(m.y)[t * m.ys + o] = __float2half_rn(s);
+  } else {
+    if (m.bias) s += reinterpret_cast<const float*>(m.bias)[o];
+    reinterpret_cast<float*>(m.y)[t * m.ys + o] = s;
+  }
+}
+
+}  // namespace zb

@@ -20,6 +20,7 @@
 #include "decode_sync.cuh"
 #include "encode.cuh"
 #include "gather.cuh"
+#include "matvec.cuh"
 #include "stage1.cuh"
 
 using namespace zb;
@@ -939,6 +940,8 @@ struct GatherItem {
   uint32_t chunk;
   uint64_t K, orig;
   uint64_t seg_base;  // the piece's first segment index entry
+  const uint8_t* d_mode;  // the piece's chunk modes (device, [K])
+  int fused;          // every chunk is in fused mode (a matvec needs that): -1 until a matvec call has read d_mode
 };
 struct PlanItems {
   uint32_t gen;
@@ -1097,7 +1100,7 @@ int zipnn_b200_decode_plan_create(const zipnn_b200_slice_item* items, int n, voi
     rec.items.resize((size_t)n);
     for (int i = 0; i < n; i++) {
       const zipnn_b200_slice_item& it = items[i];
-      rec.items[i] = GatherItem{-1, it.num_buf, (uint32_t)it.chunk, num_chunks(it.orig, it.chunk), it.orig, 0};
+      rec.items[i] = GatherItem{-1, it.num_buf, (uint32_t)it.chunk, num_chunks(it.orig, it.chunk), it.orig, 0, nullptr, -1};
     }
     for (int j = 0; j < np; j++) {
       const SlicePiece& p = P.pieces[j];
@@ -1106,6 +1109,7 @@ int zipnn_b200_decode_plan_create(const zipnn_b200_slice_item* items, int n, voi
       const bool whole = p.base == 0 && p.rows == 1 && p.len == it.orig;
       g.piece = whole && g.piece == -1 ? j : -2;   // (-2: a box or a split item; the pieces of an item are consecutive)
       g.seg_base = P.seg_base[j];
+      g.d_mode = cfgs[j].mode;
     }
     for (GatherItem& g : rec.items)
       if (g.piece < 0) g.piece = -1;
@@ -1278,6 +1282,148 @@ int zipnn_b200_decode_plan_gather(const zipnn_b200_decode_plan* plan, int item, 
     ZB_LAUNCHED();
   }
   return ZIPNN_B200_OK;
+}
+
+// ---- matvec: x W^T from the coded bitstreams of one whole-tensor item, no dense W (matvec.cuh) ------------------
+// Scratch: [32 K blocks][rs rows][n_tokens] fp32 partial sums.
+namespace {
+struct MatvecGeom {
+  uint64_t in, out, ce, total;
+  uint32_t esize, rs;
+};
+// The host-side checks shared by both calls.  The first call for an item reads its chunk modes (one synchronising copy
+// of K bytes); the answer is kept with the plan's record.
+int matvec_item(const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, cudaStream_t st, PlanState& s, GatherItem& gi,
+                MatvecGeom& M) {
+  if (!plan_state(plan, s)) return ZIPNN_B200_E_ARG;
+  const auto record = [&](GatherItem* set) -> int {
+    std::lock_guard<std::mutex> lk(g_plan_mu);
+    const auto it = g_plan_items.find((uintptr_t)s.B.error_out);
+    if (it == g_plan_items.end() || it->second.gen != s.gen) return ZIPNN_B200_E_ARG;
+    if (item < 0 || (size_t)item >= it->second.items.size()) return ZIPNN_B200_E_ARG;
+    if (set) it->second.items[(size_t)item].fused = set->fused;
+    gi = it->second.items[(size_t)item];
+    return ZIPNN_B200_OK;
+  };
+  {
+    const int rc = record(nullptr);
+    if (rc) return rc;
+  }
+  if (dtype != kMvBf16 && dtype != kMvFp16 && dtype != kMvFp32) return ZIPNN_B200_E_ARG;
+  M.esize = (uint32_t)matvec_esize(dtype);
+  M.total = gi.orig / M.esize;
+  if (in_features == 0 || gi.orig % M.esize || M.total % in_features) return ZIPNN_B200_E_ARG;
+  if (gi.piece < 0 || s.mode != kSyncReplay || gi.G != (int)M.esize || (in_features * M.esize) % 16) return ZIPNN_B200_E_UNSUPPORTED;
+  if (gi.fused < 0) {
+    std::vector<uint8_t> mode((size_t)gi.K);
+    ZB_CUDA(cudaMemcpyAsync(mode.data(), gi.d_mode, (size_t)gi.K, cudaMemcpyDeviceToHost, st));
+    ZB_CUDA(cudaStreamSynchronize(st));
+    gi.fused = 1;
+    for (const uint8_t m : mode) gi.fused &= m == kModeFused;
+    const int rc = record(&gi);
+    if (rc) return rc;
+  }
+  if (!gi.fused) return ZIPNN_B200_E_UNSUPPORTED;
+  M.in = in_features;
+  M.out = M.total / in_features;
+  M.ce = gi.chunk / M.esize;
+  M.rs = (uint32_t)matvec_block_rows(matvec_block_elems(std::min<uint64_t>(M.ce, M.total), M.esize), M.in, M.out);
+  return ZIPNN_B200_OK;
+}
+size_t matvec_scratch_bytes(const GatherItem& gi, const MatvecGeom& M, size_t n_tokens) { return (size_t)32 * gi.K * M.rs * n_tokens * sizeof(float); }
+
+extern "C++" template <int DT>
+int matvec_launch(const MatvecCfg& m, cudaStream_t st) {
+  const auto decode = [&](auto nt) -> int {
+    constexpr int NT = decltype(nt)::value;
+    // the shared-memory opt-in is per device: one bit per device ordinal, set once the attribute is
+    static std::atomic<uint64_t> attr_done{0};
+    int dev = 0;
+    ZB_CUDA(cudaGetDevice(&dev));
+    if (dev >= 64 || !((attr_done.load(std::memory_order_acquire) >> dev) & 1)) {
+      ZB_CUDA(cudaFuncSetAttribute(k_matvec<DT, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSyncSmemBytes));
+      if (dev < 64) attr_done.fetch_or(1ull << dev, std::memory_order_release);
+    }
+    static const int nb = [] {
+      int v = 0;
+      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_matvec<DT, NT>, kSyncThreads, kSyncSmemBytes) != cudaSuccess || v < 1) v = 1;
+      return v;
+    }();
+    const unsigned blocks = (unsigned)std::min<uint64_t>(4 * m.K, (uint64_t)nb * sm_count_cached());
+    k_matvec<DT, NT><<<blocks, kSyncThreads, kSyncSmemBytes, st>>>(m);
+    ZB_LAUNCHED();
+    return ZIPNN_B200_OK;
+  };
+  int rc;
+  if (m.nt <= 1) rc = decode(std::integral_constant<int, 1>{});
+  else if (m.nt <= 2) rc = decode(std::integral_constant<int, 2>{});
+  else if (m.nt <= 4) rc = decode(std::integral_constant<int, 4>{});
+  else rc = decode(std::integral_constant<int, 8>{});
+  if (rc) return rc;
+  k_matvec_reduce<DT><<<(unsigned)((m.out * m.nt + 255) / 256), 256, 0, st>>>(m);
+  ZB_LAUNCHED();
+  return ZIPNN_B200_OK;
+}
+}  // namespace
+
+static_assert(kMatvecMaxTokens == ZIPNN_B200_MATVEC_MAX_TOKENS && kMvBf16 == ZIPNN_B200_MATVEC_BF16 && kMvFp16 == ZIPNN_B200_MATVEC_FP16 &&
+                  kMvFp32 == ZIPNN_B200_MATVEC_FP32,
+              "the header's constants are the kernels'");
+
+int zipnn_b200_decode_plan_matvec_scratch_size(const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, size_t n_tokens,
+                                               size_t* out) {
+  if (!out || n_tokens > (size_t)kMatvecMaxTokens) return ZIPNN_B200_E_ARG;
+  PlanState s;
+  GatherItem gi;
+  MatvecGeom M;
+  const int rc = matvec_item(plan, item, dtype, in_features, nullptr, s, gi, M);
+  if (rc) return rc;
+  *out = matvec_scratch_bytes(gi, M, n_tokens);
+  return ZIPNN_B200_OK;
+}
+
+int zipnn_b200_decode_plan_matvec(const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, const void* d_x, size_t x_stride,
+                                  size_t n_tokens, const void* d_bias, void* d_y, size_t y_stride, void* d_scratch, size_t scratch_bytes,
+                                  void* cuda_stream) {
+  if (n_tokens > (size_t)kMatvecMaxTokens) return ZIPNN_B200_E_ARG;
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  PlanState s;
+  GatherItem gi;
+  MatvecGeom M;
+  {
+    const int rc = matvec_item(plan, item, dtype, in_features, st, s, gi, M);
+    if (rc) return rc;
+  }
+  if (n_tokens == 0) return ZIPNN_B200_OK;
+  if (!d_x || !d_y || !d_scratch || ((uintptr_t)d_x & 15) || ((uintptr_t)d_scratch & 255) || ((uintptr_t)d_y % M.esize) ||
+      ((uintptr_t)d_bias % M.esize))
+    return ZIPNN_B200_E_ARG;
+  if (n_tokens > 1 && ((x_stride * M.esize) % 16 || x_stride < M.in || y_stride < M.out)) return ZIPNN_B200_E_ARG;
+  if (scratch_bytes < matvec_scratch_bytes(gi, M, n_tokens)) return ZIPNN_B200_E_ARG;
+  MatvecCfg m;
+  m.cfg = s.B.cfgs + gi.piece;
+  m.seg = s.X.seg + gi.seg_base;
+  m.error = s.B.error_out;
+  m.x = d_x;
+  m.bias = d_bias;
+  m.y = d_y;
+  m.part = (float*)d_scratch;
+  m.in = M.in;
+  m.out = M.out;
+  m.xs = x_stride;
+  m.ys = y_stride;
+  m.ce = M.ce;
+  m.total = M.total;
+  m.K = gi.K;
+  m.esize = M.esize;
+  m.nt = (uint32_t)n_tokens;
+  m.rs = M.rs;
+  const uint64_t step = 32ull * (16 / M.esize);
+  m.step_rows = (uint32_t)(step / M.in);
+  m.step_cols = (uint32_t)(step % M.in);
+  if (dtype == kMvBf16) return matvec_launch<kMvBf16>(m, st);
+  if (dtype == kMvFp16) return matvec_launch<kMvFp16>(m, st);
+  return matvec_launch<kMvFp32>(m, st);
 }
 
 int zipnn_b200_split(const void* d_in, size_t n, int num_buf, int bits_mode, void* d_planes, size_t stride,

@@ -26,6 +26,8 @@ from .zipnn import HEADER_LEN, HUF_MAX_BLOCK, ZipNN, _cuda_stream_handle
 _HEAD = HEADER_LEN + 1 + 9 * 255   # the 32-byte header and the longest packed shape (as decompress peeks)
 _ALIGN = 16
 GATHER_SLOTS = 64   # chunk slots of gather's default scratch: 16 MiB for 256 KiB chunks
+MATVEC_MAX_TOKENS = _native.MATVEC_MAX_TOKENS
+_MATVEC_DTYPES = {torch.bfloat16: 0, torch.float16: 1, torch.float32: 2}   # ZIPNN_B200_MATVEC_*
 
 
 def _round(n: int, a: int) -> int:
@@ -163,6 +165,9 @@ class DecodePlan:
         self._ref = C.byref(self._plan)
         self._offs = [(o, p.nbytes, p.dtype, p.shape) for p, o in zip(parsed, offs)]
         self._gather_scratch = None   # gather's default scratch, grown on demand
+        self._matvec = _native.lib().zipnn_b200_decode_plan_matvec
+        self._matvec_scratch = None   # matvec's default scratch, grown on demand
+        self._matvec_ok = {}          # (output, in_features) -> eligible?
 
     def run(self) -> list:
         """Enqueue the decode on the current CUDA stream (launches only) and return `.outputs`."""
@@ -255,6 +260,113 @@ class DecodePlan:
             raise ValueError("gather's scratch must be a contiguous CUDA uint8 tensor on the plan's device")
         rc = self._gather(self._ref, k, row, ids_c.data_ptr(), n, ids_c.element_size(), out.data_ptr(), scratch.data_ptr(),
                           scratch.numel(), torch.cuda.current_stream(self.device).cuda_stream)
+        if rc:
+            _native.check(rc)
+        return out
+
+    def _matvec_item(self, k: int) -> tuple:
+        if not 0 <= k < len(self._offs):
+            raise IndexError(f"DecodePlan has {len(self._offs)} outputs, not {k + 1}")
+        _, _, dt, sh = self._offs[k]
+        return dt, sh
+
+    def _matvec_size(self, k: int, in_features: int, n_tokens: int) -> tuple:
+        dt, _ = self._matvec_item(k)
+        out = C.c_size_t(0)
+        if dt not in _MATVEC_DTYPES or in_features <= 0:
+            return _native.E_UNSUPPORTED, 0
+        with torch.cuda.device(self.device):
+            rc = _native.lib().zipnn_b200_decode_plan_matvec_scratch_size(self._ref, k, _MATVEC_DTYPES[dt], int(in_features), int(n_tokens),
+                                                                          C.byref(out))
+        return rc, out.value
+
+    def matvec_ok(self, k: int, in_features: int) -> bool:
+        """Can `matvec` multiply by output `k` seen as rows of `in_features` elements?  True for a bf16 / fp16 / fp32
+        output in one piece whose rows are a multiple of 16 bytes and whose chunks all decode in the fused mode (what
+        float weights produce; a constant tensor or a ragged tail does not).  The first call for an output
+        synchronises (it reads the chunk modes); never raises for an output that exists."""
+        _, sh = self._matvec_item(k)
+        n = 1
+        for d in sh:
+            n *= d
+        if in_features <= 0 or n == 0 or n % in_features:
+            return False
+        if (k, in_features) not in self._matvec_ok:
+            self._matvec_ok[(k, in_features)] = self._matvec_size(k, in_features, 1)[0] == _native.OK
+        return self._matvec_ok[(k, in_features)]
+
+    def matvec_scratch_bytes(self, k: int, in_features: int, n_tokens: int = MATVEC_MAX_TOKENS) -> int:
+        """Bytes of a matvec scratch for output `k`, rows of `in_features` elements and `n_tokens` rows of x."""
+        rc, n = self._matvec_size(k, in_features, n_tokens)
+        _native.check(rc)
+        return n
+
+    def matvec(self, k: int, x: torch.Tensor, bias: torch.Tensor = None, out: torch.Tensor = None,
+               scratch: torch.Tensor = None) -> torch.Tensor:
+        """`x @ W.T (+ bias)` with W = output `k` seen as [out_features, in_features], in_features = x.shape[-1],
+        computed from the coded streams: W is neither written nor read dense (zipnn_b200_decode_plan_matvec).  Two
+        launches on the current CUDA stream, no host read: capturable in a CUDA graph and replayable with new x.
+        Products and sums are fp32, each result is rounded once; two calls with the same inputs give the same bits.
+
+        x:       CUDA tensor [..., in_features] of the output's dtype on the plan's device, at most MATVEC_MAX_TOKENS
+                 rows (product of the leading dims); rows that are not 16-byte aligned are copied first.
+        bias:    optional contiguous [out_features] tensor of the same dtype.
+        out:     optional tensor of shape x.shape[:-1] + (out_features,), same dtype, contiguous in its last dim
+                 with equally spaced rows (e.g. a column slice of a wider buffer).
+        scratch: optional 256-byte aligned CUDA uint8 buffer of at least `matvec_scratch_bytes(k, in_features, rows)`
+                 bytes.  It holds nothing between calls: calls (and plan runs) that share it must be ordered on one
+                 stream.  Default: a buffer kept by the plan.
+        -> out.  ValueError for an output `matvec_ok` refuses.  Works without the plan's output buffer."""
+        dt, sh = self._matvec_item(k)
+        if not (isinstance(x, torch.Tensor) and x.is_cuda and x.device == self.device and x.dtype == dt and x.dim() >= 1):
+            raise ValueError(f"matvec takes a CUDA {dt} tensor [..., in_features] on the plan's device")
+        in_features = x.shape[-1]
+        lead = tuple(x.shape[:-1])
+        n = 1
+        for d in lead:
+            n *= d
+        if n > MATVEC_MAX_TOKENS:
+            raise ValueError(f"matvec takes at most {MATVEC_MAX_TOKENS} rows of x, not {n}")
+        if not self.matvec_ok(k, in_features):
+            raise ValueError(f"matvec cannot multiply by output {k} with in_features {in_features} (see matvec_ok)")
+        total = 1
+        for d in sh:
+            total *= d
+        out_features = total // in_features
+        es = x.element_size()
+        x2 = x.reshape(max(n, 1), in_features) if n else x.reshape(0, in_features)
+        if n and (x2.stride(1) != 1 or x2.data_ptr() % 16 or (n > 1 and (x2.stride(0) * es) % 16)):
+            x2 = x2.contiguous()
+            if x2.data_ptr() % 16:
+                x2 = x2.clone()
+        if bias is not None and not (isinstance(bias, torch.Tensor) and bias.device == self.device and bias.dtype == dt
+                                     and tuple(bias.shape) == (out_features,) and bias.is_contiguous()):
+            raise ValueError(f"matvec's bias must be a contiguous {dt} CUDA tensor of shape ({out_features},) on the plan's device")
+        shape = lead + (out_features,)
+        if out is None:
+            out = torch.empty(shape, dtype=dt, device=self.device)
+        elif not (isinstance(out, torch.Tensor) and out.is_cuda and out.device == self.device and out.dtype == dt
+                  and tuple(out.shape) == shape):
+            raise ValueError(f"matvec's out must be a {dt} CUDA tensor of shape {shape} on the plan's device")
+        if n == 0:
+            return out
+        try:
+            y2 = out.view(n, out_features)
+        except RuntimeError:
+            y2 = None
+        if y2 is None or y2.stride(1) != 1:
+            raise ValueError("matvec's out must have contiguous rows, equally spaced")
+        if scratch is None:
+            need = self.matvec_scratch_bytes(k, in_features)
+            if self._matvec_scratch is None or self._matvec_scratch.numel() < need:
+                self._matvec_scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
+            scratch = self._matvec_scratch
+        elif not (isinstance(scratch, torch.Tensor) and scratch.is_cuda and scratch.device == self.device
+                  and scratch.dtype == torch.uint8 and scratch.is_contiguous()):
+            raise ValueError("matvec's scratch must be a contiguous CUDA uint8 tensor on the plan's device")
+        rc = self._matvec(self._ref, k, _MATVEC_DTYPES[dt], in_features, x2.data_ptr(), x2.stride(0), n,
+                          bias.data_ptr() if bias is not None else None, y2.data_ptr(), y2.stride(0), scratch.data_ptr(), scratch.numel(),
+                          torch.cuda.current_stream(self.device).cuda_stream)
         if rc:
             _native.check(rc)
         return out

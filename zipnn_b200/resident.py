@@ -23,6 +23,9 @@ Rules:
   * with `gather=True` a selected `torch.nn.Embedding` (its class's own forward, no max_norm) looks its rows up
     straight from the stream (`DecodePlan.gather`: only the chunks the ids touch are decoded) and is never decoded
     whole; its output is an ordinary tensor the caller owns;
+  * with `matvec=N` a selected `torch.nn.Linear` (its class's own forward) multiplies inputs of at most N rows
+    straight from the stream (`DecodePlan.matvec`: the dense weight is neither written nor read) and decodes as
+    before for larger inputs; its bias stays a dense parameter;
   * `state_dict()` does not see compressed parameters; `decompress_module(model)` restores them as dense
     `Parameter`s, bit for bit, and removes the hooks and plans.
 
@@ -38,7 +41,7 @@ import traceback
 import torch
 
 from . import prefetch as _prefetch
-from .plan import _HEAD, DecodePlan, _Stream
+from .plan import _HEAD, MATVEC_MAX_TOKENS, DecodePlan, _Stream
 from .safetensors_io import _FileRange, _cuda_device, compress_groups, file_entries, save_coded
 from .util_safetensors import COMPRESSION_METHOD
 from .zipnn import DecodePipe, ZipNN
@@ -101,6 +104,10 @@ class _Resident:
         self.scratch = None   # the plans' shared scratch
         self.gather_scratch = None  # the gathers' scratch: the plans' one, or a buffer of its own (prefetch)
         self.gather_plan_bytes = 0  # memory of the plans that only serve gathers
+        self.matvec = 0       # matvec=N: the most input rows a matvec module multiplies without decoding
+        self.matvecs = []     # matvec=N: (linear module, plan, index into the plan's outputs)
+        self.matvec_scratch = None  # the matvecs' scratch: the plans' one when it is large enough
+        self.matvec_scratch_bytes = 0  # what the largest matvec needs of it
 
 
 def _pre_hook(plan, names):
@@ -138,6 +145,51 @@ def _gather_forward(mod, state, plan, k):
             raise RuntimeError(f"{type(mod).__name__} holds compressed weights and runs only under torch.no_grad() or "
                                "torch.inference_mode()")
         return plan.gather(k, input, scratch=state.gather_scratch)
+    return forward
+
+
+def matvecs(module: torch.nn.Module) -> bool:
+    """Does `matvec=N` multiply small inputs of `module` from its compressed weight?  A torch.nn.Linear (or subclass)
+    whose class does not override forward."""
+    return isinstance(module, torch.nn.Linear) and type(module).forward is torch.nn.Linear.forward
+
+
+def dense_biases(groups, matvec: int) -> list:
+    """`select`'s groups without the biases that stay dense under matvec=N: those owned by `matvecs` modules only (the
+    matvec adds them after the sum, so they must not need a decode)."""
+    if not matvec:
+        return groups
+    return [(p, owners) for p, owners in groups if not all(n == "bias" and matvecs(o) for o, n in owners)]
+
+
+def _check_matvec(matvec: int, prefetch: bool) -> int:
+    if not (isinstance(matvec, int) and 0 <= matvec <= MATVEC_MAX_TOKENS):
+        raise ValueError(f"matvec must be an integer from 0 to {MATVEC_MAX_TOKENS}, not {matvec!r}")
+    if matvec and prefetch:
+        raise ValueError("matvec and prefetch=True do not combine yet: the prefetch schedule decodes every module")
+    return matvec
+
+
+def _matvec_forward(mod, state, plan, k, names, dtype, device):
+    """The forward of a matvec module: an input of at most `state.matvec` rows (a host-side test of its shape) that has
+    the weight's `dtype` and `device`, outside autocast, goes to `plan.matvec` and nothing is decoded or bound; any
+    other input (a larger one, another dtype, an autocast region: whatever F.linear accepts) takes the decode, bind,
+    forward, unbind of the hooks every other compressed module has."""
+    pre, post = _pre_hook(plan, names), _unbind(names)
+
+    def forward(input):
+        width = input.shape[-1] if input.dim() else 0
+        if (width and input.numel() // width <= state.matvec and input.dtype == dtype and input.device == device
+                and not torch.is_autocast_enabled(device.type)):
+            if torch.is_grad_enabled():
+                raise RuntimeError(f"{type(mod).__name__} holds compressed weights and runs only under torch.no_grad() or "
+                                   "torch.inference_mode()")
+            return plan.matvec(k, input, bias=mod.bias, scratch=state.matvec_scratch)
+        pre(mod, (input,))
+        try:
+            return torch.nn.Linear.forward(mod, input)
+        finally:
+            post(mod, (input,), None)
     return forward
 
 
@@ -181,14 +233,17 @@ def _pack(streams: dict, dev) -> tuple:
     return buf, views
 
 
-def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: bool = False) -> tuple:
+def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: bool = False, matvec: int = 0) -> tuple:
     """The back half of compress_module and load_module: streams {group index: CUDA stream} -> per selected module
     one DecodePlan over its parameters' streams, all sharing one output and one scratch buffer.  Raises like
     `decompress` on a corrupt stream; nothing outside is touched until `_commit`.  -> (_Resident, report).
 
     gather=True: embeddings (`gathers`) get no output space.  One whose weight a whole-decoded module also holds (a
     tied lm_head) gathers through that module's plan; any other gets a plan of its own, created first, into a
-    transient buffer that is freed before the shared output buffer exists (so the peak stays that of gather=False)."""
+    transient buffer that is freed before the shared output buffer exists (so the peak stays that of gather=False).
+
+    matvec=N: a `matvecs` module whose one compressed parameter is a weight that `DecodePlan.matvec_ok` accepts is
+    listed in `state.matvecs`; its plan and its room in the shared output buffer stay (larger inputs decode)."""
     where = {id(groups[i][0]): i for i in streams}
     per_module = []
     for m in modules:
@@ -222,6 +277,9 @@ def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: 
         state.entries.append((m, plan, [(n, k) for k, (n, _) in enumerate(names)], []))
         for k, (_, i) in enumerate(names):
             by_stream.setdefault(i, (plan, k))
+        if matvec and matvecs(m) and [n for n, _ in names] == ["weight"] and plan.matvec_ok(0, m.in_features):
+            state.matvecs.append((m, plan, 0))
+    state.matvec = matvec
     for m, i in looked:
         plan, k = by_stream[i]
         state.gathers.append((m, plan, k, i in own))
@@ -257,7 +315,17 @@ def _commit(module: torch.nn.Module, state: _Resident, prefetch: bool = False) -
             state.gather_scratch = state.scratch
         for m, plan, k, _ in state.gathers:
             m.__dict__["forward"] = _gather_forward(m, state, plan, k)
+    if state.matvecs:
+        need = max(plan.matvec_scratch_bytes(k, m.in_features, state.matvec) for m, plan, k in state.matvecs)
+        state.matvec_scratch_bytes = need
+        state.matvec_scratch = state.scratch if need <= state.scratch.numel() else torch.empty(need, dtype=torch.uint8,
+                                                                                                device=state.scratch.device)
+    by_matvec = {id(m): (plan, k) for m, plan, k in state.matvecs}
     for key, (m, plan, local, hooks) in enumerate(state.entries):
+        if id(m) in by_matvec:   # no hooks: its forward decides per input whether anything is decoded
+            m.__dict__["forward"] = _matvec_forward(m, state, plan, by_matvec[id(m)][1], local, plan.outputs[by_matvec[id(m)][1]].dtype,
+                                                    plan.device)
+            continue
         if sched is None:
             pre = _pre_hook(plan, local)
         else:
@@ -271,7 +339,7 @@ def _commit(module: torch.nn.Module, state: _Resident, prefetch: bool = False) -
     setattr(module, _ATTR, state)
 
 
-def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = False, gather: bool = False) -> dict:
+def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = False, gather: bool = False, matvec: int = 0) -> dict:
     """Compress the weights of `modules` (default: every submodule that directly owns bf16 / fp16 / fp32 / fp8
     parameters) into streams kept in HBM, decoded just before each module's forward.  All parameters are compressed
     in one `compress_batch` call and must be on one CUDA device.
@@ -290,10 +358,24 @@ def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = Fals
     ("out_bytes": the largest module decoded whole), and their plans are not in "plan_bytes" (their indexes are in
     "index_bytes").  The gathers use the plans' scratch (they run on the forward's stream, as the plans do), or with
     prefetch=True a buffer of its own.  The report gains "gather_modules" and "gather_bytes": memory that exists only
-    for gathers, i.e. the plans of their own plus a scratch of their own."""
+    for gathers, i.e. the plans of their own plus a scratch of their own.
+
+    matvec=N (1 .. MATVEC_MAX_TOKENS; 0, the default, changes nothing): a selected `torch.nn.Linear` (`matvecs`) whose
+    weight `DecodePlan.matvec_ok` accepts computes inputs of at most N rows (product of the leading dims) as
+    `DecodePlan.matvec` -- two launches, the weight neither decoded nor bound -- and larger inputs as before.  The
+    results of the small inputs are fp32 sums rounded once, so they differ from the dense model's in the last bits.
+    The bias of every `matvecs` module stays a dense parameter, whether or not its weight turns out eligible (that is
+    known only once the streams exist): against matvec=0 the report's "params", "dense_bytes" and "stream_bytes" lack
+    those biases, which stay resident dense.  Inputs of another dtype or device than the weight, and inputs inside an
+    autocast region, take the decode path whatever their size.  A tied weight keeps one stream; each owner has its
+    plan as before.  The shared output buffer stays, since larger inputs (prefill) decode into it.  The report gains
+    "matvec_modules" and "matvec_scratch_bytes" (one scratch for all of them, sized for the largest; the plans'
+    scratch when that is large enough).  ValueError together with prefetch=True."""
+    matvec = _check_matvec(matvec, prefetch)
     if getattr(module, _ATTR, None) is not None:
         raise ValueError("compress_module: this module is already compressed")
     modules, groups = select(module, modules)
+    groups = dense_biases(groups, matvec)
     params = [p for p, _ in groups]
     if not params:
         setattr(module, _ATTR, None)
@@ -306,18 +388,21 @@ def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = Fals
     # the streams move into one tight buffer; the batch's output buffer (sized by the bound) is dropped
     buf, streams = _pack({i: s for i, (p, s) in enumerate(zip(params, coded)) if s.numel() < p.numel() * p.element_size()}, dev)
     del coded, params
-    state, report = _resident_state(modules, groups, streams, [buf], dev, gather)
+    state, report = _resident_state(modules, groups, streams, [buf], dev, gather, matvec)
     _commit(module, state, prefetch)
-    return _with_prefetch(report, state, prefetch, gather)
+    return _with_prefetch(report, state, prefetch, gather, matvec)
 
 
-def _with_prefetch(report: dict, state, prefetch: bool, gather: bool = False) -> dict:
+def _with_prefetch(report: dict, state, prefetch: bool, gather: bool = False, matvec: int = 0) -> dict:
     if prefetch:
         report = dict(report, prefetch_out_bytes=state.prefetch[1].numel() if state is not None and state.prefetch else 0)
     if gather:
         own = state is not None and state.gather_scratch is not None and state.gather_scratch is not state.scratch
         report = dict(report, gather_modules=len(state.gathers) if state is not None else 0,
                       gather_bytes=(state.gather_plan_bytes + (state.gather_scratch.numel() if own else 0)) if state is not None else 0)
+    if matvec:
+        report = dict(report, matvec_modules=len(state.matvecs) if state is not None else 0,
+                      matvec_scratch_bytes=state.matvec_scratch_bytes if state is not None else 0)
     return report
 
 
@@ -341,6 +426,8 @@ def decompress_module(module: torch.nn.Module) -> None:
         for h in hooks:
             h.remove()
     for m, _, _, _ in state.gathers:
+        m.__dict__.pop("forward", None)
+    for m, _, _ in state.matvecs:
         m.__dict__.pop("forward", None)
     # each module's plan decodes into the shared buffer once more; its parameters are copied out of it, so the
     # model needs its dense size plus that buffer, not twice its dense size
@@ -373,6 +460,7 @@ def decompress_module(module: torch.nn.Module) -> None:
         params.update(reordered)
     state.entries.clear()
     state.gathers.clear()
+    state.matvecs.clear()
     delattr(module, _ATTR)
 
 
@@ -446,7 +534,7 @@ def _files(filenames) -> list:
     return [os.fspath(f) for f in filenames]
 
 
-def plan_load(module: torch.nn.Module, filenames, modules=None) -> LoadPlan:
+def plan_load(module: torch.nn.Module, filenames, modules=None, matvec: int = 0) -> LoadPlan:
     """The checks and choices of `load_module`, from the files' headers: ValueError naming the keys for a missing or
     unexpected key, a dtype or shape that differs, a non-persistent buffer on the meta device, and for a module that
     is already compressed."""
@@ -454,6 +542,7 @@ def plan_load(module: torch.nn.Module, filenames, modules=None) -> LoadPlan:
         raise ValueError("load_module: this module is already compressed")
     found = file_entries(_files(filenames))
     modules, groups = select(module, modules)
+    groups = dense_biases(groups, matvec)   # (matvec=N: those biases are read to dense tensors)
     plan = LoadPlan(modules, groups)
     group_of = {id(p): gi for gi, (p, _) in enumerate(groups)}
     by_key = {}
@@ -511,7 +600,7 @@ def plan_load(module: torch.nn.Module, filenames, modules=None) -> LoadPlan:
     return plan
 
 
-def _load_device(plan: LoadPlan, dev, gather: bool = False) -> tuple:
+def _load_device(plan: LoadPlan, dev, gather: bool = False, matvec: int = 0) -> tuple:
     """Every device step of load_module; the module is not touched.  -> (_Resident or None, report, dense tensors of
     plan.dense, {group index: dense tensor} of plain entries that did not compress, moved buffers of plan.moves)."""
     pipe = DecodePipe(dev)
@@ -581,7 +670,7 @@ def _load_device(plan: LoadPlan, dev, gather: bool = False) -> tuple:
             pipe.finish()
             moved = [m._buffers[n].to(dev) for m, n in plan.moves]
             if plan.groups:
-                state, report = _resident_state(plan.modules, plan.groups, dict(sorted(streams.items())), buffers, dev, gather)
+                state, report = _resident_state(plan.modules, plan.groups, dict(sorted(streams.items())), buffers, dev, gather, matvec)
             else:
                 state, report = None, dict(_EMPTY_REPORT)
         return state, report, dense, stayed, moved
@@ -592,7 +681,7 @@ def _load_device(plan: LoadPlan, dev, gather: bool = False) -> tuple:
 
 
 def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None, prefetch: bool = False,
-                gather: bool = False) -> dict:
+                gather: bool = False, matvec: int = 0) -> dict:
     """Load a checkpoint into `module` with the weights of `modules` kept compressed on `device`: the state
     `compress_module` leaves (same selection rules, hooks, plans and report), reached without a dense copy of those
     weights on the GPU.
@@ -627,17 +716,18 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None,
     and the batched decode's workspace; plain entries add one group at a time: its input, its streams' bound and the
     compress workspace.  A model loaded from .znn files never has its compressed weights dense on the device.
 
-    prefetch, gather: as for `compress_module`.
+    prefetch, gather, matvec: as for `compress_module`.
 
     -> the report of `compress_module`."""
+    matvec = _check_matvec(matvec, prefetch)
     dev = _cuda_device(device)
     if dev is None:
         raise ValueError(f"load_module: {device!r} is not a CUDA device")
     if dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
-    plan = plan_load(module, filenames, modules)
+    plan = plan_load(module, filenames, modules, matvec)
     try:
-        state, report, dense, stayed, moved = _load_device(plan, dev, gather)
+        state, report, dense, stayed, moved = _load_device(plan, dev, gather, matvec)
     except BaseException as e:
         traceback.clear_frames(e.__traceback__)   # the frames' locals would keep the call's device memory alive
         raise
@@ -659,7 +749,7 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None,
         setattr(module, _ATTR, None)
     else:
         _commit(module, state, prefetch)
-    return _with_prefetch(report, state, prefetch, gather)
+    return _with_prefetch(report, state, prefetch, gather, matvec)
 
 
 def save_module(module: torch.nn.Module, filename, metadata=None) -> None:
