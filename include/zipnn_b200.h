@@ -24,7 +24,10 @@
  *   - `threads`, `is_redata`, `checkThAfterPercent` have no GPU meaning and are absent;
  *   - all work is enqueued on the caller's CUDA stream; the device variants only
  *     synchronise to return `*out_len` (pass out_len == NULL to stay asynchronous and
- *     read the length from the stream header bytes [24:32] yourself).
+ *     read the length from the stream header bytes [24:32] yourself).  zipnn_b200_compress
+ *     waits for the length alone: it returns while the last kernels that write the stream
+ *     may still run, so the stream is ready for what is enqueued on the same CUDA stream
+ *     after the call (another stream must wait for that one first).
  *
  * The compressed stream is byte-for-byte the reference's stream.
  * Plain C types only: device/host pointers, sizes, `void*` for cudaStream_t.
@@ -55,6 +58,9 @@ int zipnn_b200_version(void);                 /* 0x000200 = 0.2.0 */
 const char* zipnn_b200_strerror(int status);
 int zipnn_b200_last_cuda_error(void);         /* cudaError_t of the last failing runtime call */
 int zipnn_b200_sm_count(void);                /* multiprocessor count of the current device   */
+/* Copy n <= 4096 bytes of device memory to host memory once the work enqueued on cuda_stream before the call
+ * is done (synchronises the stream, through a pinned block): the look at a stream's header that sizes a decode. */
+int zipnn_b200_peek(const void* d_src, size_t n, void* h_dst, void* cuda_stream);
 
 /* ---- sizing ------------------------------------------------------------------ */
 /* Upper bound of the whole stream (python header included). */

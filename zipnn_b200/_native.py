@@ -7,6 +7,7 @@ visible, the codec raises.  The library is built in-tree by `build()` (also call
 from __future__ import annotations
 
 import ctypes as C
+import functools
 import os
 import subprocess
 import threading
@@ -74,6 +75,8 @@ def build(force: bool = False, verbose: bool = False) -> str:
 def lib() -> C.CDLL:
     """Load the shared library (building it first if the sources are newer)."""
     global _lib
+    if _lib is not None:
+        return _lib
     with _lock:
         if _lib is None:
             try:
@@ -92,6 +95,7 @@ def lib() -> C.CDLL:
                 "zipnn_b200_strerror": (C.c_char_p, [i32]),
                 "zipnn_b200_last_cuda_error": (i32, []),
                 "zipnn_b200_sm_count": (i32, []),
+                "zipnn_b200_peek": (i32, [vp, sz, vp, vp]),
                 "zipnn_b200_launch_count": (C.c_ulonglong, []),
                 "zipnn_b200_compress_bound": (i32, [sz, i32, sz, sz, szp]),
                 "zipnn_b200_compress_workspace_size": (i32, [sz, i32, sz, szp]),
@@ -132,7 +136,7 @@ def lib() -> C.CDLL:
 
 
 EXPORTS = [
-    "zipnn_b200_version", "zipnn_b200_strerror", "zipnn_b200_last_cuda_error", "zipnn_b200_sm_count",
+    "zipnn_b200_version", "zipnn_b200_strerror", "zipnn_b200_last_cuda_error", "zipnn_b200_sm_count", "zipnn_b200_peek",
     "zipnn_b200_launch_count", "zipnn_b200_compress_bound", "zipnn_b200_compress_workspace_size",
     "zipnn_b200_decompress_workspace_size", "zipnn_b200_decompress_workspace_size_full", "zipnn_b200_compress",
     "zipnn_b200_compress_batch_workspace_size", "zipnn_b200_compress_batch", "zipnn_b200_decompress", "zipnn_b200_decompress_batch_workspace_size", "zipnn_b200_decompress_batch",
@@ -163,18 +167,22 @@ def require_cuda():
         raise ZipNNNativeError(E_CUDA, "no CUDA device: zipnn_b200 has no CPU fallback")
 
 
+# The sizes depend on the arguments alone: kept, so that a call in a loop asks the library once.
+@functools.lru_cache(maxsize=256)
 def compress_bound(n: int, num_buf: int, chunk: int, hdr_len: int) -> int:
     out = C.c_size_t(0)
     check(lib().zipnn_b200_compress_bound(n, num_buf, chunk, hdr_len, C.byref(out)))
     return out.value
 
 
+@functools.lru_cache(maxsize=256)
 def compress_workspace_size(n: int, num_buf: int, chunk: int) -> int:
     out = C.c_size_t(0)
     check(lib().zipnn_b200_compress_workspace_size(n, num_buf, chunk, C.byref(out)))
     return out.value
 
 
+@functools.lru_cache(maxsize=256)
 def decompress_workspace_size(orig: int, num_buf: int, chunk: int, full: bool = False) -> int:
     out = C.c_size_t(0)
     f = lib().zipnn_b200_decompress_workspace_size_full if full else lib().zipnn_b200_decompress_workspace_size

@@ -445,11 +445,18 @@ __device__ __forceinline__ void encode_scan_block(const uint32_t* __restrict__ s
   }
 }
 
+// The python header rides in the kernel's parameters (CUDA 12.1 and later take up to 32 KiB of them): no host-to-device
+// copy in front of the encode kernels.
+constexpr size_t kHdrMax = 4096;
+struct EncHeader {
+  uint8_t b[kHdrMax];
+};
+
 __global__ void __launch_bounds__(kScanThreads) k_encode_scan(const uint32_t* __restrict__ sizes, const uint8_t* __restrict__ types,
-                                                              int G, uint64_t K, const uint8_t* __restrict__ hdr_dev,
+                                                              int G, uint64_t K, const __grid_constant__ EncHeader hdr,
                                                               uint32_t hdr_len, uint8_t* out, uint64_t* item_off, Ctrl* ctrl,
                                                               const unsigned long long* __restrict__ partials) {
-  encode_scan_block(sizes, types, G, K, hdr_dev, hdr_len, out, item_off, ctrl, partials, blockIdx.x);
+  encode_scan_block(sizes, types, G, K, hdr.b, hdr_len, out, item_off, ctrl, partials, blockIdx.x);
 }
 
 // =====================================================================================

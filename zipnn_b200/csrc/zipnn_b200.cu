@@ -94,17 +94,144 @@ struct ScopedTimer {
   }
 };
 
-int sm_count_cached() {
-  static int cached = 0;
-  if (cached == 0) {
-    int dev = 0, n = 0;
-    if (cudaGetDevice(&dev) == cudaSuccess &&
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
-      cached = n;
-    else
-      return 132;
+// ---- launch plans: what the runtime says about a kernel, asked once per device ----------------------------------
+// Occupancy queries and cudaFuncSetAttribute cost host time on every call while the GPU waits for the launch, and
+// their answers only change with the device (an attribute set on one device does not hold on another).  So each is
+// asked once per (what, kernel, block size, shared memory, current device) and kept for the life of the process.
+struct PlanKey {
+  int what;  // kPlan* below
+  const void* fn;
+  int threads;
+  size_t smem;
+  int dev;
+  bool operator==(const PlanKey& o) const { return what == o.what && fn == o.fn && threads == o.threads && smem == o.smem && dev == o.dev; }
+};
+struct PlanKeyHash {
+  size_t operator()(const PlanKey& k) const {
+    size_t h = std::hash<const void*>()(k.fn);
+    for (size_t v : {(size_t)k.what, (size_t)k.threads, k.smem, (size_t)k.dev}) h = h * 1000003u ^ std::hash<size_t>()(v);
+    return h;
   }
-  return cached;
+};
+enum { kPlanSmCount = 0, kPlanBlocksPerSm, kPlanSmemAttr, kPlanFusedWarps };
+std::mutex g_launch_mu;
+std::unordered_map<PlanKey, int, PlanKeyHash> g_launch_plans;
+
+// compute() > 0 is kept; anything else is returned and asked again next time (a failing runtime call is not cached).
+template <typename F>
+int launch_plan(int what, const void* fn, int threads, size_t smem, F&& compute) {
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) dev = -1;
+  const PlanKey key{what, fn, threads, smem, dev};
+  {
+    std::lock_guard<std::mutex> lk(g_launch_mu);
+    auto it = g_launch_plans.find(key);
+    if (it != g_launch_plans.end()) return it->second;
+  }
+  const int v = compute(dev);
+  if (v > 0) {
+    std::lock_guard<std::mutex> lk(g_launch_mu);
+    g_launch_plans.emplace(key, v);
+  }
+  return v;
+}
+
+int sm_count_cached() {
+  const int n = launch_plan(kPlanSmCount, nullptr, 0, 0, [](int dev) {
+    int v = 0;
+    return dev >= 0 && cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess ? v : 0;
+  });
+  return n > 0 ? n : 132;
+}
+
+// CTAs of `threads` threads and `smem` bytes of dynamic shared memory resident on one SM of the current device (at
+// least 1).  A kernel that needs more than 48 KiB must have had smem_attr() first.
+template <typename Kernel>
+int resident_blocks(Kernel k, size_t smem, int threads = 32) {
+  const int nb = launch_plan(kPlanBlocksPerSm, (const void*)k, threads, smem, [&](int) {
+    int v = 0;
+    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k, threads, smem) == cudaSuccess ? v : 0;
+  });
+  return nb > 0 ? nb : 1;
+}
+
+// Raise the dynamic shared-memory limit of kernel k on the current device to `smem` (every caller passes the most
+// the kernel ever launches with).  false: the runtime refused.
+template <typename Kernel>
+bool smem_attr(Kernel k, size_t smem) {
+  return launch_plan(kPlanSmemAttr, (const void*)k, 0, smem, [&](int) {
+    return cuda_ok(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) ? 1 : 0;
+  }) > 0;
+}
+
+// ---- small pinned host blocks for the results a call reads back -------------------------------------------------
+// A device-to-host copy into pageable memory is staged by the driver and holds the host for longer; into pinned
+// memory it is one DMA, and the caller waits once, on the stream.  Blocks are taken per call and given back, so
+// calls on several threads never share one.
+constexpr size_t kPinnedBlock = 4096;
+std::mutex g_pinned_mu;
+std::vector<void*> g_pinned_free;
+
+struct PinnedBlock {
+  void* p = nullptr;
+  PinnedBlock() {
+    {
+      std::lock_guard<std::mutex> lk(g_pinned_mu);
+      if (!g_pinned_free.empty()) {
+        p = g_pinned_free.back();
+        g_pinned_free.pop_back();
+        return;
+      }
+    }
+    if (!cuda_ok(cudaHostAlloc(&p, kPinnedBlock, cudaHostAllocPortable))) p = nullptr;
+  }
+  ~PinnedBlock() {
+    if (!p) return;
+    std::lock_guard<std::mutex> lk(g_pinned_mu);
+    g_pinned_free.push_back(p);
+  }
+  PinnedBlock(const PinnedBlock&) = delete;
+  PinnedBlock& operator=(const PinnedBlock&) = delete;
+};
+
+// Events a call waits on (no timing), taken per call and given back.  An event can only be recorded on a stream of
+// the device it was made on, so they are kept per device.
+std::mutex g_wait_mu;
+std::unordered_map<int, std::vector<cudaEvent_t>> g_wait_free;
+
+struct WaitEvent {
+  cudaEvent_t e = nullptr;
+  int dev = -1;
+  WaitEvent() {
+    if (!cuda_ok(cudaGetDevice(&dev))) return;
+    {
+      std::lock_guard<std::mutex> lk(g_wait_mu);
+      std::vector<cudaEvent_t>& v = g_wait_free[dev];
+      if (!v.empty()) {
+        e = v.back();
+        v.pop_back();
+        return;
+      }
+    }
+    if (!cuda_ok(cudaEventCreateWithFlags(&e, cudaEventDisableTiming))) e = nullptr;
+  }
+  ~WaitEvent() {
+    if (!e) return;
+    std::lock_guard<std::mutex> lk(g_wait_mu);
+    g_wait_free[dev].push_back(e);
+  }
+  WaitEvent(const WaitEvent&) = delete;
+  WaitEvent& operator=(const WaitEvent&) = delete;
+};
+
+// `n` <= kPinnedBlock bytes of device memory at d_src to host memory at h_dst, after the work enqueued on st before.
+int read_back(void* h_dst, const void* d_src, size_t n, cudaStream_t st) {
+  PinnedBlock b;
+  if (!b.p) return ZIPNN_B200_E_CUDA;
+  ZB_CUDA(cudaMemcpyAsync(b.p, d_src, n, cudaMemcpyDeviceToHost, st));
+  ZB_CUDA(cudaStreamSynchronize(st));
+  memcpy(h_dst, b.p, n);
+  return ZIPNN_B200_OK;
 }
 
 // ---- tensor maps (TMA descriptors) ------------------------------------------------------
@@ -159,21 +286,14 @@ Knobs knobs() {
   return k;
 }
 
-template <typename Kernel>
-int resident_blocks(Kernel k, size_t smem, int threads = 32) {
-  int nb = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k, threads, smem) != cudaSuccess || nb < 1) nb = 1;
-  return nb;
-}
-
 // Most warps one CTA of k_huf_decode_fused<G, PB> can hold and still be resident: fused_max_warps by the shared-memory
 // arithmetic, confirmed by the occupancy calculator (which knows the per-CTA reserve and the allocation granularity).
 template <int G, int PB>
 int fused_cta_warps() {
-  static const int w = [] {
+  return launch_plan(kPlanFusedWarps, (const void*)k_huf_decode_fused<G, PB>, 0, 0, [](int) {
     constexpr int wmax = fused_max_warps<G, PB>();
     int best = 1;
-    if (cudaFuncSetAttribute(k_huf_decode_fused<G, PB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fused_smem_bytes<G>(PB, wmax)) == cudaSuccess) {
+    if (smem_attr(k_huf_decode_fused<G, PB>, fused_smem_bytes<G>(PB, wmax))) {
       for (int v = wmax; v > 1; v--) {
         int nb = 0;
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_huf_decode_fused<G, PB>, 32 * v, fused_smem_bytes<G>(PB, v)) == cudaSuccess && nb >= 1) {
@@ -184,8 +304,7 @@ int fused_cta_warps() {
     }
     (void)cudaGetLastError();
     return best;
-  }();
-  return w;
+  });
 }
 
 // Warps per CTA of the default launch of each variant, 0 for one one-warp CTA per chunk group.  From about 9 warps per SM
@@ -223,9 +342,12 @@ void launch_fused(DecodeCfg cfg, uint8_t* out, const TmaMaps& maps, uint64_t gro
     cfg.fused_claim = 1;
   } else {
     smem = fused_smem_bytes<G>(PB) + kn.smem_pad;
-    int nb = resident_blocks(k_huf_decode_fused<G, PB>, smem);
-    if (kn.warps_per_sm > 0) nb = std::min(nb, kn.warps_per_sm);
-    grid = mode == 1 ? (unsigned)groups : (unsigned)std::min<uint64_t>(groups, (uint64_t)nb * sms);
+    grid = (unsigned)groups;
+    if (mode == 0) {
+      int nb = resident_blocks(k_huf_decode_fused<G, PB>, smem);
+      if (kn.warps_per_sm > 0) nb = std::min(nb, kn.warps_per_sm);
+      grid = (unsigned)std::min<uint64_t>(groups, (uint64_t)nb * sms);
+    }
   }
   if (getenv("ZIPNN_B200_DEBUG"))
     fprintf(stderr, "[zipnn_b200] fused launch: G=%d PB=%d mode=%d warps_per_cta=%d grid=%u resident_warps_per_sm=%d\n", G, PB, mode, W, grid,
@@ -292,8 +414,8 @@ int dispatch_G(int G, F&& f) {
 
 int read_ctrl_error(void* d_ws, cudaStream_t st) {
   uint32_t err = 0;
-  ZB_CUDA(cudaMemcpyAsync(&err, d_ws, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-  ZB_CUDA(cudaStreamSynchronize(st));
+  const int rc = read_back(&err, d_ws, sizeof(uint32_t), st);
+  if (rc) return rc;
   if (err & kErrCorrupt) return ZIPNN_B200_E_CORRUPT;
   if (err & kErrUnsupported) return ZIPNN_B200_E_UNSUPPORTED;
   if (err & kErrWorkspace) return ZIPNN_B200_E_CAPACITY;
@@ -322,6 +444,11 @@ const char* zipnn_b200_strerror(int s) {
 
 int zipnn_b200_last_cuda_error(void) { return g_last_cuda_error.load(); }
 int zipnn_b200_sm_count(void) { return sm_count_cached(); }
+
+int zipnn_b200_peek(const void* d_src, size_t n, void* h_dst, void* cuda_stream) {
+  if (n > kPinnedBlock || (n && (!d_src || !h_dst))) return ZIPNN_B200_E_ARG;
+  return n ? read_back(h_dst, d_src, n, (cudaStream_t)cuda_stream) : ZIPNN_B200_OK;
+}
 unsigned long long zipnn_b200_launch_count(void) { return g_launches.load(); }
 
 void zipnn_b200_timing_enable(int on) {
@@ -461,18 +588,10 @@ int zipnn_b200_decompress(const void* d_body, size_t body_len, int num_buf, int 
     ZB_LAUNCHED();
   }
   if (use_sync) {
-    static bool attr_done[5] = {false, false, false, false, false};
     int rc = dispatch_G(G, [&](auto g) -> int {
       constexpr int GG = decltype(g)::value;
-      if (!attr_done[GG]) {
-        ZB_CUDA(cudaFuncSetAttribute(k_huf_decode_sync<GG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSyncSmemBytes));
-        attr_done[GG] = true;
-      }
-      static const int nb = [] {
-        int v = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_huf_decode_sync<GG>, kSyncThreads, kSyncSmemBytes) != cudaSuccess || v < 1) v = 1;
-        return v;
-      }();
+      if (!smem_attr(k_huf_decode_sync<GG>, kSyncSmemBytes)) return ZIPNN_B200_E_CUDA;
+      const int nb = resident_blocks(k_huf_decode_sync<GG>, kSyncSmemBytes, kSyncThreads);
       const unsigned grid = (unsigned)std::min<uint64_t>(4 * nitems, (uint64_t)nb * sm_count_cached());
       {
         ScopedTimer tp(kKParseTables, st);
@@ -644,16 +763,8 @@ static int batch_prepare(const std::vector<DecodeCfg>& cfgs, const std::vector<u
 // The sync decoder of a decode plan: record (create) or replay (run) of the segment starts.
 extern "C++" template <int M>
 int launch_sync_plan(const BatchCfg& B, const SegIndex& X, uint64_t items, cudaStream_t st) {
-  static bool attr_done = false;
-  if (!attr_done) {
-    ZB_CUDA(cudaFuncSetAttribute(k_huf_decode_sync_plan<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSyncSmemBytes));
-    attr_done = true;
-  }
-  static const int nb = [] {
-    int v = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_huf_decode_sync_plan<M>, kSyncThreads, kSyncSmemBytes) != cudaSuccess || v < 1) v = 1;
-    return v;
-  }();
+  if (!smem_attr(k_huf_decode_sync_plan<M>, kSyncSmemBytes)) return ZIPNN_B200_E_CUDA;
+  const int nb = resident_blocks(k_huf_decode_sync_plan<M>, kSyncSmemBytes, kSyncThreads);
   const unsigned blocks = (unsigned)std::min<uint64_t>(items, (uint64_t)nb * sm_count_cached());
   ScopedTimer tm(kKHufDecodeSync, st);
   k_huf_decode_sync_plan<M><<<blocks, kSyncThreads, kSyncSmemBytes, st>>>(B, X);
@@ -670,16 +781,8 @@ static int batch_decode(const BatchCfg& B, const BatchGrid& grid, cudaStream_t s
     const int rc = mode == kSyncRecord ? launch_sync_plan<kSyncRecord>(B, *X, grid.items, st) : launch_sync_plan<kSyncReplay>(B, *X, grid.items, st);
     if (rc) return rc;
   } else {
-    static bool attr_done = false;
-    if (!attr_done) {
-      ZB_CUDA(cudaFuncSetAttribute(k_huf_decode_sync_batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSyncSmemBytes));
-      attr_done = true;
-    }
-    static const int nb = [] {
-      int v = 0;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_huf_decode_sync_batch, kSyncThreads, kSyncSmemBytes) != cudaSuccess || v < 1) v = 1;
-      return v;
-    }();
+    if (!smem_attr(k_huf_decode_sync_batch, kSyncSmemBytes)) return ZIPNN_B200_E_CUDA;
+    const int nb = resident_blocks(k_huf_decode_sync_batch, kSyncSmemBytes, kSyncThreads);
     const unsigned blocks = (unsigned)std::min<uint64_t>(grid.items, (uint64_t)nb * sms);
     ScopedTimer tm(kKHufDecodeSync, st);
     k_huf_decode_sync_batch<<<blocks, kSyncThreads, kSyncSmemBytes, st>>>(B);
@@ -1142,16 +1245,8 @@ int zipnn_b200_decode_plan_run_shifted(const zipnn_b200_decode_plan* plan, int64
   PlanState s;
   if (!plan_state(plan, s) || (out_shift & 15)) return ZIPNN_B200_E_ARG;
   if (s.mode != kSyncReplay) return ZIPNN_B200_E_UNSUPPORTED;
-  static bool attr_done = false;
-  if (!attr_done) {
-    ZB_CUDA(cudaFuncSetAttribute(k_plan_replay_persistent, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPlanReplaySmemBytes));
-    attr_done = true;
-  }
-  static const int nb = [] {
-    int v = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_plan_replay_persistent, kSyncThreads, kPlanReplaySmemBytes) != cudaSuccess || v < 1) v = 1;
-    return v;
-  }();
+  if (!smem_attr(k_plan_replay_persistent, kPlanReplaySmemBytes)) return ZIPNN_B200_E_CUDA;
+  const int nb = resident_blocks(k_plan_replay_persistent, kPlanReplaySmemBytes, kSyncThreads);
   // more CTAs than units (or than the overflow CTAs a tensor may use) would only claim nothing
   const uint64_t limit = (uint64_t)nb * sm_count_cached();
   const uint64_t useful = std::max<uint64_t>(std::max<uint64_t>(1, s.grid.items + s.grid.tiles), s.grid.max_ovf);
@@ -1255,16 +1350,8 @@ int zipnn_b200_decode_plan_gather(const zipnn_b200_decode_plan* plan, int item, 
   // passes: the distinct chunks are at most min(n * span, K), `slots` per pass (a bound of n alone, not of the ids)
   const uint64_t most = n_ids > gi.K / g.span ? gi.K : std::min<uint64_t>(gi.K, n_ids * g.span);
   const uint64_t passes = (most + slots - 1) / slots;
-  static bool attr_done = false;
-  if (!attr_done) {
-    ZB_CUDA(cudaFuncSetAttribute(k_gather_decode, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPlanReplaySmemBytes));
-    attr_done = true;
-  }
-  static const int nb = [] {
-    int v = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_gather_decode, kSyncThreads, kPlanReplaySmemBytes) != cudaSuccess || v < 1) v = 1;
-    return v;
-  }();
+  if (!smem_attr(k_gather_decode, kPlanReplaySmemBytes)) return ZIPNN_B200_E_CUDA;
+  const int nb = resident_blocks(k_gather_decode, kPlanReplaySmemBytes, kSyncThreads);
   const int sms = sm_count_cached();
   const unsigned inv_blocks = (unsigned)std::max<uint64_t>(1, ((uint64_t)gi.G * gi.K + kGatherIndexThreads - 1) / kGatherIndexThreads);
   k_gather_index<<<1 + inv_blocks, kGatherIndexThreads, 0, st>>>(g);
@@ -1336,19 +1423,8 @@ extern "C++" template <int DT>
 int matvec_launch(const MatvecCfg& m, cudaStream_t st) {
   const auto decode = [&](auto nt) -> int {
     constexpr int NT = decltype(nt)::value;
-    // the shared-memory opt-in is per device: one bit per device ordinal, set once the attribute is
-    static std::atomic<uint64_t> attr_done{0};
-    int dev = 0;
-    ZB_CUDA(cudaGetDevice(&dev));
-    if (dev >= 64 || !((attr_done.load(std::memory_order_acquire) >> dev) & 1)) {
-      ZB_CUDA(cudaFuncSetAttribute(k_matvec<DT, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSyncSmemBytes));
-      if (dev < 64) attr_done.fetch_or(1ull << dev, std::memory_order_release);
-    }
-    static const int nb = [] {
-      int v = 0;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_matvec<DT, NT>, kSyncThreads, kSyncSmemBytes) != cudaSuccess || v < 1) v = 1;
-      return v;
-    }();
+    if (!smem_attr(k_matvec<DT, NT>, kSyncSmemBytes)) return ZIPNN_B200_E_CUDA;
+    const int nb = resident_blocks(k_matvec<DT, NT>, kSyncSmemBytes, kSyncThreads);
     const unsigned blocks = (unsigned)std::min<uint64_t>(4 * m.K, (uint64_t)nb * sm_count_cached());
     k_matvec<DT, NT><<<blocks, kSyncThreads, kSyncSmemBytes, st>>>(m);
     ZB_LAUNCHED();

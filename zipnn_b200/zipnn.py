@@ -19,6 +19,8 @@ reference as well), file-path arguments.
 from __future__ import annotations
 
 import ctypes as C
+import contextlib
+import functools
 import math
 import multiprocessing
 import os
@@ -71,6 +73,13 @@ def _xor_bytes(a, b):
     return np.bitwise_xor(_as_u8_numpy(a), _as_u8_numpy(b))
 
 
+@functools.lru_cache(maxsize=None)
+def _default_threads() -> int:
+    """min(cores, 16), the reference's default thread count, asked once: os.cpu_count() reads sysfs, which costs a
+    fraction of a millisecond on a large host, and a ZipNN object is often made per tensor."""
+    return min(multiprocessing.cpu_count(), 16)
+
+
 def _layout_for_dtype(code: int):
     """(bit_reorder, byte_reorder, num_buf) per dtype: reference zipnn/zipnn.py:788-815."""
     if code in (FLOAT8_E4M3FN, FLOAT8_E5M2):
@@ -119,7 +128,7 @@ class ZipNN:
         self.input_format = EnumFormat(input_format).value
         self.bytearray_dtype = bytearray_dtype
         self.is_monotonic = is_monotonic
-        self.threads = threads or min(multiprocessing.cpu_count(), 16)
+        self.threads = threads or _default_threads()
         self.compression_threshold = compression_threshold
         self.check_th_after_percent = check_th_after_percent
         self.byte_reorder = byte_reorder
@@ -289,7 +298,8 @@ class ZipNN:
         self._header[5], self._header[6], self._header[15] = byte_reorder, bit_reorder, code
 
         if fmt == EnumFormat.TORCH.value:
-            flat = _torch_flat_u8(data)
+            # a contiguous CUDA tensor goes as it is: the device call needs its address and byte size only
+            flat = data if data.is_cuda and data.is_contiguous() else _torch_flat_u8(data)
         elif fmt == EnumFormat.NUMPY.value:
             flat = torch.from_numpy(np.ascontiguousarray(data).reshape(-1).view(np.uint8))
         elif isinstance(data, torch.Tensor):   # byte format, bytes held in a (possibly CUDA) uint8 tensor
@@ -306,9 +316,9 @@ class ZipNN:
         return bytes(self._header) + self._ext_header, chunk
 
     def compress_bin(self, flat_u8, bit_reorder: int, byte_reorder: int, num_buf: int, shape):
-        """Header assembly + the native call (zipnn/zipnn.py:670-746).  `flat_u8` is a flat uint8
-        view of the input: a torch tensor (CPU or CUDA) or a numpy array (host bytes)."""
-        n = flat_u8.numel() if isinstance(flat_u8, torch.Tensor) else flat_u8.size
+        """Header assembly + the native call (zipnn/zipnn.py:670-746).  `flat_u8` holds the input's bytes: a flat
+        uint8 torch tensor (CPU or CUDA), a contiguous CUDA tensor of any dtype, or a numpy array (host bytes)."""
+        n = flat_u8.nbytes if isinstance(flat_u8, torch.Tensor) else flat_u8.size
         python_header, chunk = self._plan_header(n, num_buf, shape)
         self._last_plan = dict(header=python_header, num_buf=num_buf, bit_reorder=bit_reorder,
                                byte_reorder=byte_reorder, chunk=chunk, threshold=self.compression_threshold)
@@ -508,7 +518,12 @@ class ZipNN:
         if total < after_header:
             raise RuntimeError("corrupt ZipNN stream: truncated header")
         if isinstance(stream, torch.Tensor):
-            out_u8 = _decompress_device(stream[after_header:], num_buf, self._bit_reorder, self._byte_reorder, chunk, n)
+            tdt = torch_dtype_of_code(code) if self.input_format == EnumFormat.TORCH.value else None
+            if tdt is not None and math.prod(self.shape_bytes) * tdt.itemsize == n:
+                # the tensor itself is the destination: no views to make of the decoded bytes
+                out = torch.empty(self.shape_bytes, dtype=tdt, device=stream.device)
+                return _decompress_device(stream, num_buf, self._bit_reorder, self._byte_reorder, chunk, n, after_header, out)
+            out_u8 = _decompress_device(stream, num_buf, self._bit_reorder, self._byte_reorder, chunk, n, after_header)
         else:
             out_u8 = _decompress_host(stream[after_header:], num_buf, self._bit_reorder, self._byte_reorder, chunk, n,
                                       out=getattr(self, "_out", None))
@@ -846,6 +861,8 @@ class DecodePipe:
 def _as_stream(data):
     """CUDA/CPU uint8 tensor stays a tensor if on CUDA; everything else becomes a uint8 ndarray."""
     if isinstance(data, torch.Tensor):
+        if data.is_cuda and data.dtype == torch.uint8 and data.dim() == 1 and data.is_contiguous():
+            return data    # what compress returns: no view ops on the way in
         t = data.detach().contiguous().reshape(-1)
         t = t if t.dtype == torch.uint8 else t.view(torch.uint8)
         return t if t.is_cuda else t.numpy()
@@ -853,13 +870,32 @@ def _as_stream(data):
 
 
 def _peek(stream, nbytes: int) -> bytes:
+    """The first nbytes of a stream.  For a CUDA stream, one synchronising copy through the library's pinned block:
+    a tensor slice copied to the host costs several torch calls and a pageable copy while the GPU waits."""
     if isinstance(stream, torch.Tensor):
-        return stream[:nbytes].cpu().numpy().tobytes()
+        n = min(nbytes, stream.numel())
+        buf = C.create_string_buffer(n)
+        with _on_device(stream.device):
+            _native.check(_native.lib().zipnn_b200_peek(stream.data_ptr(), n, buf, _cuda_stream_handle(stream.device)))
+        return buf.raw
     return stream[:nbytes].tobytes()
 
 
-def _cuda_stream_handle() -> int:
-    return torch.cuda.current_stream().cuda_stream
+_raw_stream = getattr(torch._C, "_cuda_getCurrentRawStream", None)
+
+
+def _cuda_stream_handle(device=None) -> int:
+    """cudaStream_t of the current stream of `device` (default: the current device)."""
+    if _raw_stream is not None:
+        return _raw_stream(torch.cuda.current_device() if device is None or device.index is None else device.index)
+    return torch.cuda.current_stream(device).cuda_stream
+
+
+def _on_device(device):
+    """The native calls launch on the current device: make it `device` for the call, when it is not already."""
+    if device.index is None or device.index == torch.cuda.current_device():
+        return contextlib.nullcontext()
+    return torch.cuda.device(device)
 
 
 def _aligned(t: torch.Tensor) -> torch.Tensor:
@@ -868,19 +904,19 @@ def _aligned(t: torch.Tensor) -> torch.Tensor:
 
 def _compress_device(flat_u8: torch.Tensor, header: bytes, num_buf: int, bits_mode: int, bytes_mode: int,
                      chunk: int, threshold: float) -> torch.Tensor:
-    _native.require_cuda()
-    L = _native.lib()
+    """`flat_u8`: a contiguous CUDA tensor of any dtype, coded as its bytes."""
     flat_u8 = _aligned(flat_u8)
-    n = flat_u8.numel()
-    with torch.cuda.device(flat_u8.device):
-        bound = _native.compress_bound(n, num_buf, chunk, len(header))
-        out = torch.empty(bound, dtype=torch.uint8, device=flat_u8.device)
-        ws = torch.empty(_native.compress_workspace_size(n, num_buf, chunk), dtype=torch.uint8, device=flat_u8.device)
+    n = flat_u8.nbytes
+    dev = flat_u8.device
+    bound = _native.compress_bound(n, num_buf, chunk, len(header))
+    wsz = _native.compress_workspace_size(n, num_buf, chunk)
+    with _on_device(dev):
+        out = torch.empty(bound, dtype=torch.uint8, device=dev)
+        ws = torch.empty(wsz, dtype=torch.uint8, device=dev)
         out_len = C.c_size_t(0)
-        hdr = (C.c_char * len(header)).from_buffer_copy(header)
-        _native.check(L.zipnn_b200_compress(flat_u8.data_ptr() if n else None, n, hdr, len(header), num_buf, bits_mode,
-                                            bytes_mode, chunk, threshold, out.data_ptr(), bound, C.byref(out_len),
-                                            ws.data_ptr(), ws.numel(), _cuda_stream_handle()))
+        _native.check(_native.lib().zipnn_b200_compress(flat_u8.data_ptr() if n else None, n, header, len(header), num_buf,
+                                                        bits_mode, bytes_mode, chunk, threshold, out.data_ptr(), bound,
+                                                        C.byref(out_len), ws.data_ptr(), wsz, _cuda_stream_handle(dev)))
     return out[: out_len.value]
 
 
@@ -924,19 +960,22 @@ def _compress_device_batch(flats: list, plans: list) -> list:
 
 
 def _decompress_device(body: torch.Tensor, num_buf: int, bits_mode: int, bytes_mode: int, chunk: int,
-                       orig: int) -> torch.Tensor:
-    _native.require_cuda()
-    L = _native.lib()
-    with torch.cuda.device(body.device):
-        out = torch.empty(orig, dtype=torch.uint8, device=body.device)
+                       orig: int, body_off: int = 0, out: torch.Tensor = None) -> torch.Tensor:
+    """Decode body[body_off:] (a flat uint8 CUDA tensor) into `out` (a contiguous tensor of orig bytes on the same
+    device; by default a new uint8 one) and return `out`."""
+    dev = body.device
+    with _on_device(dev):
+        if out is None:
+            out = torch.empty(orig, dtype=torch.uint8, device=dev)
         if orig == 0:
             return out
         st = _native.E_CAPACITY
         for full in (False, True):   # the full workspace is only needed by unusual streams
-            ws = torch.empty(_native.decompress_workspace_size(orig, num_buf, chunk, full=full), dtype=torch.uint8,
-                             device=body.device)
-            st = L.zipnn_b200_decompress(body.data_ptr(), body.numel(), num_buf, bits_mode, bytes_mode, chunk, orig,
-                                         out.data_ptr(), ws.data_ptr(), ws.numel(), _cuda_stream_handle(), 1)
+            wsz = _native.decompress_workspace_size(orig, num_buf, chunk, full=full)
+            ws = torch.empty(wsz, dtype=torch.uint8, device=dev)
+            st = _native.lib().zipnn_b200_decompress(body.data_ptr() + body_off, body.numel() - body_off, num_buf, bits_mode,
+                                                     bytes_mode, chunk, orig, out.data_ptr(), ws.data_ptr(), wsz,
+                                                     _cuda_stream_handle(dev), 1)
             if st != _native.E_CAPACITY:
                 break
     if st == _native.E_CORRUPT:
