@@ -24,6 +24,7 @@ import functools
 import math
 import multiprocessing
 import os
+import threading
 
 import numpy as np
 import torch
@@ -568,6 +569,10 @@ class DecodePipe:
     _shared_pool = None
     _shared_streams = {}
     _slab_cache = []           # pinned slabs of finished pipes, reused by the next one
+    # the three above: pipes are built and released on a loader's threads at once.  Re-entrant: a pipe left in a
+    # reference cycle (its pending redo closures hold it) is released by __del__ on whatever thread the cyclic
+    # collector runs, which may be a thread inside this lock already
+    _shared_lock = threading.RLock()
 
     def __init__(self, device, streams: int = 4, stage_buffers: int = 4, copy_threads: int = 0):
         _native.require_cuda()
@@ -577,9 +582,10 @@ class DecodePipe:
         # side streams are process-wide per device: the caching allocator keeps one pool per stream, so a
         # second file loaded through fresh streams would pay cudaMalloc for every tensor again
         key = (self.device.index, streams)
-        if key not in DecodePipe._shared_streams:
-            DecodePipe._shared_streams[key] = [torch.cuda.Stream(self.device) for _ in range(streams)]
-        self._streams = DecodePipe._shared_streams[key]
+        with DecodePipe._shared_lock:
+            if key not in DecodePipe._shared_streams:
+                DecodePipe._shared_streams[key] = [torch.cuda.Stream(self.device) for _ in range(streams)]
+            self._streams = DecodePipe._shared_streams[key]
         self._body = [None] * streams      # per side stream, reused in stream order
         self._ws = [None] * streams
         self._stage = [None] * stage_buffers
@@ -592,15 +598,29 @@ class DecodePipe:
         # pinned slabs and reader threads are process-wide: page-locking 256 MiB costs tens to hundreds
         # of milliseconds, more than a small checkpoint takes to load
         nthreads = copy_threads or max(1, min(16, (multiprocessing.cpu_count() or 2) // 2))
-        if nthreads > 1 and DecodePipe._shared_pool is None:
-            from concurrent.futures import ThreadPoolExecutor
-            DecodePipe._shared_pool = ThreadPoolExecutor(max_workers=nthreads)
-        self._pool = DecodePipe._shared_pool if nthreads > 1 else None
-        # only slabs of the current size: SLAB_BYTES may have changed since they were cached
-        DecodePipe._slab_cache[:] = [sl for sl in DecodePipe._slab_cache if sl.numel() == self.SLAB_BYTES]
-        for j in range(stage_buffers):
-            if DecodePipe._slab_cache:
-                self._stage[j] = DecodePipe._slab_cache.pop()
+        with DecodePipe._shared_lock:
+            if nthreads > 1 and DecodePipe._shared_pool is None:
+                from concurrent.futures import ThreadPoolExecutor
+                DecodePipe._shared_pool = ThreadPoolExecutor(max_workers=nthreads)
+            self._pool = DecodePipe._shared_pool if nthreads > 1 else None
+        for j, sl in enumerate(DecodePipe._take_slabs(self.SLAB_BYTES, stage_buffers)):
+            self._stage[j] = sl
+
+    @staticmethod
+    def _take_slabs(nbytes: int, most: int) -> list:
+        """Up to `most` cached slabs of `nbytes` bytes, each handed to this caller alone.  Slabs of another size
+        are dropped: SLAB_BYTES may have changed since they were cached."""
+        with DecodePipe._shared_lock:
+            cache = DecodePipe._slab_cache
+            cache[:] = [sl for sl in cache if sl.numel() == nbytes]
+            return [cache.pop() for _ in range(min(most, len(cache)))]
+
+    @staticmethod
+    def _give_slab(sl: torch.Tensor) -> None:
+        """Keep a slab no pipe uses any more for the next one (at most 8 are kept)."""
+        with DecodePipe._shared_lock:
+            if len(DecodePipe._slab_cache) < 8:
+                DecodePipe._slab_cache.append(sl)
 
     # ---- host side: fill a pinned slab
     def _fill_from_host(self, dst: torch.Tensor, src: torch.Tensor):
@@ -845,8 +865,8 @@ class DecodePipe:
             if evt is not None:
                 evt.synchronize()
         for j, sl in enumerate(self._stage):
-            if sl is not None and sl.numel() == self.SLAB_BYTES and len(DecodePipe._slab_cache) < 8:
-                DecodePipe._slab_cache.append(sl)
+            if sl is not None and sl.numel() == self.SLAB_BYTES:
+                DecodePipe._give_slab(sl)
             self._stage[j] = None
             self._stage_evt[j] = None
 
