@@ -262,6 +262,27 @@ int zipnn_b200_decode_plan_matvec(const zipnn_b200_decode_plan* plan, int item, 
                                   const void* d_x, size_t x_stride, size_t n_tokens, const void* d_bias, void* d_y,
                                   size_t y_stride, void* d_scratch, size_t scratch_bytes, void* cuda_stream);
 
+/* _matmul: what _matvec computes, for up to ZIPNN_B200_MATMUL_MAX_TOKENS rows of x, on tensor cores (mma.m16n8k16
+ * with fp32 accumulation): the dense W is never written or read back.  Arguments, eligible items, the first call's
+ * read of the chunk modes, the scratch and stream rules and the error reporting are those of _matvec.  bf16 and fp16
+ * only: ZIPNN_B200_MATVEC_FP32 answers E_UNSUPPORTED, and the caller decodes the item as before.
+ * Launches: 2 whatever n_tokens and the shapes are -- the plan run's per-bitstream replay decoder, whose fused merge
+ * hands each 16 bytes it forms to the tensor cores as a fragment of 8 rows x 32 columns of W, and writes one fp32
+ * partial sum per (bitstream, tile of 8 rows it touches, token, row) to d_scratch, and a reduction that adds each row's
+ * partial sums in ascending element order, adds the bias and rounds once.  No atomics on floats, no copy, memset or
+ * synchronisation: capturable in a CUDA graph, replayable with new x, and two calls with the same inputs give the same
+ * bits.  The tensor cores' fp32 sums are not rounded to nearest at every addition, so a result may differ from
+ * _matvec's in the last bits.  n_tokens == 0 launches nothing.  x must be finite: an infinity in x can give NaN in a
+ * row that straddles two bitstreams where the dense product gives an infinity.
+ * Host-side rejections launch and write nothing: E_ARG as for _matvec, with ZIPNN_B200_MATMUL_MAX_TOKENS as the row
+ * limit and scratch_bytes below _matmul_scratch_size; E_UNSUPPORTED for fp32 and for every item _matvec refuses. */
+#define ZIPNN_B200_MATMUL_MAX_TOKENS 64
+int zipnn_b200_decode_plan_matmul_scratch_size(const zipnn_b200_decode_plan* plan, int item, int dtype,
+                                               size_t in_features, size_t n_tokens, size_t* out);
+int zipnn_b200_decode_plan_matmul(const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features,
+                                  const void* d_x, size_t x_stride, size_t n_tokens, const void* d_bias, void* d_y,
+                                  size_t y_stride, void* d_scratch, size_t scratch_bytes, void* cuda_stream);
+
 /* ---- stage 1 alone ------------------------------------------------------------ */
 /* d_planes: num_buf planes of `stride` bytes each; plane g receives byte g of every element
  * of the (optionally rotated) input.  Lengths as in the reference: n/num_buf, the first

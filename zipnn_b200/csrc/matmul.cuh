@@ -1,0 +1,223 @@
+// matmul.cuh -- y = x W^T for up to 64 rows of x on tensor cores, with W a whole-tensor item of a decode plan that is
+// never written dense.
+//
+// y[t][o] = sum_i x[t][i] * W[o][i] (+ bias[o]), t < n_tokens <= kMatmulMaxTokens, W row-major [out][in] of bf16 or
+// fp16, every chunk of it in fused mode (the host checks, as for the matvec).  Two launches per call:
+//
+//   k_matmul         sync_process in replay mode, one CTA per coded bitstream, as k_matvec: only the epilogue differs.
+//                    `MatmulEp::quarter` feeds the 16-byte vectors ZB_FUSED_VECTOR forms to mma.m16n8k16 as B fragments.
+//   k_matmul_reduce  one thread per (token, output row) adds the row's partial sums in ascending element order, adds the
+//                    bias, rounds once to the output type and stores.
+//
+// Fragments.  The quarter plane of a bitstream is a contiguous element range of W.  It is cut into row tiles of 8
+// consecutive W rows (the first tile starts at the quarter's first row) and each tile into column steps of 32.  In a
+// step, lane (g = lane >> 2, j = lane & 3) forms the vector of row g, columns 8j .. 8j + 7.  Its four registers are the
+// B fragments (n = g) of two k16 mma steps s = 0, 1 with the k order
+//     kappa = 2j + b      -> column 8j + 4s + b,        kappa = 2j + 8 + b  -> column 8j + 4s + 2 + b      (b = 0, 1)
+// so register 2s is b0b1 and register 2s + 1 is b2b3 of step s, with no shuffle.  The A fragments under the same
+// order are one 16-byte load of x per token row: columns 8j .. 8j + 7 of tokens g and g + 8 of each 16-row tile, whose
+// words 2s and 2s + 1 are a0a1 / a4a5 (token g) and a2a3 / a6a7 (token g + 8).  D is [token][W row of the tile].
+//
+// Masking.  A vector outside the quarter's range (partial first and last rows, columns past `in`) is zero and reads no
+// shared memory; x columns past `in` and tokens past n_tokens are zero fragments and are not loaded.  The zero B
+// vectors of a row that straddles two quarters meet real x, so an infinite x there gives NaN where the dense product
+// gives an infinity: x must be finite.
+//
+// Bank conflicts.  The 8 rows of a tile lie `in` bytes apart in the quarter plane (one byte per element): with `in` a
+// multiple of 128 (every llama shape) the 8 lanes that read the same columns of 8 rows hit the same banks, 8 wavefronts
+// for an 8-byte load instead of 2.  So the steps go in groups of 4: in its load i of a group, lane (g, j) forms the
+// vector of step (i + g) & 3, which puts the 4 rows of each half warp in 4 different 32-byte column ranges, and two
+// rounds of selects move the vectors back to step order.
+//
+// Work split and partial sums.  The warps take the column groups of a tile in turn (warp w: groups w, w + 8, ...) and
+// keep 4 fp32 accumulators per lane per 16-token tile in registers.  At the end of a tile they add up in shared memory
+// (S.sbuf: the staged bitstream is dead once the quarter plane is emitted), warp by warp in a fixed order, and the CTA
+// writes one fp32 per (row of the tile, token) to part[(((chunk * 4 + bitstream) * rt + tile) * n_tokens + t) * 8 +
+// row].  Every slot the reduce reads is written by exactly one CTA in every call; no atomics, no memset, and the order
+// of every addition is fixed by the shapes, so two calls with the same inputs give the same bits at any grid size.
+#pragma once
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
+#include "matvec.cuh"
+
+namespace zb {
+
+constexpr int kMatmulMaxTokens = 64;
+constexpr int kMatmulTileRows = 8;    // W rows per tile: n of the mma
+constexpr int kMatmulGroupCols = 128;  // 4 column steps of 32
+
+struct MatmulCfg {
+  const DecodeCfg* cfg;   // the item's piece, in plan memory
+  SegEntry* seg;          // the piece's segment index
+  uint32_t* error;        // the plan's error word
+  const void* x;
+  const void* bias;       // or nullptr
+  void* y;
+  float* part;            // the partial sums (scratch)
+  uint64_t in, out;       // features
+  uint64_t xs, ys;        // row strides of x and y, in elements
+  uint64_t ce, total, K;  // elements of a full chunk and of the tensor; chunks
+  uint32_t nt, rt;        // tokens; row tiles per quarter in the slot layout
+};
+
+// Row tiles a quarter of q elements may touch, wherever it starts (rows of `in` elements).
+__host__ __device__ inline uint64_t matmul_quarter_tiles(uint64_t q, uint64_t in, uint64_t out) {
+  return (matvec_block_rows(q, in, out) + kMatmulTileRows - 1) / kMatmulTileRows;
+}
+
+template <int DT>
+__device__ __forceinline__ void mma_16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+  if constexpr (DT == kMvBf16) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+  } else {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+  }
+}
+
+// MT: 16-token tiles a lane accumulates, n_tokens rounded up to 16, 32 or 64.  Tiles wholly past n_tokens are skipped.
+template <int DT, int MT>
+struct MatmulEp {
+  static constexpr bool on = true;
+  MatmulCfg m;
+
+  template <int G>
+  __device__ __forceinline__ void quarter(const SyncShared& S, uint64_t c, int stream, uint32_t out_off, uint32_t count, bool rot) const {
+    static_assert(G == 2, "16-bit weights: two byte planes");
+    constexpr int TT = 16 * MT;
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint32_t g = (uint32_t)lane >> 2, j = (uint32_t)lane & 3u;
+    const uint64_t in = m.in;
+    const uint64_t e0 = c * m.ce + out_off, e1 = e0 + count;
+    const uint64_t r_first = e0 / in;
+    const uint32_t tiles = (uint32_t)((e1 - 1) / in - r_first) / kMatmulTileRows + 1;
+    const uint32_t groups = (uint32_t)((in + kMatmulGroupCols - 1) / kMatmulGroupCols);
+    const uint32_t mts = min((uint32_t)MT, (m.nt + 15u) >> 4);  // token tiles with a token in them
+    const uint8_t* const xb = reinterpret_cast<const uint8_t*>(m.x);
+    float* const red = reinterpret_cast<float*>(const_cast<uint8_t*>(S.sbuf));  // [warp][row][TT]
+    float* const slots = m.part + (c * 4 + (uint32_t)stream) * m.rt * m.nt * kMatmulTileRows;
+    const uint32_t rg = g & 3u;
+    for (uint32_t tile = 0; tile < tiles; tile++) {
+      const uint64_t rowe = (r_first + (uint64_t)tile * kMatmulTileRows + g) * in;  // this lane's row, as an element
+      float acc[MT][4];
+#pragma unroll
+      for (int mt = 0; mt < MT; mt++) acc[mt][0] = acc[mt][1] = acc[mt][2] = acc[mt][3] = 0.f;
+      for (uint32_t grp = (uint32_t)wid; grp < groups; grp += kSyncThreads / 32) {
+        const uint64_t k0 = (uint64_t)grp * kMatmulGroupCols;
+        uint32_t v[4][4];
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+          const uint64_t col = k0 + 32u * (((uint32_t)i + g) & 3u) + 8u * j;
+          const uint64_t e = rowe + col;
+          if (col < in && e >= e0 && e < e1) {
+            const uint32_t vo = (uint32_t)(e - e0) * 2u;
+            uint32_t fv[4];  // (a plain name: the macro's own loop index is `i`)
+            ZB_FUSED_VECTOR(G, S, out_off, vo, rot, fv);
+#pragma unroll
+            for (int q = 0; q < 4; q++) v[i][q] = fv[q];
+          } else {
+            v[i][0] = v[i][1] = v[i][2] = v[i][3] = 0u;
+          }
+        }
+        // v[i] holds step (i + rg) & 3: rotate by rg so that v[t] holds step t
+        uint32_t u[4][4];
+#pragma unroll
+        for (int t = 0; t < 4; t++)
+#pragma unroll
+          for (int q = 0; q < 4; q++) u[t][q] = (rg & 1u) ? v[(t + 3) & 3][q] : v[t][q];
+#pragma unroll
+        for (int t = 0; t < 4; t++)
+#pragma unroll
+          for (int q = 0; q < 4; q++) v[t][q] = (rg & 2u) ? u[(t + 2) & 3][q] : u[t][q];
+#pragma unroll
+        for (int t = 0; t < 4; t++) {
+          const uint64_t kc = k0 + 32u * (uint32_t)t;
+          if (kc >= in) break;  // (uniform)
+          const uint64_t col = kc + 8u * j;
+          const bool cv = col < in;
+#pragma unroll
+          for (int mt = 0; mt < MT; mt++) {
+            if ((uint32_t)mt >= mts) break;  // (uniform)
+            const uint32_t t0 = 16u * (uint32_t)mt + g, t1 = t0 + 8u;
+            uint4 xa = make_uint4(0u, 0u, 0u, 0u), xc = xa;
+            if (cv && t0 < m.nt) xa = __ldg(reinterpret_cast<const uint4*>(xb + ((uint64_t)t0 * m.xs + col) * 2u));
+            if (cv && t1 < m.nt) xc = __ldg(reinterpret_cast<const uint4*>(xb + ((uint64_t)t1 * m.xs + col) * 2u));
+            mma_16816<DT>(acc[mt], xa.x, xc.x, xa.y, xc.y, v[t][0], v[t][1]);
+            mma_16816<DT>(acc[mt], xa.z, xc.z, xa.w, xc.w, v[t][2], v[t][3]);
+          }
+        }
+      }
+      // D: acc[mt] = {[token 16mt + g][row 2j], [16mt + g][2j + 1], [16mt + g + 8][2j], [16mt + g + 8][2j + 1]}
+#pragma unroll
+      for (int mt = 0; mt < MT; mt++) {
+        float* const r0 = red + ((uint32_t)wid * kMatmulTileRows + 2u * j) * TT + 16u * (uint32_t)mt + g;
+        r0[0] = acc[mt][0];
+        r0[TT] = acc[mt][1];
+        r0[8] = acc[mt][2];
+        r0[TT + 8] = acc[mt][3];
+      }
+      __syncthreads();
+      float* const out = slots + (uint64_t)tile * m.nt * kMatmulTileRows;
+      for (uint32_t idx = threadIdx.x; idx < m.nt * kMatmulTileRows; idx += kSyncThreads) {
+        const uint32_t row = idx & (kMatmulTileRows - 1), t = idx / kMatmulTileRows;
+        float s = 0.f;
+#pragma unroll
+        for (int w = 0; w < kSyncThreads / 32; w++) s += red[((uint32_t)w * kMatmulTileRows + row) * TT + t];
+        out[idx] = s;
+      }
+      __syncthreads();  // the sums are read before the next tile writes them
+    }
+  }
+};
+static_assert(sizeof(((SyncShared*)0)->sbuf) >= (kSyncThreads / 32) * kMatmulTileRows * kMatmulMaxTokens * sizeof(float),
+              "the warps' sums of a tile fit in the stream buffer");
+
+// One CTA per coded bitstream of the item (every chunk is fused: its one coded item is the top byte plane).
+template <int DT, int MT>
+__global__ void __launch_bounds__(kSyncThreads, 3) k_matmul(MatmulCfg m) {
+  extern __shared__ __align__(1024) unsigned char smem_raw[];
+  const SyncCarve cv = sync_carve(smem_raw);
+  SyncShared& S = *cv.S;
+  const DecodeCfg& cfg = *m.cfg;
+  const MatmulEp<DT, MT> ep{m};
+  const uint64_t works = 4ull * cfg.ctrl->huf_count;
+  for (uint64_t work = blockIdx.x; work < works; work += gridDim.x) {
+    __syncthreads();  // the previous bitstream's shared state is dead
+    sync_process<2, false, kSyncReplay, false, MatmulEp<DT, MT>>(cfg, nullptr, S, cv.lut, cv.lut_s, work, m.seg + work * kSyncThreads, nullptr,
+                                                                  &ep);
+  }
+}
+
+template <int DT>
+__global__ void __launch_bounds__(256) k_matmul_reduce(MatmulCfg m) {
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    const uint32_t e = *(volatile uint32_t*)&m.cfg->ctrl->error;  // a decode error of this call
+    if (e) atomicOr(m.error, e);
+  }
+  const uint64_t idx = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (idx >= m.out * m.nt) return;
+  const uint64_t t = idx / m.out, o = idx - t * m.out;
+  float s = 0.f;
+  for (uint64_t e = o * m.in; e < (o + 1) * m.in;) {
+    const uint64_t c = e / m.ce;
+    const uint64_t q = (c == m.K - 1 ? m.total - c * m.ce : m.ce) / 4;
+    const uint64_t st = (e - c * m.ce) / q;
+    const uint64_t qs = c * m.ce + st * q;
+    const uint64_t r = o - qs / m.in;  // the row within the quarter's rows
+    s += m.part[((((c * 4 + st) * m.rt + r / kMatmulTileRows) * m.nt + t) * kMatmulTileRows) + r % kMatmulTileRows];
+    e = qs + q;
+  }
+  if (DT == kMvBf16) {
+    if (m.bias) s += __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(m.bias)[o]);
+    reinterpret_cast<__nv_bfloat16*>(m.y)[t * m.ys + o] = __float2bfloat16_rn(s);
+  } else {
+    if (m.bias) s += __half2float(reinterpret_cast<const __half*>(m.bias)[o]);
+    reinterpret_cast<__half*>(m.y)[t * m.ys + o] = __float2half_rn(s);
+  }
+}
+
+}  // namespace zb

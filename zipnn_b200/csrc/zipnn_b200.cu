@@ -20,6 +20,7 @@
 #include "decode_sync.cuh"
 #include "encode.cuh"
 #include "gather.cuh"
+#include "matmul.cuh"
 #include "matvec.cuh"
 #include "stage1.cuh"
 
@@ -1500,6 +1501,99 @@ int zipnn_b200_decode_plan_matvec(const zipnn_b200_decode_plan* plan, int item, 
   if (dtype == kMvBf16) return matvec_launch<kMvBf16>(m, st);
   if (dtype == kMvFp16) return matvec_launch<kMvFp16>(m, st);
   return matvec_launch<kMvFp32>(m, st);
+}
+
+// ---- matmul: x W^T for up to 64 rows of x on tensor cores, no dense W (matmul.cuh) --------------------------------
+// Scratch: [4 K quarters][rt row tiles][n_tokens][8 rows] fp32 partial sums.
+namespace {
+// matvec_item's checks, and 16-bit weights only: fp32 would need TF32 or a split scheme, so it is left to the decode.
+int matmul_item(const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, cudaStream_t st, PlanState& s, GatherItem& gi,
+                MatvecGeom& M, uint32_t& rt) {
+  const int rc = matvec_item(plan, item, dtype, in_features, st, s, gi, M);
+  if (rc) return rc;
+  if (dtype == kMvFp32) return ZIPNN_B200_E_UNSUPPORTED;
+  rt = (uint32_t)matmul_quarter_tiles(std::min<uint64_t>(M.ce, M.total) / 4, M.in, M.out);
+  return ZIPNN_B200_OK;
+}
+size_t matmul_scratch_bytes(const GatherItem& gi, uint32_t rt, size_t n_tokens) {
+  return (size_t)4 * gi.K * rt * n_tokens * kMatmulTileRows * sizeof(float);
+}
+
+extern "C++" template <int DT>
+int matmul_launch(const MatmulCfg& m, cudaStream_t st) {
+  const auto decode = [&](auto mt) -> int {
+    constexpr int MT = decltype(mt)::value;
+    if (!smem_attr(k_matmul<DT, MT>, kSyncSmemBytes)) return ZIPNN_B200_E_CUDA;
+    const int nb = resident_blocks(k_matmul<DT, MT>, kSyncSmemBytes, kSyncThreads);
+    const unsigned blocks = (unsigned)std::min<uint64_t>(4 * m.K, (uint64_t)nb * sm_count_cached());
+    k_matmul<DT, MT><<<blocks, kSyncThreads, kSyncSmemBytes, st>>>(m);
+    ZB_LAUNCHED();
+    return ZIPNN_B200_OK;
+  };
+  int rc;
+  if (m.nt <= 16) rc = decode(std::integral_constant<int, 1>{});
+  else if (m.nt <= 32) rc = decode(std::integral_constant<int, 2>{});
+  else rc = decode(std::integral_constant<int, 4>{});
+  if (rc) return rc;
+  k_matmul_reduce<DT><<<(unsigned)((m.out * m.nt + 255) / 256), 256, 0, st>>>(m);
+  ZB_LAUNCHED();
+  return ZIPNN_B200_OK;
+}
+}  // namespace
+
+static_assert(kMatmulMaxTokens == ZIPNN_B200_MATMUL_MAX_TOKENS, "the header's constant is the kernels'");
+
+int zipnn_b200_decode_plan_matmul_scratch_size(const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, size_t n_tokens,
+                                               size_t* out) {
+  if (!out || n_tokens > (size_t)kMatmulMaxTokens) return ZIPNN_B200_E_ARG;
+  PlanState s;
+  GatherItem gi;
+  MatvecGeom M;
+  uint32_t rt;
+  const int rc = matmul_item(plan, item, dtype, in_features, nullptr, s, gi, M, rt);
+  if (rc) return rc;
+  *out = matmul_scratch_bytes(gi, rt, n_tokens);
+  return ZIPNN_B200_OK;
+}
+
+int zipnn_b200_decode_plan_matmul(const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, const void* d_x, size_t x_stride,
+                                  size_t n_tokens, const void* d_bias, void* d_y, size_t y_stride, void* d_scratch, size_t scratch_bytes,
+                                  void* cuda_stream) {
+  if (n_tokens > (size_t)kMatmulMaxTokens) return ZIPNN_B200_E_ARG;
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  PlanState s;
+  GatherItem gi;
+  MatvecGeom M;
+  uint32_t rt;
+  {
+    const int rc = matmul_item(plan, item, dtype, in_features, st, s, gi, M, rt);
+    if (rc) return rc;
+  }
+  if (n_tokens == 0) return ZIPNN_B200_OK;
+  if (!d_x || !d_y || !d_scratch || ((uintptr_t)d_x & 15) || ((uintptr_t)d_scratch & 255) || ((uintptr_t)d_y % M.esize) ||
+      ((uintptr_t)d_bias % M.esize))
+    return ZIPNN_B200_E_ARG;
+  if (n_tokens > 1 && ((x_stride * M.esize) % 16 || x_stride < M.in || y_stride < M.out)) return ZIPNN_B200_E_ARG;
+  if (scratch_bytes < matmul_scratch_bytes(gi, rt, n_tokens)) return ZIPNN_B200_E_ARG;
+  MatmulCfg m;
+  m.cfg = s.B.cfgs + gi.piece;
+  m.seg = s.X.seg + gi.seg_base;
+  m.error = s.B.error_out;
+  m.x = d_x;
+  m.bias = d_bias;
+  m.y = d_y;
+  m.part = (float*)d_scratch;
+  m.in = M.in;
+  m.out = M.out;
+  m.xs = x_stride;
+  m.ys = y_stride;
+  m.ce = M.ce;
+  m.total = M.total;
+  m.K = gi.K;
+  m.nt = (uint32_t)n_tokens;
+  m.rt = rt;
+  if (dtype == kMvBf16) return matmul_launch<kMvBf16>(m, st);
+  return matmul_launch<kMvFp16>(m, st);
 }
 
 int zipnn_b200_split(const void* d_in, size_t n, int num_buf, int bits_mode, void* d_planes, size_t stride,

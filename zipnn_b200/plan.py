@@ -27,7 +27,9 @@ _HEAD = HEADER_LEN + 1 + 9 * 255   # the 32-byte header and the longest packed s
 _ALIGN = 16
 GATHER_SLOTS = 64   # chunk slots of gather's default scratch: 16 MiB for 256 KiB chunks
 MATVEC_MAX_TOKENS = _native.MATVEC_MAX_TOKENS
+MATMUL_MAX_TOKENS = _native.MATMUL_MAX_TOKENS
 _MATVEC_DTYPES = {torch.bfloat16: 0, torch.float16: 1, torch.float32: 2}   # ZIPNN_B200_MATVEC_*
+_MATMUL_DTYPES = (torch.bfloat16, torch.float16)
 
 
 def _round(n: int, a: int) -> int:
@@ -166,8 +168,10 @@ class DecodePlan:
         self._offs = [(o, p.nbytes, p.dtype, p.shape) for p, o in zip(parsed, offs)]
         self._gather_scratch = None   # gather's default scratch, grown on demand
         self._matvec = _native.lib().zipnn_b200_decode_plan_matvec
-        self._matvec_scratch = None   # matvec's default scratch, grown on demand
+        self._matmul = _native.lib().zipnn_b200_decode_plan_matmul
+        self._scratches = {}          # "matvec" / "matmul" -> that call's default scratch, grown on demand
         self._matvec_ok = {}          # (output, in_features) -> eligible?
+        self._matmul_ok = {}
 
     def run(self) -> list:
         """Enqueue the decode on the current CUDA stream (launches only) and return `.outputs`."""
@@ -317,18 +321,60 @@ class DecodePlan:
                  bytes.  It holds nothing between calls: calls (and plan runs) that share it must be ordered on one
                  stream.  Default: a buffer kept by the plan.
         -> out.  ValueError for an output `matvec_ok` refuses.  Works without the plan's output buffer."""
+        return self._product("matvec", k, x, bias, out, scratch)
+
+    def _matmul_size(self, k: int, in_features: int, n_tokens: int) -> tuple:
+        dt, _ = self._matvec_item(k)
+        out = C.c_size_t(0)
+        if dt not in _MATMUL_DTYPES or in_features <= 0:
+            return _native.E_UNSUPPORTED, 0
+        with torch.cuda.device(self.device):
+            rc = _native.lib().zipnn_b200_decode_plan_matmul_scratch_size(self._ref, k, _MATVEC_DTYPES[dt], int(in_features), int(n_tokens),
+                                                                          C.byref(out))
+        return rc, out.value
+
+    def matmul_ok(self, k: int, in_features: int) -> bool:
+        """Can `matmul` multiply by output `k` seen as rows of `in_features` elements?  What `matvec_ok` accepts, for
+        bf16 and fp16 outputs only (an fp32 output decodes).  Never raises for an output that exists."""
+        dt, _ = self._matvec_item(k)
+        if dt not in _MATMUL_DTYPES or not self.matvec_ok(k, in_features):
+            return False
+        if (k, in_features) not in self._matmul_ok:
+            self._matmul_ok[(k, in_features)] = self._matmul_size(k, in_features, 1)[0] == _native.OK
+        return self._matmul_ok[(k, in_features)]
+
+    def matmul_scratch_bytes(self, k: int, in_features: int, n_tokens: int = MATMUL_MAX_TOKENS) -> int:
+        """Bytes of a matmul scratch for output `k`, rows of `in_features` elements and `n_tokens` rows of x."""
+        rc, n = self._matmul_size(k, in_features, n_tokens)
+        _native.check(rc)
+        return n
+
+    def matmul(self, k: int, x: torch.Tensor, bias: torch.Tensor = None, out: torch.Tensor = None,
+               scratch: torch.Tensor = None) -> torch.Tensor:
+        """`matvec` for up to MATMUL_MAX_TOKENS rows of x, on tensor cores (zipnn_b200_decode_plan_matmul): the same
+        arguments and rules, with `matmul_ok` and `matmul_scratch_bytes` in place of the matvec's.  bf16 and fp16
+        weights only.  Products and sums are fp32 (the tensor cores' sums are not rounded to nearest at each step, so
+        a result may differ from the matvec's in the last bits), each result is rounded once; two calls with the same
+        inputs give the same bits.  x must be finite: an infinity may give NaN where the dense product gives one."""
+        return self._product("matmul", k, x, bias, out, scratch)
+
+    def _product(self, name: str, k: int, x, bias, out, scratch) -> torch.Tensor:
+        """matvec and matmul: the checks and the call, `name` choosing the limit, eligibility, scratch and function."""
+        mm = name == "matmul"
+        limit = MATMUL_MAX_TOKENS if mm else MATVEC_MAX_TOKENS
+        ok, scratch_bytes = (self.matmul_ok, self.matmul_scratch_bytes) if mm else (self.matvec_ok, self.matvec_scratch_bytes)
         dt, sh = self._matvec_item(k)
         if not (isinstance(x, torch.Tensor) and x.is_cuda and x.device == self.device and x.dtype == dt and x.dim() >= 1):
-            raise ValueError(f"matvec takes a CUDA {dt} tensor [..., in_features] on the plan's device")
+            raise ValueError(f"{name} takes a CUDA {dt} tensor [..., in_features] on the plan's device")
         in_features = x.shape[-1]
         lead = tuple(x.shape[:-1])
         n = 1
         for d in lead:
             n *= d
-        if n > MATVEC_MAX_TOKENS:
-            raise ValueError(f"matvec takes at most {MATVEC_MAX_TOKENS} rows of x, not {n}")
-        if not self.matvec_ok(k, in_features):
-            raise ValueError(f"matvec cannot multiply by output {k} with in_features {in_features} (see matvec_ok)")
+        if n > limit:
+            raise ValueError(f"{name} takes at most {limit} rows of x, not {n}")
+        if not ok(k, in_features):
+            raise ValueError(f"{name} cannot multiply by output {k} with in_features {in_features} (see {name}_ok)")
         total = 1
         for d in sh:
             total *= d
@@ -341,13 +387,13 @@ class DecodePlan:
                 x2 = x2.clone()
         if bias is not None and not (isinstance(bias, torch.Tensor) and bias.device == self.device and bias.dtype == dt
                                      and tuple(bias.shape) == (out_features,) and bias.is_contiguous()):
-            raise ValueError(f"matvec's bias must be a contiguous {dt} CUDA tensor of shape ({out_features},) on the plan's device")
+            raise ValueError(f"{name}'s bias must be a contiguous {dt} CUDA tensor of shape ({out_features},) on the plan's device")
         shape = lead + (out_features,)
         if out is None:
             out = torch.empty(shape, dtype=dt, device=self.device)
         elif not (isinstance(out, torch.Tensor) and out.is_cuda and out.device == self.device and out.dtype == dt
                   and tuple(out.shape) == shape):
-            raise ValueError(f"matvec's out must be a {dt} CUDA tensor of shape {shape} on the plan's device")
+            raise ValueError(f"{name}'s out must be a {dt} CUDA tensor of shape {shape} on the plan's device")
         if n == 0:
             return out
         try:
@@ -355,18 +401,19 @@ class DecodePlan:
         except RuntimeError:
             y2 = None
         if y2 is None or y2.stride(1) != 1:
-            raise ValueError("matvec's out must have contiguous rows, equally spaced")
+            raise ValueError(f"{name}'s out must have contiguous rows, equally spaced")
         if scratch is None:
-            need = self.matvec_scratch_bytes(k, in_features)
-            if self._matvec_scratch is None or self._matvec_scratch.numel() < need:
-                self._matvec_scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
-            scratch = self._matvec_scratch
+            need = scratch_bytes(k, in_features)
+            own = self._scratches.get(name)
+            if own is None or own.numel() < need:
+                own = self._scratches[name] = torch.empty(need, dtype=torch.uint8, device=self.device)
+            scratch = own
         elif not (isinstance(scratch, torch.Tensor) and scratch.is_cuda and scratch.device == self.device
                   and scratch.dtype == torch.uint8 and scratch.is_contiguous()):
-            raise ValueError("matvec's scratch must be a contiguous CUDA uint8 tensor on the plan's device")
-        rc = self._matvec(self._ref, k, _MATVEC_DTYPES[dt], in_features, x2.data_ptr(), x2.stride(0), n,
-                          bias.data_ptr() if bias is not None else None, y2.data_ptr(), y2.stride(0), scratch.data_ptr(), scratch.numel(),
-                          torch.cuda.current_stream(self.device).cuda_stream)
+            raise ValueError(f"{name}'s scratch must be a contiguous CUDA uint8 tensor on the plan's device")
+        rc = (self._matmul if mm else self._matvec)(self._ref, k, _MATVEC_DTYPES[dt], in_features, x2.data_ptr(), x2.stride(0), n,
+                                                    bias.data_ptr() if bias is not None else None, y2.data_ptr(), y2.stride(0),
+                                                    scratch.data_ptr(), scratch.numel(), torch.cuda.current_stream(self.device).cuda_stream)
         if rc:
             _native.check(rc)
         return out

@@ -26,6 +26,8 @@ Rules:
   * with `matvec=N` a selected `torch.nn.Linear` (its class's own forward) multiplies inputs of at most N rows
     straight from the stream (`DecodePlan.matvec`: the dense weight is neither written nor read) and decodes as
     before for larger inputs; its bias stays a dense parameter;
+  * with `matmul=N` such a Linear with a bf16 / fp16 weight multiplies inputs of more rows than the matvec takes and
+    at most N on tensor cores (`DecodePlan.matmul`), again without a dense weight;
   * `state_dict()` does not see compressed parameters; `decompress_module(model)` restores them as dense
     `Parameter`s, bit for bit, and removes the hooks and plans.
 
@@ -41,7 +43,7 @@ import traceback
 import torch
 
 from . import prefetch as _prefetch
-from .plan import _HEAD, MATVEC_MAX_TOKENS, DecodePlan, _Stream
+from .plan import _HEAD, MATMUL_MAX_TOKENS, MATVEC_MAX_TOKENS, DecodePlan, _Stream
 from .safetensors_io import _FileRange, _cuda_device, compress_groups, file_entries, save_coded
 from .util_safetensors import COMPRESSION_METHOD
 from .zipnn import DecodePipe, ZipNN
@@ -108,6 +110,10 @@ class _Resident:
         self.matvecs = []     # matvec=N: (linear module, plan, index into the plan's outputs)
         self.matvec_scratch = None  # the matvecs' scratch: the plans' one when it is large enough
         self.matvec_scratch_bytes = 0  # what the largest matvec needs of it
+        self.matmul = 0       # matmul=N: the most input rows a matmul module multiplies without decoding
+        self.matmuls = set()  # matmul=N: id() of the `matvecs` modules whose weight `DecodePlan.matmul_ok` accepts
+        self.matmul_scratch = None  # the matmuls' scratch: the plans' one when it is large enough
+        self.matmul_scratch_bytes = 0  # what the largest matmul needs of it
 
 
 def _pre_hook(plan, names):
@@ -162,29 +168,37 @@ def dense_biases(groups, matvec: int) -> list:
     return [(p, owners) for p, owners in groups if not all(n == "bias" and matvecs(o) for o, n in owners)]
 
 
-def _check_matvec(matvec: int, prefetch: bool) -> int:
-    if not (isinstance(matvec, int) and 0 <= matvec <= MATVEC_MAX_TOKENS):
-        raise ValueError(f"matvec must be an integer from 0 to {MATVEC_MAX_TOKENS}, not {matvec!r}")
+def _check_matvec(matvec: int, prefetch: bool, name: str = "matvec", limit: int = MATVEC_MAX_TOKENS) -> int:
+    if not (isinstance(matvec, int) and 0 <= matvec <= limit):
+        raise ValueError(f"{name} must be an integer from 0 to {limit}, not {matvec!r}")
     if matvec and prefetch:
-        raise ValueError("matvec and prefetch=True do not combine yet: the prefetch schedule decodes every module")
+        raise ValueError(f"{name} and prefetch=True do not combine yet: the prefetch schedule decodes every module")
     return matvec
 
 
-def _matvec_forward(mod, state, plan, k, names, dtype, device):
+def _check_matmul(matmul: int, prefetch: bool) -> int:
+    return _check_matvec(matmul, prefetch, "matmul", MATMUL_MAX_TOKENS)
+
+
+def _matvec_forward(mod, state, plan, k, names, dtype, device, matmul: int = 0):
     """The forward of a matvec module: an input of at most `state.matvec` rows (a host-side test of its shape) that has
-    the weight's `dtype` and `device`, outside autocast, goes to `plan.matvec` and nothing is decoded or bound; any
-    other input (a larger one, another dtype, an autocast region: whatever F.linear accepts) takes the decode, bind,
-    forward, unbind of the hooks every other compressed module has."""
+    the weight's `dtype` and `device`, outside autocast, goes to `plan.matvec`; one of more rows and at most `matmul`
+    (the module's limit: `state.matmul` for the modules in `state.matmuls`, else 0) goes to `plan.matmul`.  Then nothing
+    is decoded or bound.  Any other input (a larger one, another dtype, an autocast region: whatever F.linear accepts)
+    takes the decode, bind, forward, unbind of the hooks every other compressed module has."""
     pre, post = _pre_hook(plan, names), _unbind(names)
 
     def forward(input):
         width = input.shape[-1] if input.dim() else 0
-        if (width and input.numel() // width <= state.matvec and input.dtype == dtype and input.device == device
+        rows = input.numel() // width if width else None
+        if (rows is not None and rows <= max(state.matvec, matmul) and input.dtype == dtype and input.device == device
                 and not torch.is_autocast_enabled(device.type)):
             if torch.is_grad_enabled():
                 raise RuntimeError(f"{type(mod).__name__} holds compressed weights and runs only under torch.no_grad() or "
                                    "torch.inference_mode()")
-            return plan.matvec(k, input, bias=mod.bias, scratch=state.matvec_scratch)
+            if rows <= state.matvec:
+                return plan.matvec(k, input, bias=mod.bias, scratch=state.matvec_scratch)
+            return plan.matmul(k, input, bias=mod.bias, scratch=state.matmul_scratch)
         pre(mod, (input,))
         try:
             return torch.nn.Linear.forward(mod, input)
@@ -233,7 +247,8 @@ def _pack(streams: dict, dev) -> tuple:
     return buf, views
 
 
-def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: bool = False, matvec: int = 0) -> tuple:
+def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: bool = False, matvec: int = 0,
+                    matmul: int = 0) -> tuple:
     """The back half of compress_module and load_module: streams {group index: CUDA stream} -> per selected module
     one DecodePlan over its parameters' streams, all sharing one output and one scratch buffer.  Raises like
     `decompress` on a corrupt stream; nothing outside is touched until `_commit`.  -> (_Resident, report).
@@ -243,7 +258,8 @@ def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: 
     transient buffer that is freed before the shared output buffer exists (so the peak stays that of gather=False).
 
     matvec=N: a `matvecs` module whose one compressed parameter is a weight that `DecodePlan.matvec_ok` accepts is
-    listed in `state.matvecs`; its plan and its room in the shared output buffer stay (larger inputs decode)."""
+    listed in `state.matvecs`; its plan and its room in the shared output buffer stay (larger inputs decode).
+    matmul=N: the same for `DecodePlan.matmul_ok`; such a module is also in `state.matmuls`."""
     where = {id(groups[i][0]): i for i in streams}
     per_module = []
     for m in modules:
@@ -277,9 +293,13 @@ def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: 
         state.entries.append((m, plan, [(n, k) for k, (n, _) in enumerate(names)], []))
         for k, (_, i) in enumerate(names):
             by_stream.setdefault(i, (plan, k))
-        if matvec and matvecs(m) and [n for n, _ in names] == ["weight"] and plan.matvec_ok(0, m.in_features):
-            state.matvecs.append((m, plan, 0))
-    state.matvec = matvec
+        if (matvec or matmul) and matvecs(m) and [n for n, _ in names] == ["weight"]:
+            mm = bool(matmul) and plan.matmul_ok(0, m.in_features)
+            if mm or (matvec and plan.matvec_ok(0, m.in_features)):
+                state.matvecs.append((m, plan, 0))
+            if mm:
+                state.matmuls.add(id(m))
+    state.matvec, state.matmul = matvec, matmul
     for m, i in looked:
         plan, k = by_stream[i]
         state.gathers.append((m, plan, k, i in own))
@@ -315,16 +335,21 @@ def _commit(module: torch.nn.Module, state: _Resident, prefetch: bool = False) -
             state.gather_scratch = state.scratch
         for m, plan, k, _ in state.gathers:
             m.__dict__["forward"] = _gather_forward(m, state, plan, k)
-    if state.matvecs:
+    if state.matvecs and state.matvec:
         need = max(plan.matvec_scratch_bytes(k, m.in_features, state.matvec) for m, plan, k in state.matvecs)
         state.matvec_scratch_bytes = need
         state.matvec_scratch = state.scratch if need <= state.scratch.numel() else torch.empty(need, dtype=torch.uint8,
+                                                                                                device=state.scratch.device)
+    if state.matmuls:
+        need = max(plan.matmul_scratch_bytes(k, m.in_features, state.matmul) for m, plan, k in state.matvecs if id(m) in state.matmuls)
+        state.matmul_scratch_bytes = need
+        state.matmul_scratch = state.scratch if need <= state.scratch.numel() else torch.empty(need, dtype=torch.uint8,
                                                                                                 device=state.scratch.device)
     by_matvec = {id(m): (plan, k) for m, plan, k in state.matvecs}
     for key, (m, plan, local, hooks) in enumerate(state.entries):
         if id(m) in by_matvec:   # no hooks: its forward decides per input whether anything is decoded
             m.__dict__["forward"] = _matvec_forward(m, state, plan, by_matvec[id(m)][1], local, plan.outputs[by_matvec[id(m)][1]].dtype,
-                                                    plan.device)
+                                                    plan.device, state.matmul if id(m) in state.matmuls else 0)
             continue
         if sched is None:
             pre = _pre_hook(plan, local)
@@ -339,7 +364,8 @@ def _commit(module: torch.nn.Module, state: _Resident, prefetch: bool = False) -
     setattr(module, _ATTR, state)
 
 
-def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = False, gather: bool = False, matvec: int = 0) -> dict:
+def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = False, gather: bool = False, matvec: int = 0,
+                    matmul: int = 0) -> dict:
     """Compress the weights of `modules` (default: every submodule that directly owns bf16 / fp16 / fp32 / fp8
     parameters) into streams kept in HBM, decoded just before each module's forward.  All parameters are compressed
     in one `compress_batch` call and must be on one CUDA device.
@@ -370,12 +396,20 @@ def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = Fals
     autocast region, take the decode path whatever their size.  A tied weight keeps one stream; each owner has its
     plan as before.  The shared output buffer stays, since larger inputs (prefill) decode into it.  The report gains
     "matvec_modules" and "matvec_scratch_bytes" (one scratch for all of them, sized for the largest; the plans'
-    scratch when that is large enough).  ValueError together with prefetch=True."""
+    scratch when that is large enough).  ValueError together with prefetch=True.
+
+    matmul=N (0 .. MATMUL_MAX_TOKENS; 0, the default, changes nothing): a `matvecs` module whose bf16 / fp16 weight
+    `DecodePlan.matmul_ok` accepts computes inputs of more than `matvec` rows and at most N as `DecodePlan.matmul`
+    (tensor cores, two launches, the weight neither decoded nor bound); inputs of at most `matvec` rows still take the
+    matvec, larger ones, other dtypes or devices and autocast regions the decode.  The biases stay dense as for
+    matvec.  The report gains "matmul_modules" and "matmul_scratch_bytes" (one scratch for all of them, as for the
+    matvec).  ValueError together with prefetch=True."""
     matvec = _check_matvec(matvec, prefetch)
+    matmul = _check_matmul(matmul, prefetch)
     if getattr(module, _ATTR, None) is not None:
         raise ValueError("compress_module: this module is already compressed")
     modules, groups = select(module, modules)
-    groups = dense_biases(groups, matvec)
+    groups = dense_biases(groups, max(matvec, matmul))
     params = [p for p, _ in groups]
     if not params:
         setattr(module, _ATTR, None)
@@ -388,12 +422,12 @@ def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = Fals
     # the streams move into one tight buffer; the batch's output buffer (sized by the bound) is dropped
     buf, streams = _pack({i: s for i, (p, s) in enumerate(zip(params, coded)) if s.numel() < p.numel() * p.element_size()}, dev)
     del coded, params
-    state, report = _resident_state(modules, groups, streams, [buf], dev, gather, matvec)
+    state, report = _resident_state(modules, groups, streams, [buf], dev, gather, matvec, matmul)
     _commit(module, state, prefetch)
-    return _with_prefetch(report, state, prefetch, gather, matvec)
+    return _with_prefetch(report, state, prefetch, gather, matvec, matmul)
 
 
-def _with_prefetch(report: dict, state, prefetch: bool, gather: bool = False, matvec: int = 0) -> dict:
+def _with_prefetch(report: dict, state, prefetch: bool, gather: bool = False, matvec: int = 0, matmul: int = 0) -> dict:
     if prefetch:
         report = dict(report, prefetch_out_bytes=state.prefetch[1].numel() if state is not None and state.prefetch else 0)
     if gather:
@@ -403,6 +437,9 @@ def _with_prefetch(report: dict, state, prefetch: bool, gather: bool = False, ma
     if matvec:
         report = dict(report, matvec_modules=len(state.matvecs) if state is not None else 0,
                       matvec_scratch_bytes=state.matvec_scratch_bytes if state is not None else 0)
+    if matmul:
+        report = dict(report, matmul_modules=len(state.matmuls) if state is not None else 0,
+                      matmul_scratch_bytes=state.matmul_scratch_bytes if state is not None else 0)
     return report
 
 
@@ -461,6 +498,7 @@ def decompress_module(module: torch.nn.Module) -> None:
     state.entries.clear()
     state.gathers.clear()
     state.matvecs.clear()
+    state.matmuls.clear()
     delattr(module, _ATTR)
 
 
@@ -600,7 +638,7 @@ def plan_load(module: torch.nn.Module, filenames, modules=None, matvec: int = 0)
     return plan
 
 
-def _load_device(plan: LoadPlan, dev, gather: bool = False, matvec: int = 0) -> tuple:
+def _load_device(plan: LoadPlan, dev, gather: bool = False, matvec: int = 0, matmul: int = 0) -> tuple:
     """Every device step of load_module; the module is not touched.  -> (_Resident or None, report, dense tensors of
     plan.dense, {group index: dense tensor} of plain entries that did not compress, moved buffers of plan.moves)."""
     pipe = DecodePipe(dev)
@@ -670,7 +708,8 @@ def _load_device(plan: LoadPlan, dev, gather: bool = False, matvec: int = 0) -> 
             pipe.finish()
             moved = [m._buffers[n].to(dev) for m, n in plan.moves]
             if plan.groups:
-                state, report = _resident_state(plan.modules, plan.groups, dict(sorted(streams.items())), buffers, dev, gather, matvec)
+                state, report = _resident_state(plan.modules, plan.groups, dict(sorted(streams.items())), buffers, dev, gather, matvec,
+                                                matmul)
             else:
                 state, report = None, dict(_EMPTY_REPORT)
         return state, report, dense, stayed, moved
@@ -681,7 +720,7 @@ def _load_device(plan: LoadPlan, dev, gather: bool = False, matvec: int = 0) -> 
 
 
 def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None, prefetch: bool = False,
-                gather: bool = False, matvec: int = 0) -> dict:
+                gather: bool = False, matvec: int = 0, matmul: int = 0) -> dict:
     """Load a checkpoint into `module` with the weights of `modules` kept compressed on `device`: the state
     `compress_module` leaves (same selection rules, hooks, plans and report), reached without a dense copy of those
     weights on the GPU.
@@ -716,18 +755,19 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None,
     and the batched decode's workspace; plain entries add one group at a time: its input, its streams' bound and the
     compress workspace.  A model loaded from .znn files never has its compressed weights dense on the device.
 
-    prefetch, gather, matvec: as for `compress_module`.
+    prefetch, gather, matvec, matmul: as for `compress_module`.
 
     -> the report of `compress_module`."""
     matvec = _check_matvec(matvec, prefetch)
+    matmul = _check_matmul(matmul, prefetch)
     dev = _cuda_device(device)
     if dev is None:
         raise ValueError(f"load_module: {device!r} is not a CUDA device")
     if dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
-    plan = plan_load(module, filenames, modules, matvec)
+    plan = plan_load(module, filenames, modules, max(matvec, matmul))
     try:
-        state, report, dense, stayed, moved = _load_device(plan, dev, gather, matvec)
+        state, report, dense, stayed, moved = _load_device(plan, dev, gather, matvec, matmul)
     except BaseException as e:
         traceback.clear_frames(e.__traceback__)   # the frames' locals would keep the call's device memory alive
         raise
@@ -749,7 +789,7 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None,
         setattr(module, _ATTR, None)
     else:
         _commit(module, state, prefetch)
-    return _with_prefetch(report, state, prefetch, gather, matvec)
+    return _with_prefetch(report, state, prefetch, gather, matvec, matmul)
 
 
 def save_module(module: torch.nn.Module, filename, metadata=None) -> None:
