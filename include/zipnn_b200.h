@@ -220,7 +220,7 @@ int zipnn_b200_decode_plan_run_shifted(const zipnn_b200_decode_plan* plan, int64
  * Host-side rejections launch and write nothing: E_ARG for id_bytes other than 4 or 8, row_bytes 0 or not dividing
  * the item's bytes, a NULL d_ids, d_out or d_scratch (n_ids > 0), misaligned ids or scratch, a scratch smaller than
  * one slot, an item index out of range, or a plan whose create failed; E_UNSUPPORTED for an item that is a box, is
- * empty or was split into several pieces (over 16384 chunks), and for a plan without a segment index.
+ * empty or was split into several pieces (16384 chunks or more), and for a plan without a segment index.
  * _gather_scratch_size: the scratch bytes of `slots` slots (capped to K; slots >= 1), same checks. */
 int zipnn_b200_decode_plan_gather_scratch_size(const zipnn_b200_decode_plan* plan, int item, size_t row_bytes,
                                                size_t slots, size_t* out);
@@ -239,7 +239,7 @@ int zipnn_b200_decode_plan_gather(const zipnn_b200_decode_plan* plan, int item, 
  * order.  No atomics on floats, no copy, memset or synchronisation: capturable in a CUDA graph, replayable with new x,
  * and two calls with the same inputs give the same bits.  n_tokens == 0 launches nothing.
  * Eligible items (else E_UNSUPPORTED, and the caller decodes the item as before): a whole tensor in one piece (not a
- * box, not empty, at most 16384 chunks) of a plan with a segment index; num_buf equal to the dtype's size;
+ * box, not empty, at most 16383 chunks) of a plan with a segment index; num_buf equal to the dtype's size;
  * in_features * element size a multiple of 16; every chunk in the fused decode mode (one coded plane, the top byte
  * plane; chunk length a multiple of 512) -- what float weights produce.  The first _matvec or _matvec_scratch_size call
  * for an item reads its chunk modes from the device and synchronises cuda_stream (the null stream for _scratch_size);
