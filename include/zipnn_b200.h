@@ -228,6 +228,31 @@ int zipnn_b200_decode_plan_gather(const zipnn_b200_decode_plan* plan, int item, 
                                   size_t n_ids, int id_bytes, void* d_out, void* d_scratch, size_t scratch_bytes,
                                   void* cuda_stream);
 
+/* _run_select: the plan run for the slices that ids select, and nothing else (the routed experts of a mixture-of-
+ * experts layer).  Every item is seen as `rows` slices along dim 0 of item bytes / rows bytes each; for every id e in
+ * d_ids (n_ids of them, int32 or int64: id_bytes 4 or 8, aligned to their size, duplicates allowed) the bytes of slice
+ * e of every item are written to the item's d_out, as _run writes them.  Exactly the chunks that meet a selected slice
+ * are decoded, whole (a chunk that straddles two slices included), and no other byte of any d_out is written: the
+ * other slices keep whatever they held.
+ * Launches only (no copy, memset or synchronisation: capturable in a CUDA graph, replayable with new ids in d_ids): 5
+ * launches whatever the id values are -- an index kernel that compacts the plan's work lists to the selected chunks,
+ * the replay decoder, the regroup and the overflow decoder over those lists, and the plan run's error pass.  The
+ * grids depend on n_ids, never on the id values.  n_ids == 0 launches nothing.
+ * An id outside [0, rows) (negative included) selects nothing and sets ZIPNN_B200_E_INDEX in the plan's error word,
+ * which _status returns (sticky, as for _gather).
+ * d_scratch (256-byte aligned, at least _select_scratch_size bytes) holds nothing between calls: calls that share it
+ * must be ordered on one stream, as for _gather.  It must not overlap the plan's own scratch, which a selected run
+ * uses as _run does (runs of one plan, and of plans sharing that scratch, ordered on one stream).
+ * Host-side rejections launch and write nothing: E_ARG for id_bytes other than 4 or 8, rows 0 or not dividing some
+ * item's bytes, a NULL d_ids or d_scratch (n_ids > 0), misaligned ids or scratch, a scratch below
+ * _select_scratch_size, or a plan whose create failed; E_UNSUPPORTED for a plan without items, a plan without a
+ * segment index, or an item that is not one whole-tensor piece (a box, an empty item, or one split into pieces:
+ * 16384 chunks or more).
+ * _select_scratch_size: the scratch bytes, same checks; they depend on the plan alone. */
+int zipnn_b200_decode_plan_select_scratch_size(const zipnn_b200_decode_plan* plan, size_t rows, size_t* out);
+int zipnn_b200_decode_plan_run_select(const zipnn_b200_decode_plan* plan, size_t rows, const void* d_ids, size_t n_ids,
+                                      int id_bytes, void* d_scratch, size_t scratch_bytes, void* cuda_stream);
+
 /* _matvec: y = x W^T (+ bias) for a few rows of x, straight from the coded bitstreams of item `item`: the dense W is
  * never written or read back.  W is the item's decoded tensor, row-major [out_features][in_features] of `dtype`
  * (out_features = the item's elements / in_features); x is n_tokens rows of in_features elements, x_stride elements

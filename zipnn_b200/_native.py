@@ -118,6 +118,8 @@ def lib() -> C.CDLL:
                 "zipnn_b200_decode_plan_run_shifted": (i32, [C.POINTER(DecodePlanStruct), C.c_int64, i32, vp]),
                 "zipnn_b200_decode_plan_gather_scratch_size": (i32, [C.POINTER(DecodePlanStruct), i32, sz, sz, szp]),
                 "zipnn_b200_decode_plan_gather": (i32, [C.POINTER(DecodePlanStruct), i32, sz, vp, sz, i32, vp, vp, sz, vp]),
+                "zipnn_b200_decode_plan_select_scratch_size": (i32, [C.POINTER(DecodePlanStruct), sz, szp]),
+                "zipnn_b200_decode_plan_run_select": (i32, [C.POINTER(DecodePlanStruct), sz, vp, sz, i32, vp, sz, vp]),
                 "zipnn_b200_decode_plan_matvec_scratch_size": (i32, [C.POINTER(DecodePlanStruct), i32, i32, sz, sz, szp]),
                 "zipnn_b200_decode_plan_matvec": (i32, [C.POINTER(DecodePlanStruct), i32, i32, sz, vp, sz, sz, vp, vp, sz, vp, sz, vp]),
                 "zipnn_b200_decode_plan_matmul_scratch_size": (i32, [C.POINTER(DecodePlanStruct), i32, i32, sz, sz, szp]),
@@ -146,6 +148,7 @@ EXPORTS = [
     "zipnn_b200_decompress_slices_workspace_size", "zipnn_b200_decompress_slices", "zipnn_b200_decode_plan_size",
     "zipnn_b200_decode_plan_create", "zipnn_b200_decode_plan_run", "zipnn_b200_decode_plan_status", "zipnn_b200_decode_plan_index", "zipnn_b200_decode_plan_run_shifted",
     "zipnn_b200_decode_plan_gather_scratch_size", "zipnn_b200_decode_plan_gather",
+    "zipnn_b200_decode_plan_select_scratch_size", "zipnn_b200_decode_plan_run_select",
     "zipnn_b200_decode_plan_matvec_scratch_size", "zipnn_b200_decode_plan_matvec",
     "zipnn_b200_decode_plan_matmul_scratch_size", "zipnn_b200_decode_plan_matmul", "zipnn_b200_split", "zipnn_b200_regroup", "zipnn_b200_compress_host", "zipnn_b200_decompress_host",
     "zipnn_b200_timing_enable", "zipnn_b200_timing_kernel_count", "zipnn_b200_timing_kernel_name",

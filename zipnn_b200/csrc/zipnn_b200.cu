@@ -22,6 +22,7 @@
 #include "gather.cuh"
 #include "matmul.cuh"
 #include "matvec.cuh"
+#include "select.cuh"
 #include "stage1.cuh"
 
 using namespace zb;
@@ -1370,6 +1371,112 @@ int zipnn_b200_decode_plan_gather(const zipnn_b200_decode_plan* plan, int item, 
     ZB_LAUNCHED();
   }
   return ZIPNN_B200_OK;
+}
+
+// ---- selected runs: the plan run for the chunks of the slices [e] that ids select (select.cuh) -----------------
+// Scratch: [256 B: counts][DecodeCfg np][Ctrl np][hsel uint2 per coded item][tsel uint2 per tile][osel u32 per chunk].
+namespace {
+struct SelectLayout {
+  size_t ocfg_off, octrl_off, hsel_off, tsel_off, osel_off, bytes;
+};
+SelectLayout select_layout(const PlanState& s) {
+  SelectLayout L;
+  const size_t np = s.B.n;
+  L.ocfg_off = 256;
+  L.octrl_off = round_up(L.ocfg_off + sizeof(DecodeCfg) * np, 256);
+  L.hsel_off = round_up(L.octrl_off + sizeof(Ctrl) * np, 256);
+  L.tsel_off = round_up(L.hsel_off + sizeof(uint2) * (s.grid.items / 4), 256);
+  L.osel_off = round_up(L.tsel_off + sizeof(uint2) * s.grid.tiles, 256);
+  L.bytes = round_up(L.osel_off + sizeof(uint32_t) * s.grid.chunks, 256);
+  return L;
+}
+// The host-side checks shared by both calls: every item is one whole-tensor piece (so piece j is item j) of a plan with
+// a segment index, and its bytes split into `rows` equal slices.  -> the items' records.
+int select_items(const zipnn_b200_decode_plan* plan, size_t rows, PlanState& s, std::vector<GatherItem>& items) {
+  if (!plan_state(plan, s)) return ZIPNN_B200_E_ARG;
+  {
+    std::lock_guard<std::mutex> lk(g_plan_mu);
+    const auto it = g_plan_items.find((uintptr_t)s.B.error_out);
+    if (it == g_plan_items.end() || it->second.gen != s.gen) return ZIPNN_B200_E_ARG;
+    items = it->second.items;
+  }
+  if (s.mode != kSyncReplay || items.empty() || items.size() > 65535) return ZIPNN_B200_E_UNSUPPORTED;  // (grid.y of the overflow)
+  for (const GatherItem& gi : items)
+    if (gi.piece < 0) return ZIPNN_B200_E_UNSUPPORTED;
+  for (const GatherItem& gi : items)
+    if (rows == 0 || gi.orig % rows) return ZIPNN_B200_E_ARG;
+  return ZIPNN_B200_OK;
+}
+}  // namespace
+
+int zipnn_b200_decode_plan_select_scratch_size(const zipnn_b200_decode_plan* plan, size_t rows, size_t* out) {
+  if (!out) return ZIPNN_B200_E_ARG;
+  PlanState s;
+  std::vector<GatherItem> items;
+  const int rc = select_items(plan, rows, s, items);
+  if (rc) return rc;
+  *out = select_layout(s).bytes;
+  return ZIPNN_B200_OK;
+}
+
+int zipnn_b200_decode_plan_run_select(const zipnn_b200_decode_plan* plan, size_t rows, const void* d_ids, size_t n_ids, int id_bytes,
+                                      void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (id_bytes != 4 && id_bytes != 8) return ZIPNN_B200_E_ARG;
+  PlanState s;
+  std::vector<GatherItem> items;
+  {
+    const int rc = select_items(plan, rows, s, items);
+    if (rc) return rc;
+  }
+  if (n_ids == 0) return ZIPNN_B200_OK;
+  if (!d_ids || !d_scratch || ((uintptr_t)d_ids % (uintptr_t)id_bytes) || ((uintptr_t)d_scratch & 255)) return ZIPNN_B200_E_ARG;
+  if (n_ids > (1ull << 40)) return ZIPNN_B200_E_ARG;
+  const SelectLayout L = select_layout(s);
+  if (scratch_bytes < L.bytes) return ZIPNN_B200_E_ARG;
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  uint8_t* ws = (uint8_t*)d_scratch;
+  SelectCfg sel;
+  sel.ids = d_ids;
+  sel.n = n_ids;
+  sel.id8 = id_bytes == 8;
+  sel.rows = rows;
+  sel.error = s.B.error_out;
+  sel.count = (uint32_t*)ws;
+  sel.ocfg = (DecodeCfg*)(ws + L.ocfg_off);
+  sel.octrl = (Ctrl*)(ws + L.octrl_off);
+  sel.hsel = (uint2*)(ws + L.hsel_off);
+  sel.tsel = (uint2*)(ws + L.tsel_off);
+  sel.osel = (uint32_t*)(ws + L.osel_off);
+  // grids from bounds of n alone: an item's touched chunks are at most min(n * span, K)
+  uint64_t bitstreams = 0, tiles = 0, most = 0;
+  for (const GatherItem& gi : items) {
+    const uint64_t span = gather_span(gi.orig / rows, gi.chunk, gi.K);
+    const uint64_t m = n_ids > gi.K / span ? gi.K : std::min<uint64_t>(gi.K, n_ids * span);
+    bitstreams += 4ull * gi.G * m;
+    tiles += m * ((gi.chunk + kMergeTile - 1) / kMergeTile);
+    most = std::max(most, m);
+  }
+  if (!smem_attr(k_select_sync, kSyncSmemBytes)) return ZIPNN_B200_E_CUDA;
+  const int nb = resident_blocks(k_select_sync, kSyncSmemBytes, kSyncThreads);
+  const int sms = sm_count_cached();
+  k_select_index<<<1, kGatherIndexThreads, 0, st>>>(s.B, sel);
+  ZB_LAUNCHED();
+  {
+    ScopedTimer tm(kKHufDecodeSync, st);
+    k_select_sync<<<(unsigned)std::min<uint64_t>(bitstreams, (uint64_t)nb * sms), kSyncThreads, kSyncSmemBytes, st>>>(s.B, s.X, sel);
+    ZB_LAUNCHED();
+  }
+  {
+    ScopedTimer tm(kKRegroup, st);
+    k_select_regroup<<<(unsigned)std::min<uint64_t>(tiles, (uint64_t)sms * 16), kMergeThreads, 0, st>>>(s.B, sel);
+    ZB_LAUNCHED();
+  }
+  {
+    ScopedTimer tm(kKDecodeOverflow, st);
+    k_select_overflow<<<dim3((unsigned)std::min<uint64_t>(s.grid.max_ovf, most), s.B.n), kMergeThreads, sizeof(DecodeSmem), st>>>(sel);
+    ZB_LAUNCHED();
+  }
+  return batch_errors(s.B, st);
 }
 
 // ---- matvec: x W^T from the coded bitstreams of one whole-tensor item, no dense W (matvec.cuh) ------------------

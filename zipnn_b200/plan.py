@@ -109,7 +109,8 @@ def _raise_status(rc: int) -> None:
     if rc == _native.E_CORRUPT:
         raise _native.ZipNNNativeError(rc, "Thread processing failed: corrupt ZipNN stream")
     if rc == _native.E_INDEX:
-        raise IndexError("zipnn_b200: a gather of this plan met an id outside [0, rows) (its rows were zeroed)")
+        raise IndexError("zipnn_b200: a gather or selected run of this plan met an id outside [0, rows) (a gather zeroed "
+                         "its rows, a selected run selected nothing for it)")
     _native.check(rc)
 
 
@@ -172,6 +173,8 @@ class DecodePlan:
         self._scratches = {}          # "matvec" / "matmul" -> that call's default scratch, grown on demand
         self._matvec_ok = {}          # (output, in_features) -> eligible?
         self._matmul_ok = {}
+        self._select_ok = None        # select_ok(), once asked
+        self._select_scratch = None   # run_select's default scratch
 
     def run(self) -> list:
         """Enqueue the decode on the current CUDA stream (launches only) and return `.outputs`."""
@@ -267,6 +270,67 @@ class DecodePlan:
         if rc:
             _native.check(rc)
         return out
+
+    def _select_size(self) -> tuple:
+        """-> (status, scratch bytes) of zipnn_b200_decode_plan_select_scratch_size for rows = shape[0] of the outputs."""
+        rows = {sh[0] if len(sh) else None for _, _, _, sh in self._offs}
+        if len(rows) != 1 or None in rows or 0 in rows:
+            return _native.E_UNSUPPORTED, 0
+        out = C.c_size_t(0)
+        rc = _native.lib().zipnn_b200_decode_plan_select_scratch_size(self._ref, rows.pop(), C.byref(out))
+        return rc, out.value
+
+    def select_ok(self) -> bool:
+        """Can `run_select` decode slices of this plan's outputs?  True when every output has at least one dimension
+        and the same `shape[0]` as the others, and is a whole tensor in one piece (not empty, at most 16383 chunks) of
+        a plan with a segment index.  Never raises."""
+        if self._select_ok is None:
+            self._select_ok = self._select_size()[0] == _native.OK
+        return self._select_ok
+
+    def select_scratch_bytes(self) -> int:
+        """Bytes of a `run_select` scratch for this plan (a few bytes per chunk; it depends on the plan alone)."""
+        rc, n = self._select_size()
+        _native.check(rc)
+        return n
+
+    def run_select(self, ids: torch.Tensor, scratch: torch.Tensor = None) -> list:
+        """Enqueue the decode of the slices `outputs[k][e]` (along dim 0) of every output k for every id e in `ids`
+        on the current CUDA stream, and return `.outputs` (zipnn_b200_decode_plan_run_select): only the chunks that
+        meet a selected slice are decoded (whole), no other byte of the outputs is written, so the slices that were
+        not selected hold unspecified bytes.  Launches only, a fixed number of them, the ids never read on the host:
+        capturable in a CUDA graph and replayable with new ids copied into the captured tensor.
+
+        ids:     CUDA int32 or int64 tensor of any shape on the plan's device; duplicates allowed; empty: nothing runs.
+        scratch: optional 256-byte aligned CUDA uint8 buffer of at least `select_scratch_bytes()` bytes, not the plan's
+                 own scratch.  It holds nothing between calls: calls that share it must be ordered on one stream.
+                 Default: a buffer kept by the plan.
+        An id outside [0, shape[0]) selects nothing and makes `check()` raise IndexError (from then on: the plan's
+        error word is sticky).  ValueError for a plan `select_ok` refuses."""
+        if self._out is None:
+            raise RuntimeError("DecodePlan: the output buffer was released (release_out); only gather runs")
+        if not (isinstance(ids, torch.Tensor) and ids.is_cuda and ids.device == self.device and ids.dtype in (torch.int32, torch.int64)):
+            raise ValueError("run_select takes CUDA int32 or int64 ids on the plan's device")
+        if not self.select_ok():
+            raise ValueError("run_select needs outputs that share shape[0], each a whole tensor in one piece (see select_ok)")
+        ids_c = ids.contiguous()
+        n = ids_c.numel()
+        if n == 0:
+            return self.outputs
+        if scratch is None:
+            need = self.select_scratch_bytes()
+            if self._select_scratch is None or self._select_scratch.numel() < need:
+                self._select_scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
+            scratch = self._select_scratch
+        elif not (isinstance(scratch, torch.Tensor) and scratch.is_cuda and scratch.device == self.device
+                  and scratch.dtype == torch.uint8 and scratch.is_contiguous()):
+            raise ValueError("run_select's scratch must be a contiguous CUDA uint8 tensor on the plan's device")
+        rc = _native.lib().zipnn_b200_decode_plan_run_select(self._ref, self._offs[0][3][0], ids_c.data_ptr(), n, ids_c.element_size(),
+                                                             scratch.data_ptr(), scratch.numel(),
+                                                             torch.cuda.current_stream(self.device).cuda_stream)
+        if rc:
+            _native.check(rc)
+        return self.outputs
 
     def _matvec_item(self, k: int) -> tuple:
         if not 0 <= k < len(self._offs):

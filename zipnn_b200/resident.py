@@ -28,6 +28,9 @@ Rules:
     before for larger inputs; its bias stays a dense parameter;
   * with `matmul=N` such a Linear with a bf16 / fp16 weight multiplies inputs of more rows than the matvec takes and
     at most N on tensor cores (`DecodePlan.matmul`), again without a dense weight;
+  * with `experts=True` the experts module of a mixture-of-experts layer (`experts_module`: 3D weights [E, ...] called
+    as experts(hidden_states, top_k_index, top_k_weights)) decodes only the slices [e] of the experts its router
+    picked (`DecodePlan.run_select`); its own forward then runs unchanged and reads only those slices;
   * `state_dict()` does not see compressed parameters; `decompress_module(model)` restores them as dense
     `Parameter`s, bit for bit, and removes the hooks and plans.
 
@@ -114,6 +117,8 @@ class _Resident:
         self.matmuls = set()  # matmul=N: id() of the `matvecs` modules whose weight `DecodePlan.matmul_ok` accepts
         self.matmul_scratch = None  # the matmuls' scratch: the plans' one when it is large enough
         self.matmul_scratch_bytes = 0  # what the largest matmul needs of it
+        self.experts = set()  # experts=True: id() of the `entries` modules that decode only their routed experts
+        self.select_scratch = None  # the experts modules' run_select scratch, sized for the largest
 
 
 def _pre_hook(plan, names):
@@ -122,6 +127,23 @@ def _pre_hook(plan, names):
             raise RuntimeError(f"{type(mod).__name__} holds compressed weights and runs only under torch.no_grad() or "
                                "torch.inference_mode() (its decoded weights live in a shared buffer)")
         outs = plan.run()
+        for name, k in names:
+            object.__setattr__(mod, name, outs[k])
+    return hook
+
+
+def _pre_hook_experts(plan, names, state):
+    # the ids: experts(hidden_states, top_k_index, top_k_weights), positional or by keyword
+    def hook(mod, args, kwargs):
+        if torch.is_grad_enabled():
+            raise RuntimeError(f"{type(mod).__name__} holds compressed weights and runs only under torch.no_grad() or "
+                               "torch.inference_mode() (its decoded weights live in a shared buffer)")
+        ids = args[1] if len(args) > 1 else kwargs.get("top_k_index")
+        if (isinstance(ids, torch.Tensor) and ids.is_cuda and ids.device == plan.device
+                and ids.dtype in (torch.int32, torch.int64)):
+            outs = plan.run_select(ids, scratch=state.select_scratch)
+        else:
+            outs = plan.run()
         for name, k in names:
             object.__setattr__(mod, name, outs[k])
     return hook
@@ -158,6 +180,25 @@ def matvecs(module: torch.nn.Module) -> bool:
     """Does `matvec=N` multiply small inputs of `module` from its compressed weight?  A torch.nn.Linear (or subclass)
     whose class does not override forward."""
     return isinstance(module, torch.nn.Linear) and type(module).forward is torch.nn.Linear.forward
+
+
+def experts_module(module: torch.nn.Module, names=None) -> bool:
+    """Does `experts=True` decode only the routed experts of `module`?  A module whose integer attribute `num_experts`
+    equals shape[0] of every parameter in `names` (default: every parameter of the codec's dtypes it owns directly;
+    there must be one): the convention of transformers' `*Experts` modules (gate_up_proj [E, 2I, H], down_proj
+    [E, H, I], biases [E, ...]).  Once its streams exist, its plan must also pass `DecodePlan.select_ok`."""
+    n = getattr(module, "num_experts", None)
+    if not isinstance(n, int) or isinstance(n, bool) or n <= 0:
+        return False
+    params = [p for name, p in _own_params(module) if names is None or name in names]
+    return bool(params) and all(p.dim() >= 1 and p.shape[0] == n for p in params)
+
+
+def _check_experts(experts: bool, prefetch: bool) -> bool:
+    if experts and prefetch:
+        raise ValueError("experts=True and prefetch=True do not combine: the prefetch schedule decodes every module "
+                         "before its router has picked the experts")
+    return bool(experts)
 
 
 def dense_biases(groups, matvec: int) -> list:
@@ -248,7 +289,7 @@ def _pack(streams: dict, dev) -> tuple:
 
 
 def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: bool = False, matvec: int = 0,
-                    matmul: int = 0) -> tuple:
+                    matmul: int = 0, experts: bool = False) -> tuple:
     """The back half of compress_module and load_module: streams {group index: CUDA stream} -> per selected module
     one DecodePlan over its parameters' streams, all sharing one output and one scratch buffer.  Raises like
     `decompress` on a corrupt stream; nothing outside is touched until `_commit`.  -> (_Resident, report).
@@ -259,7 +300,8 @@ def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: 
 
     matvec=N: a `matvecs` module whose one compressed parameter is a weight that `DecodePlan.matvec_ok` accepts is
     listed in `state.matvecs`; its plan and its room in the shared output buffer stay (larger inputs decode).
-    matmul=N: the same for `DecodePlan.matmul_ok`; such a module is also in `state.matmuls`."""
+    matmul=N: the same for `DecodePlan.matmul_ok`; such a module is also in `state.matmuls`.
+    experts=True: an `experts_module` whose plan passes `DecodePlan.select_ok` is in `state.experts`."""
     where = {id(groups[i][0]): i for i in streams}
     per_module = []
     for m in modules:
@@ -299,6 +341,8 @@ def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: 
                 state.matvecs.append((m, plan, 0))
             if mm:
                 state.matmuls.add(id(m))
+        if experts and experts_module(m, [n for n, _ in names]) and plan.select_ok():
+            state.experts.add(id(m))
     state.matvec, state.matmul = matvec, matmul
     for m, i in looked:
         plan, k = by_stream[i]
@@ -345,17 +389,24 @@ def _commit(module: torch.nn.Module, state: _Resident, prefetch: bool = False) -
         state.matmul_scratch_bytes = need
         state.matmul_scratch = state.scratch if need <= state.scratch.numel() else torch.empty(need, dtype=torch.uint8,
                                                                                                 device=state.scratch.device)
+    if state.experts:
+        need = max(plan.select_scratch_bytes() for m, plan, _, _ in state.entries if id(m) in state.experts)
+        state.select_scratch = torch.empty(need, dtype=torch.uint8, device=state.scratch.device)
     by_matvec = {id(m): (plan, k) for m, plan, k in state.matvecs}
     for key, (m, plan, local, hooks) in enumerate(state.entries):
         if id(m) in by_matvec:   # no hooks: its forward decides per input whether anything is decoded
             m.__dict__["forward"] = _matvec_forward(m, state, plan, by_matvec[id(m)][1], local, plan.outputs[by_matvec[id(m)][1]].dtype,
                                                     plan.device, state.matmul if id(m) in state.matmuls else 0)
             continue
-        if sched is None:
-            pre = _pre_hook(plan, local)
+        if id(m) in state.experts:
+            hooks.append(m.register_forward_pre_hook(_pre_hook_experts(plan, local, state), with_kwargs=True))
         else:
-            pre = _pre_hook_prefetch(sched, key, local, [plan.views(b) for b in sched.ops.slots])
-        hooks += [m.register_forward_pre_hook(pre), m.register_forward_hook(_unbind(local), always_call=True)]
+            if sched is None:
+                pre = _pre_hook(plan, local)
+            else:
+                pre = _pre_hook_prefetch(sched, key, local, [plan.views(b) for b in sched.ops.slots])
+            hooks.append(m.register_forward_pre_hook(pre))
+        hooks.append(m.register_forward_hook(_unbind(local), always_call=True))
     # the dense parameters go: nothing here keeps their storage alive
     for _, _, _, owners in state.params.values():
         for o, n in owners:
@@ -365,7 +416,7 @@ def _commit(module: torch.nn.Module, state: _Resident, prefetch: bool = False) -
 
 
 def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = False, gather: bool = False, matvec: int = 0,
-                    matmul: int = 0) -> dict:
+                    matmul: int = 0, experts: bool = False) -> dict:
     """Compress the weights of `modules` (default: every submodule that directly owns bf16 / fp16 / fp32 / fp8
     parameters) into streams kept in HBM, decoded just before each module's forward.  All parameters are compressed
     in one `compress_batch` call and must be on one CUDA device.
@@ -403,9 +454,20 @@ def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = Fals
     (tensor cores, two launches, the weight neither decoded nor bound); inputs of at most `matvec` rows still take the
     matvec, larger ones, other dtypes or devices and autocast regions the decode.  The biases stay dense as for
     matvec.  The report gains "matmul_modules" and "matmul_scratch_bytes" (one scratch for all of them, as for the
-    matvec).  ValueError together with prefetch=True."""
+    matvec).  ValueError together with prefetch=True.
+
+    experts=True (default False, which changes nothing): a selected module that `experts_module` accepts, and whose
+    plan `DecodePlan.select_ok` accepts, decodes through a forward pre-hook that takes the ids from its forward's second
+    positional argument or keyword `top_k_index` (transformers' `experts(hidden_states, top_k_index, top_k_weights)`).
+    For CUDA int32 / int64 ids on the plan's device the hook runs `DecodePlan.run_select`: only the chunks of the
+    experts those ids name are decoded; any other call decodes the whole module.  The module's own forward then reads
+    only the slices [e] of the routed experts, so its outputs equal the dense module's bit for bit, whichever experts
+    implementation it uses; the other slices of the shared buffer hold stale bytes.  The report gains
+    "experts_modules" and "experts_scratch_bytes" (one run_select scratch shared by them all, sized for the largest).
+    ValueError together with prefetch=True."""
     matvec = _check_matvec(matvec, prefetch)
     matmul = _check_matmul(matmul, prefetch)
+    experts = _check_experts(experts, prefetch)
     if getattr(module, _ATTR, None) is not None:
         raise ValueError("compress_module: this module is already compressed")
     modules, groups = select(module, modules)
@@ -422,12 +484,13 @@ def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = Fals
     # the streams move into one tight buffer; the batch's output buffer (sized by the bound) is dropped
     buf, streams = _pack({i: s for i, (p, s) in enumerate(zip(params, coded)) if s.numel() < p.numel() * p.element_size()}, dev)
     del coded, params
-    state, report = _resident_state(modules, groups, streams, [buf], dev, gather, matvec, matmul)
+    state, report = _resident_state(modules, groups, streams, [buf], dev, gather, matvec, matmul, experts)
     _commit(module, state, prefetch)
-    return _with_prefetch(report, state, prefetch, gather, matvec, matmul)
+    return _with_prefetch(report, state, prefetch, gather, matvec, matmul, experts)
 
 
-def _with_prefetch(report: dict, state, prefetch: bool, gather: bool = False, matvec: int = 0, matmul: int = 0) -> dict:
+def _with_prefetch(report: dict, state, prefetch: bool, gather: bool = False, matvec: int = 0, matmul: int = 0,
+                   experts: bool = False) -> dict:
     if prefetch:
         report = dict(report, prefetch_out_bytes=state.prefetch[1].numel() if state is not None and state.prefetch else 0)
     if gather:
@@ -440,6 +503,9 @@ def _with_prefetch(report: dict, state, prefetch: bool, gather: bool = False, ma
     if matmul:
         report = dict(report, matmul_modules=len(state.matmuls) if state is not None else 0,
                       matmul_scratch_bytes=state.matmul_scratch_bytes if state is not None else 0)
+    if experts:
+        report = dict(report, experts_modules=len(state.experts) if state is not None else 0,
+                      experts_scratch_bytes=state.select_scratch.numel() if state is not None and state.select_scratch is not None else 0)
     return report
 
 
@@ -499,6 +565,7 @@ def decompress_module(module: torch.nn.Module) -> None:
     state.gathers.clear()
     state.matvecs.clear()
     state.matmuls.clear()
+    state.experts.clear()
     delattr(module, _ATTR)
 
 
@@ -638,7 +705,7 @@ def plan_load(module: torch.nn.Module, filenames, modules=None, matvec: int = 0)
     return plan
 
 
-def _load_device(plan: LoadPlan, dev, gather: bool = False, matvec: int = 0, matmul: int = 0) -> tuple:
+def _load_device(plan: LoadPlan, dev, gather: bool = False, matvec: int = 0, matmul: int = 0, experts: bool = False) -> tuple:
     """Every device step of load_module; the module is not touched.  -> (_Resident or None, report, dense tensors of
     plan.dense, {group index: dense tensor} of plain entries that did not compress, moved buffers of plan.moves)."""
     pipe = DecodePipe(dev)
@@ -709,7 +776,7 @@ def _load_device(plan: LoadPlan, dev, gather: bool = False, matvec: int = 0, mat
             moved = [m._buffers[n].to(dev) for m, n in plan.moves]
             if plan.groups:
                 state, report = _resident_state(plan.modules, plan.groups, dict(sorted(streams.items())), buffers, dev, gather, matvec,
-                                                matmul)
+                                                matmul, experts)
             else:
                 state, report = None, dict(_EMPTY_REPORT)
         return state, report, dense, stayed, moved
@@ -720,7 +787,7 @@ def _load_device(plan: LoadPlan, dev, gather: bool = False, matvec: int = 0, mat
 
 
 def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None, prefetch: bool = False,
-                gather: bool = False, matvec: int = 0, matmul: int = 0) -> dict:
+                gather: bool = False, matvec: int = 0, matmul: int = 0, experts: bool = False) -> dict:
     """Load a checkpoint into `module` with the weights of `modules` kept compressed on `device`: the state
     `compress_module` leaves (same selection rules, hooks, plans and report), reached without a dense copy of those
     weights on the GPU.
@@ -755,11 +822,12 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None,
     and the batched decode's workspace; plain entries add one group at a time: its input, its streams' bound and the
     compress workspace.  A model loaded from .znn files never has its compressed weights dense on the device.
 
-    prefetch, gather, matvec, matmul: as for `compress_module`.
+    prefetch, gather, matvec, matmul, experts: as for `compress_module`.
 
     -> the report of `compress_module`."""
     matvec = _check_matvec(matvec, prefetch)
     matmul = _check_matmul(matmul, prefetch)
+    experts = _check_experts(experts, prefetch)
     dev = _cuda_device(device)
     if dev is None:
         raise ValueError(f"load_module: {device!r} is not a CUDA device")
@@ -767,7 +835,7 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None,
         dev = torch.device("cuda", torch.cuda.current_device())
     plan = plan_load(module, filenames, modules, max(matvec, matmul))
     try:
-        state, report, dense, stayed, moved = _load_device(plan, dev, gather, matvec, matmul)
+        state, report, dense, stayed, moved = _load_device(plan, dev, gather, matvec, matmul, experts)
     except BaseException as e:
         traceback.clear_frames(e.__traceback__)   # the frames' locals would keep the call's device memory alive
         raise
@@ -789,7 +857,7 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None,
         setattr(module, _ATTR, None)
     else:
         _commit(module, state, prefetch)
-    return _with_prefetch(report, state, prefetch, gather, matvec, matmul)
+    return _with_prefetch(report, state, prefetch, gather, matvec, matmul, experts)
 
 
 def save_module(module: torch.nn.Module, filename, metadata=None) -> None:
