@@ -47,20 +47,6 @@ constexpr int kMatmulMaxTokens = 64;
 constexpr int kMatmulTileRows = 8;    // W rows per tile: n of the mma
 constexpr int kMatmulGroupCols = 128;  // 4 column steps of 32
 
-struct MatmulCfg {
-  const DecodeCfg* cfg;   // the item's piece, in plan memory
-  SegEntry* seg;          // the piece's segment index
-  uint32_t* error;        // the plan's error word
-  const void* x;
-  const void* bias;       // or nullptr
-  void* y;
-  float* part;            // the partial sums (scratch)
-  uint64_t in, out;       // features
-  uint64_t xs, ys;        // row strides of x and y, in elements
-  uint64_t ce, total, K;  // elements of a full chunk and of the tensor; chunks
-  uint32_t nt, rt;        // tokens; row tiles per quarter in the slot layout
-};
-
 // Row tiles a quarter of q elements may touch, wherever it starts (rows of `in` elements).
 __host__ __device__ inline uint64_t matmul_quarter_tiles(uint64_t q, uint64_t in, uint64_t out) {
   return (matvec_block_rows(q, in, out) + kMatmulTileRows - 1) / kMatmulTileRows;
@@ -83,7 +69,7 @@ __device__ __forceinline__ void mma_16816(float (&d)[4], uint32_t a0, uint32_t a
 template <int DT, int MT>
 struct MatmulEp {
   static constexpr bool on = true;
-  MatmulCfg m;
+  ProductCfg m;
 
   template <int G>
   __device__ __forceinline__ void quarter(const SyncShared& S, uint64_t c, int stream, uint32_t out_off, uint32_t count, bool rot) const {
@@ -176,48 +162,26 @@ struct MatmulEp {
 static_assert(sizeof(((SyncShared*)0)->sbuf) >= (kSyncThreads / 32) * kMatmulTileRows * kMatmulMaxTokens * sizeof(float),
               "the warps' sums of a tile fit in the stream buffer");
 
-// One CTA per coded bitstream of the item (every chunk is fused: its one coded item is the top byte plane).
 template <int DT, int MT>
-__global__ void __launch_bounds__(kSyncThreads, 3) k_matmul(MatmulCfg m) {
-  extern __shared__ __align__(1024) unsigned char smem_raw[];
-  const SyncCarve cv = sync_carve(smem_raw);
-  SyncShared& S = *cv.S;
-  const DecodeCfg& cfg = *m.cfg;
-  const MatmulEp<DT, MT> ep{m};
-  const uint64_t works = 4ull * cfg.ctrl->huf_count;
-  for (uint64_t work = blockIdx.x; work < works; work += gridDim.x) {
-    __syncthreads();  // the previous bitstream's shared state is dead
-    sync_process<2, false, kSyncReplay, false, MatmulEp<DT, MT>>(cfg, nullptr, S, cv.lut, cv.lut_s, work, m.seg + work * kSyncThreads, nullptr,
-                                                                  &ep);
-  }
+__global__ void __launch_bounds__(kSyncThreads, 3) k_matmul(ProductCfg m) {
+  product_streams<2>(m, MatmulEp<DT, MT>{m});
 }
 
 template <int DT>
-__global__ void __launch_bounds__(256) k_matmul_reduce(MatmulCfg m) {
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    const uint32_t e = *(volatile uint32_t*)&m.cfg->ctrl->error;  // a decode error of this call
-    if (e) atomicOr(m.error, e);
-  }
-  const uint64_t idx = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  if (idx >= m.out * m.nt) return;
-  const uint64_t t = idx / m.out, o = idx - t * m.out;
-  float s = 0.f;
-  for (uint64_t e = o * m.in; e < (o + 1) * m.in;) {
-    const uint64_t c = e / m.ce;
-    const uint64_t q = (c == m.K - 1 ? m.total - c * m.ce : m.ce) / 4;
-    const uint64_t st = (e - c * m.ce) / q;
-    const uint64_t qs = c * m.ce + st * q;
-    const uint64_t r = o - qs / m.in;  // the row within the quarter's rows
-    s += m.part[((((c * 4 + st) * m.rt + r / kMatmulTileRows) * m.nt + t) * kMatmulTileRows) + r % kMatmulTileRows];
-    e = qs + q;
-  }
-  if (DT == kMvBf16) {
-    if (m.bias) s += __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(m.bias)[o]);
-    reinterpret_cast<__nv_bfloat16*>(m.y)[t * m.ys + o] = __float2bfloat16_rn(s);
-  } else {
-    if (m.bias) s += __half2float(reinterpret_cast<const __half*>(m.bias)[o]);
-    reinterpret_cast<__half*>(m.y)[t * m.ys + o] = __float2half_rn(s);
-  }
+__global__ void __launch_bounds__(256) k_matmul_reduce(ProductCfg m) {
+  product_reduce<DT>(m, [&](uint64_t t, uint64_t o) {
+    float s = 0.f;
+    for (uint64_t e = o * m.in; e < (o + 1) * m.in;) {
+      const uint64_t c = e / m.ce;
+      const uint64_t q = (c == m.K - 1 ? m.total - c * m.ce : m.ce) / 4;
+      const uint64_t st = (e - c * m.ce) / q;
+      const uint64_t qs = c * m.ce + st * q;
+      const uint64_t r = o - qs / m.in;  // the row within the quarter's rows
+      s += m.part[((((c * 4 + st) * m.rt + r / kMatmulTileRows) * m.nt + t) * kMatmulTileRows) + r % kMatmulTileRows];
+      e = qs + q;
+    }
+    return s;
+  });
 }
 
 }  // namespace zb

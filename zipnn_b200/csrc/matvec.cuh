@@ -34,7 +34,8 @@ constexpr int kMatvecMaxTokens = 8;
 enum : int { kMvBf16 = 0, kMvFp16 = 1, kMvFp32 = 2 };
 __host__ __device__ constexpr int matvec_esize(int dt) { return dt == kMvFp32 ? 4 : 2; }
 
-struct MatvecCfg {
+// The launch arguments of k_matvec and k_matmul and of their reduce kernels.
+struct ProductCfg {
   const DecodeCfg* cfg;   // the item's piece, in plan memory
   SegEntry* seg;          // the piece's segment index
   uint32_t* error;        // the plan's error word
@@ -45,8 +46,9 @@ struct MatvecCfg {
   uint64_t in, out;       // features
   uint64_t xs, ys;        // row strides of x and y, in elements
   uint64_t ce, total, K;  // elements of a full chunk and of the tensor; chunks
-  uint32_t esize, nt, rs; // element bytes, tokens, slots (rows) per block
-  uint32_t step_rows, step_cols;  // one 32-vector step as whole rows + columns
+  uint32_t esize, nt, rs; // element bytes, tokens, slots (rows) per block of the matvec
+  uint32_t step_rows, step_cols;  // one 32-vector step of the matvec as whole rows + columns
+  uint32_t rt;            // row tiles per quarter in the matmul's slot layout
 };
 
 // Elements of a block of a chunk with n elements: a quarter's vectors split over 8 warps, in whole 32-vector steps.
@@ -63,7 +65,7 @@ __host__ __device__ inline uint64_t matvec_block_rows(uint64_t be, uint64_t in, 
 struct MatvecBlock {
   uint64_t id, start, end;
 };
-__device__ __forceinline__ MatvecBlock matvec_block_of(const MatvecCfg& m, uint64_t e) {
+__device__ __forceinline__ MatvecBlock matvec_block_of(const ProductCfg& m, uint64_t e) {
   const uint64_t c = e / m.ce;
   const uint64_t n = c == m.K - 1 ? m.total - c * m.ce : m.ce;
   const uint64_t q = n / 4, be = matvec_block_elems(n, m.esize);
@@ -99,7 +101,7 @@ template <int DT, int NT>
 struct MatvecEp {
   static constexpr bool on = true;
   static constexpr int EPV = 16 / matvec_esize(DT);
-  MatvecCfg m;
+  ProductCfg m;
 
   __device__ __forceinline__ void flush(float (&acc)[NT], float* slot, int lane) const {
 #pragma unroll
@@ -185,24 +187,25 @@ struct MatvecEp {
   }
 };
 
-// One CTA per coded bitstream of the item (every chunk is fused: its one coded item is the top byte plane).
-template <int DT, int NT>
-__global__ void __launch_bounds__(kSyncThreads, 3) k_matvec(MatvecCfg m) {
+// The bitstream loop of k_matvec and k_matmul: one CTA per coded bitstream of the item (every chunk is fused: its one
+// coded item is the top byte plane), each decoded as by a plan run, with the epilogue's `quarter` in place of its stores.
+template <int G, typename Ep>
+__device__ __forceinline__ void product_streams(const ProductCfg& m, const Ep& ep) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const SyncCarve cv = sync_carve(smem_raw);
   SyncShared& S = *cv.S;
   const DecodeCfg& cfg = *m.cfg;
-  const MatvecEp<DT, NT> ep{m};
   const uint64_t works = 4ull * cfg.ctrl->huf_count;
   for (uint64_t work = blockIdx.x; work < works; work += gridDim.x) {
     __syncthreads();  // the previous bitstream's shared state is dead
-    sync_process<matvec_esize(DT), false, kSyncReplay, false, MatvecEp<DT, NT>>(cfg, nullptr, S, cv.lut, cv.lut_s, work, m.seg + work * kSyncThreads,
-                                                                                nullptr, &ep);
+    sync_process<G, false, kSyncReplay, false, Ep>(cfg, nullptr, S, cv.lut, cv.lut_s, work, m.seg + work * kSyncThreads, nullptr, &ep);
   }
 }
 
-template <int DT>
-__global__ void __launch_bounds__(256) k_matvec_reduce(MatvecCfg m) {
+// The reduce kernels' frame: one thread per (token t, output row o).  sum(t, o) adds the row's partial sums in
+// ascending element order; the bias is added, the result rounded once to the output type and stored.
+template <int DT, typename Sum>
+__device__ __forceinline__ void product_reduce(const ProductCfg& m, Sum&& sum) {
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     const uint32_t e = *(volatile uint32_t*)&m.cfg->ctrl->error;  // a decode error of this call
     if (e) atomicOr(m.error, e);
@@ -210,12 +213,7 @@ __global__ void __launch_bounds__(256) k_matvec_reduce(MatvecCfg m) {
   const uint64_t idx = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   if (idx >= m.out * m.nt) return;
   const uint64_t t = idx / m.out, o = idx - t * m.out;
-  float s = 0.f;
-  for (uint64_t e = o * m.in; e < (o + 1) * m.in;) {
-    const MatvecBlock b = matvec_block_of(m, e);
-    s += m.part[((b.id * m.rs) + o - b.start / m.in) * m.nt + t];
-    e = b.end;
-  }
+  float s = sum(t, o);
   if (DT == kMvBf16) {
     if (m.bias) s += __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(m.bias)[o]);
     reinterpret_cast<__nv_bfloat16*>(m.y)[t * m.ys + o] = __float2bfloat16_rn(s);
@@ -226,6 +224,24 @@ __global__ void __launch_bounds__(256) k_matvec_reduce(MatvecCfg m) {
     if (m.bias) s += reinterpret_cast<const float*>(m.bias)[o];
     reinterpret_cast<float*>(m.y)[t * m.ys + o] = s;
   }
+}
+
+template <int DT, int NT>
+__global__ void __launch_bounds__(kSyncThreads, 3) k_matvec(ProductCfg m) {
+  product_streams<matvec_esize(DT)>(m, MatvecEp<DT, NT>{m});
+}
+
+template <int DT>
+__global__ void __launch_bounds__(256) k_matvec_reduce(ProductCfg m) {
+  product_reduce<DT>(m, [&](uint64_t t, uint64_t o) {
+    float s = 0.f;
+    for (uint64_t e = o * m.in; e < (o + 1) * m.in;) {
+      const MatvecBlock b = matvec_block_of(m, e);
+      s += m.part[((b.id * m.rs) + o - b.start / m.in) * m.nt + t];
+      e = b.end;
+    }
+    return s;
+  });
 }
 
 }  // namespace zb

@@ -166,6 +166,14 @@ bool smem_attr(Kernel k, size_t smem) {
   }) > 0;
 }
 
+// A grid of at most `want` CTAs of kernel k that are all resident at once on the current device.  0: the runtime
+// refused the shared-memory limit (smem_attr).
+template <typename Kernel>
+unsigned resident_grid(Kernel k, size_t smem, int threads, uint64_t want) {
+  if (!smem_attr(k, smem)) return 0;
+  return (unsigned)std::min<uint64_t>(want, (uint64_t)resident_blocks(k, smem, threads) * sm_count_cached());
+}
+
 // ---- small pinned host blocks for the results a call reads back -------------------------------------------------
 // A device-to-host copy into pageable memory is staged by the driver and holds the host for longer; into pinned
 // memory it is one DMA, and the caller waits once, on the stream.  Blocks are taken per call and given back, so
@@ -381,6 +389,9 @@ constexpr uint64_t kDefaultSlots = 64;
 constexpr uint64_t kSyncTablesMaxChunks = 16384;  // largest tensor the sync decoder can be asked to take (ZIPNN_B200_SYNC_MAX is clamped to it)
 constexpr uint64_t kSyncDefaultMaxChunks = 3072;  // crossover with the one-thread-per-bitstream kernels for one- and two-plane types
                                                   // (H100 SXM at 400 W: they win up to 3072 chunks and lose from 3584 on)
+// Plane-pool slots of the default workspace of K chunks: one per chunk up to kDefaultSlots, else the pool and the
+// overflow CTAs' slots.
+inline uint64_t pool_slots(uint64_t K) { return K <= kDefaultSlots ? K : kDefaultSlots + kOverflowCtas; }
 struct DecWs {
   size_t items_off, mode_off, slot_off, rlist_off, olist_off, hlist_off, tables_off, fill_off, planes_off, pstride, fixed;
 };
@@ -496,9 +507,7 @@ int zipnn_b200_compress_bound(size_t n, int num_buf, size_t chunk, size_t hdr_le
 int zipnn_b200_decompress_workspace_size(size_t orig, int num_buf, size_t chunk, size_t* out) {
   if (!out || chunk == 0 || !(num_buf == 1 || num_buf == 2 || num_buf == 4)) return ZIPNN_B200_E_ARG;
   const DecWs L = dec_ws_layout(orig, num_buf, chunk);
-  const uint64_t K = num_chunks(orig, chunk);
-  const uint64_t slots = K <= kDefaultSlots ? K : kDefaultSlots + kOverflowCtas;
-  *out = L.fixed + (size_t)slots * num_buf * L.pstride;
+  *out = L.fixed + (size_t)pool_slots(num_chunks(orig, chunk)) * num_buf * L.pstride;
   return ZIPNN_B200_OK;
 }
 
@@ -592,9 +601,8 @@ int zipnn_b200_decompress(const void* d_body, size_t body_len, int num_buf, int 
   if (use_sync) {
     int rc = dispatch_G(G, [&](auto g) -> int {
       constexpr int GG = decltype(g)::value;
-      if (!smem_attr(k_huf_decode_sync<GG>, kSyncSmemBytes)) return ZIPNN_B200_E_CUDA;
-      const int nb = resident_blocks(k_huf_decode_sync<GG>, kSyncSmemBytes, kSyncThreads);
-      const unsigned grid = (unsigned)std::min<uint64_t>(4 * nitems, (uint64_t)nb * sm_count_cached());
+      const unsigned grid = resident_grid(k_huf_decode_sync<GG>, kSyncSmemBytes, kSyncThreads, 4 * nitems);
+      if (!grid) return ZIPNN_B200_E_CUDA;
       {
         ScopedTimer tp(kKParseTables, st);
         k_parse_tables<<<(unsigned)((nitems + kParseWarps - 1) / kParseWarps), kParseWarps * 32, 0, st>>>(cfg);
@@ -728,17 +736,37 @@ struct BatchGrid {
   uint64_t chunks, items, tiles, max_ovf;  // chunk_start[n], item_start[n], tile_start[n]; overflow CTAs per tensor
 };
 
-static int batch_prepare(const std::vector<DecodeCfg>& cfgs, const std::vector<uint64_t>& starts, int n, uint8_t* ws, uint64_t max_ovf,
-                         cudaStream_t st, BatchCfg& B, BatchGrid& grid) {
-  grid.chunks = starts[n];
-  grid.items = starts[2 * (n + 1) - 1];
-  grid.tiles = starts[3 * (n + 1) - 1];
-  grid.max_ovf = max_ovf;
+// The descriptors of a batch of n pieces, as batch_prepare copies them behind the error word: a DecodeCfg per piece,
+// then chunk_start, item_start and tile_start (n + 1 each: prefix sums of the chunks, coded-bitstream items and merge
+// tiles the batch kernels take from each piece).
+struct BatchDescs {
+  int n;
+  std::vector<DecodeCfg> cfgs;
+  std::vector<uint64_t> starts;
+  uint64_t max_ovf;  // overflow CTAs per piece: the largest ovf_slots of a piece with chunks, at least the start value
+  BatchDescs(int n_, uint64_t max_ovf_) : n(n_), starts(3 * ((size_t)n_ + 1), 0), max_ovf(max_ovf_) { cfgs.reserve((size_t)n_); }
+  uint64_t start(int array, int j) const { return starts[(size_t)array * (n + 1) + j]; }
+  // The next piece: cfg, of which the batch kernels decode kc chunks (0: none, the piece is only a descriptor).
+  void add(const DecodeCfg& cfg, uint64_t kc) {
+    const size_t j = cfgs.size();
+    cfgs.push_back(cfg);
+    const uint64_t counts[3] = {kc, 4ull * cfg.G * kc, kc * ((cfg.chunk + kMergeTile - 1) / kMergeTile)};
+    for (int a = 0; a < 3; a++) starts[(size_t)a * (n + 1) + j + 1] = starts[(size_t)a * (n + 1) + j] + counts[a];
+    if (kc) max_ovf = std::max<uint64_t>(max_ovf, cfg.ovf_slots);
+  }
+};
+
+static int batch_prepare(const BatchDescs& D, uint8_t* ws, cudaStream_t st, BatchCfg& B, BatchGrid& grid) {
+  const int n = D.n;
+  grid.chunks = D.start(0, n);
+  grid.items = D.start(1, n);
+  grid.tiles = D.start(2, n);
+  grid.max_ovf = D.max_ovf;
   // descriptors to the device (pageable source: the copy is staged before the call returns)
   uint8_t* d_cfgs = ws + 256;
   uint8_t* d_starts = d_cfgs + sizeof(DecodeCfg) * (size_t)n;
-  ZB_CUDA(cudaMemcpyAsync(d_cfgs, cfgs.data(), sizeof(DecodeCfg) * (size_t)n, cudaMemcpyHostToDevice, st));
-  ZB_CUDA(cudaMemcpyAsync(d_starts, starts.data(), sizeof(uint64_t) * starts.size(), cudaMemcpyHostToDevice, st));
+  ZB_CUDA(cudaMemcpyAsync(d_cfgs, D.cfgs.data(), sizeof(DecodeCfg) * (size_t)n, cudaMemcpyHostToDevice, st));
+  ZB_CUDA(cudaMemcpyAsync(d_starts, D.starts.data(), sizeof(uint64_t) * D.starts.size(), cudaMemcpyHostToDevice, st));
   B.cfgs = (const DecodeCfg*)d_cfgs;
   B.chunk_start = (const uint64_t*)d_starts;
   B.item_start = B.chunk_start + (n + 1);
@@ -765,9 +793,8 @@ static int batch_prepare(const std::vector<DecodeCfg>& cfgs, const std::vector<u
 // The sync decoder of a decode plan: record (create) or replay (run) of the segment starts.
 extern "C++" template <int M>
 int launch_sync_plan(const BatchCfg& B, const SegIndex& X, uint64_t items, cudaStream_t st) {
-  if (!smem_attr(k_huf_decode_sync_plan<M>, kSyncSmemBytes)) return ZIPNN_B200_E_CUDA;
-  const int nb = resident_blocks(k_huf_decode_sync_plan<M>, kSyncSmemBytes, kSyncThreads);
-  const unsigned blocks = (unsigned)std::min<uint64_t>(items, (uint64_t)nb * sm_count_cached());
+  const unsigned blocks = resident_grid(k_huf_decode_sync_plan<M>, kSyncSmemBytes, kSyncThreads, items);
+  if (!blocks) return ZIPNN_B200_E_CUDA;
   ScopedTimer tm(kKHufDecodeSync, st);
   k_huf_decode_sync_plan<M><<<blocks, kSyncThreads, kSyncSmemBytes, st>>>(B, X);
   ZB_LAUNCHED();
@@ -783,9 +810,8 @@ static int batch_decode(const BatchCfg& B, const BatchGrid& grid, cudaStream_t s
     const int rc = mode == kSyncRecord ? launch_sync_plan<kSyncRecord>(B, *X, grid.items, st) : launch_sync_plan<kSyncReplay>(B, *X, grid.items, st);
     if (rc) return rc;
   } else {
-    if (!smem_attr(k_huf_decode_sync_batch, kSyncSmemBytes)) return ZIPNN_B200_E_CUDA;
-    const int nb = resident_blocks(k_huf_decode_sync_batch, kSyncSmemBytes, kSyncThreads);
-    const unsigned blocks = (unsigned)std::min<uint64_t>(grid.items, (uint64_t)nb * sms);
+    const unsigned blocks = resident_grid(k_huf_decode_sync_batch, kSyncSmemBytes, kSyncThreads, grid.items);
+    if (!blocks) return ZIPNN_B200_E_CUDA;
     ScopedTimer tm(kKHufDecodeSync, st);
     k_huf_decode_sync_batch<<<blocks, kSyncThreads, kSyncSmemBytes, st>>>(B);
     ZB_LAUNCHED();
@@ -811,10 +837,9 @@ static int batch_errors(const BatchCfg& B, cudaStream_t st) {
   return ZIPNN_B200_OK;
 }
 
-static int run_batch_kernels(const std::vector<DecodeCfg>& cfgs, const std::vector<uint64_t>& starts, int n, uint8_t* ws, uint64_t max_ovf,
-                             cudaStream_t st, BatchCfg& B) {
+static int run_batch_kernels(const BatchDescs& D, uint8_t* ws, cudaStream_t st, BatchCfg& B) {
   BatchGrid grid;
-  const int rc = batch_prepare(cfgs, starts, n, ws, max_ovf, st, B, grid);
+  const int rc = batch_prepare(D, ws, st, B, grid);
   return rc ? rc : batch_decode(B, grid, st);
 }
 
@@ -825,51 +850,41 @@ int zipnn_b200_decompress_batch(const zipnn_b200_batch_item* items, int n, void*
   uint8_t* ws = (uint8_t*)d_ws;
   const size_t hdr = batch_header_bytes(n);
   if (ws_bytes < hdr) return ZIPNN_B200_E_CAPACITY;
-  std::vector<DecodeCfg> cfgs((size_t)n);
-  std::vector<uint64_t> starts(3 * ((size_t)n + 1), 0);
-  uint64_t* chunk_start = starts.data();
-  uint64_t* item_start = chunk_start + (n + 1);
-  uint64_t* tile_start = item_start + (n + 1);
+  BatchDescs D(n, 0);
   size_t at = hdr;
   std::vector<int> big;  // tensors that go through the single-tensor path on the same stream
-  uint64_t max_ovf = 0;
   ZB_CUDA(cudaMemsetAsync(ws, 0, 256, st));
   for (int i = 0; i < n; i++) {
     const zipnn_b200_batch_item& it = items[i];
     if (!valid_layout(it.num_buf, it.bytes_mode, it.chunk)) return ZIPNN_B200_E_ARG;
     const size_t slice = batch_slice_bytes(it);
     if (at + slice > ws_bytes) return ZIPNN_B200_E_CAPACITY;
-    chunk_start[i + 1] = chunk_start[i];
-    item_start[i + 1] = item_start[i];
-    tile_start[i + 1] = tile_start[i];
-    memset(&cfgs[i], 0, sizeof(DecodeCfg));
-    cfgs[i].ctrl = (Ctrl*)ws;  // (never raised: an empty tensor has no kernel work)
-    if (it.orig == 0) continue;
+    DecodeCfg cfg;
+    memset(&cfg, 0, sizeof(DecodeCfg));
+    cfg.ctrl = (Ctrl*)ws;  // (never raised: an empty tensor has no kernel work)
+    if (it.orig == 0) {
+      D.add(cfg, 0);
+      continue;
+    }
     if (!it.d_body || !it.d_out || ((uintptr_t)it.d_out & 15)) return ZIPNN_B200_E_ARG;
     const uint64_t K = num_chunks(it.orig, it.chunk);
     const bool small = K <= sync_max_chunks(it.num_buf);
-    const int rc = fill_decode_cfg(cfgs[i], it.d_body, it.body_len, it.num_buf, it.bits_mode, it.chunk, it.orig, it.d_out, ws + at, slice, small);
+    const int rc = fill_decode_cfg(cfg, it.d_body, it.body_len, it.num_buf, it.bits_mode, it.chunk, it.orig, it.d_out, ws + at, slice, small);
     if (rc) return rc;
     ZB_CUDA(cudaMemsetAsync(ws + at, 0, kCtrlBytes, st));
-    if (small) {
-      chunk_start[i + 1] += K;
-      item_start[i + 1] += 4ull * it.num_buf * K;
-      tile_start[i + 1] += K * ((it.chunk + kMergeTile - 1) / kMergeTile);
-      max_ovf = std::max<uint64_t>(max_ovf, cfgs[i].ovf_slots);
-    } else {
-      big.push_back(i);
-    }
+    D.add(cfg, small ? K : 0);
+    if (!small) big.push_back(i);
     at += slice;
   }
   BatchCfg B;
   {
-    const int rc = run_batch_kernels(cfgs, starts, n, ws, max_ovf, st, B);
+    const int rc = run_batch_kernels(D, ws, st, B);
     if (rc) return rc;
   }
   for (int i : big) {
     const zipnn_b200_batch_item& it = items[i];
     const int rc = zipnn_b200_decompress(it.d_body, it.body_len, it.num_buf, it.bits_mode, it.bytes_mode, it.chunk, it.orig, it.d_out,
-                                         (void*)cfgs[i].ctrl, batch_slice_bytes(it), st, 0);
+                                         (void*)D.cfgs[i].ctrl, batch_slice_bytes(it), st, 0);
     if (rc) return rc;
   }
   {
@@ -947,8 +962,18 @@ int plan_slices(const zipnn_b200_slice_item* items, int n, std::vector<SlicePiec
 size_t slice_piece_bytes(const zipnn_b200_slice_item& it, const SlicePiece& p) {
   const uint64_t kc = p.c1 - p.c0;
   const DecWs L = dec_ws_layout(it.orig, it.num_buf, it.chunk, kc);
-  const uint64_t slots = kc <= kDefaultSlots ? kc : kDefaultSlots + kOverflowCtas;
-  return round_up(L.fixed + (size_t)slots * it.num_buf * L.pstride, 256);
+  return round_up(L.fixed + (size_t)pool_slots(kc) * it.num_buf * L.pstride, 256);
+}
+// The piece's box as the window of cfg: the decoders write only its bytes, packed, and start at chunk p.c0.
+void set_box(DecodeCfg& cfg, const SlicePiece& p) {
+  cfg.box_base = p.base;
+  cfg.box_rows = p.rows;
+  cfg.box_pitch = p.pitch;
+  cfg.box_len = p.len;
+  cfg.box_step_rows = kBoxStep / p.pitch;
+  cfg.box_step_cols = kBoxStep % p.pitch;
+  cfg.box_fast = ((p.base | p.pitch | p.len) & 15) == 0;
+  cfg.c0 = p.c0;
 }
 }  // namespace
 
@@ -976,12 +1001,7 @@ int zipnn_b200_decompress_slices(const zipnn_b200_slice_item* items, int n, void
   uint8_t* ws = (uint8_t*)d_ws;
   size_t at = batch_header_bytes(np);
   if (ws_bytes < at) return ZIPNN_B200_E_CAPACITY;
-  std::vector<DecodeCfg> cfgs((size_t)np);
-  std::vector<uint64_t> starts(3 * ((size_t)np + 1), 0);
-  uint64_t* chunk_start = starts.data();
-  uint64_t* item_start = chunk_start + (np + 1);
-  uint64_t* tile_start = item_start + (np + 1);
-  uint64_t max_ovf = 1;  // the overflow kernel always runs (its CTAs return at once when no piece has overflow slots): a fixed launch count
+  BatchDescs D(np, 1);  // the overflow kernel always runs (its CTAs return at once when no piece has overflow slots): a fixed launch count
   ZB_CUDA(cudaMemsetAsync(ws, 0, 256, st));
   for (int j = 0; j < np; j++) {
     const SlicePiece& p = pieces[j];
@@ -989,28 +1009,18 @@ int zipnn_b200_decompress_slices(const zipnn_b200_slice_item* items, int n, void
     const size_t slice = slice_piece_bytes(it, p);
     if (at + slice > ws_bytes) return ZIPNN_B200_E_CAPACITY;
     const uint64_t kc = p.c1 - p.c0;
-    DecodeCfg& cfg = cfgs[j];
+    DecodeCfg cfg;
     const int rc = fill_decode_cfg(cfg, it.d_body, it.body_len, it.num_buf, it.bits_mode, it.chunk, it.orig, (uint8_t*)it.d_out + p.out_off,
                                    ws + at, slice, true, kc);
     if (rc) return rc;
-    cfg.box_base = p.base;
-    cfg.box_rows = p.rows;
-    cfg.box_pitch = p.pitch;
-    cfg.box_len = p.len;
-    cfg.box_step_rows = kBoxStep / p.pitch;
-    cfg.box_step_cols = kBoxStep % p.pitch;
-    cfg.box_fast = ((p.base | p.pitch | p.len) & 15) == 0;
-    cfg.c0 = p.c0;
+    set_box(cfg, p);
     ZB_CUDA(cudaMemsetAsync(ws + at, 0, kCtrlBytes, st));
-    chunk_start[j + 1] = chunk_start[j] + kc;
-    item_start[j + 1] = item_start[j] + 4ull * it.num_buf * kc;
-    tile_start[j + 1] = tile_start[j] + kc * ((it.chunk + kMergeTile - 1) / kMergeTile);
-    max_ovf = std::max<uint64_t>(max_ovf, cfg.ovf_slots);
+    D.add(cfg, kc);
     at += slice;
   }
   BatchCfg B;
   {
-    const int rc = run_batch_kernels(cfgs, starts, np, ws, max_ovf, st, B);
+    const int rc = run_batch_kernels(D, ws, st, B);
     if (rc) return rc;
   }
   {
@@ -1062,13 +1072,25 @@ size_t plan_piece_meta_bytes(const zipnn_b200_slice_item& it, const SlicePiece& 
 size_t plan_piece_scratch_bytes(const zipnn_b200_slice_item& it, const SlicePiece& p) {
   const uint64_t kc = p.c1 - p.c0;
   const DecWs L = dec_ws_layout(it.orig, it.num_buf, it.chunk, kc);
-  const uint64_t slots = kc <= kDefaultSlots ? kc : kDefaultSlots + kOverflowCtas;
-  return round_up((size_t)slots * it.num_buf * L.pstride, 256);
+  return round_up((size_t)pool_slots(kc) * it.num_buf * L.pstride, 256);
 }
 bool plan_state(const zipnn_b200_decode_plan* plan, PlanState& s) {
   if (!plan) return false;
   memcpy(&s, plan->opaque, sizeof(s));
   return s.magic == kPlanMagic;
+}
+constexpr int64_t kAllItems = INT64_MIN;  // (no int item is)
+// f(items) on the host records of plan s, under g_plan_mu: every read and write of g_plan_items happens here.  E_ARG
+// for a plan whose memory a later create has taken, and unless `item` is kAllItems, for an item the plan does not have.
+extern "C++" template <typename F>
+int with_plan_items(const PlanState& s, int64_t item, F&& f) {
+  std::lock_guard<std::mutex> lk(g_plan_mu);
+  const auto it = g_plan_items.find((uintptr_t)s.B.error_out);
+  if (it == g_plan_items.end() || it->second.gen != s.gen) return ZIPNN_B200_E_ARG;
+  std::vector<GatherItem>& items = it->second.items;
+  if (item != kAllItems && (item < 0 || (uint64_t)item >= items.size())) return ZIPNN_B200_E_ARG;
+  f(items);
+  return ZIPNN_B200_OK;
 }
 struct PlanLayout {
   std::vector<SlicePiece> pieces;
@@ -1150,37 +1172,20 @@ int zipnn_b200_decode_plan_create(const zipnn_b200_slice_item* items, int n, voi
   uint8_t* meta = (uint8_t*)d_plan;
   uint8_t* scratch = (uint8_t*)d_scratch;
   size_t at = P.metas_off, sat = 0;
-  std::vector<DecodeCfg> cfgs((size_t)np);
-  std::vector<uint64_t> starts(3 * ((size_t)np + 1), 0);
-  uint64_t* chunk_start = starts.data();
-  uint64_t* item_start = chunk_start + (np + 1);
-  uint64_t* tile_start = item_start + (np + 1);
-  uint64_t max_ovf = 1;  // (as in the slice call: a fixed launch count)
+  BatchDescs D(np, 1);  // (as in the slice call: a fixed launch count)
   for (int j = 0; j < np; j++) {
     const SlicePiece& p = P.pieces[j];
     const zipnn_b200_slice_item& it = items[p.item];
     const size_t mb = plan_piece_meta_bytes(it, p), sb = plan_piece_scratch_bytes(it, p);
     const uint64_t kc = p.c1 - p.c0;
-    DecodeCfg& cfg = cfgs[j];
+    DecodeCfg cfg;
     const int rc = fill_decode_cfg(cfg, it.d_body, it.body_len, it.num_buf, it.bits_mode, it.chunk, it.orig, (uint8_t*)it.d_out + p.out_off,
                                    meta + at, mb, true, kc, scratch + sat, sb);
     if (rc) return rc;
     // a piece that is a whole tensor decodes without the window, as in the batch call
     const bool whole = p.base == 0 && p.rows == 1 && p.len == it.orig;
-    if (!whole) {
-      cfg.box_base = p.base;
-      cfg.box_rows = p.rows;
-      cfg.box_pitch = p.pitch;
-      cfg.box_len = p.len;
-      cfg.box_step_rows = kBoxStep / p.pitch;
-      cfg.box_step_cols = kBoxStep % p.pitch;
-      cfg.box_fast = ((p.base | p.pitch | p.len) & 15) == 0;
-      cfg.c0 = p.c0;
-    }
-    chunk_start[j + 1] = chunk_start[j] + kc;
-    item_start[j + 1] = item_start[j] + 4ull * it.num_buf * kc;
-    tile_start[j + 1] = tile_start[j] + kc * ((it.chunk + kMergeTile - 1) / kMergeTile);
-    max_ovf = std::max<uint64_t>(max_ovf, cfg.ovf_slots);
+    if (!whole) set_box(cfg, p);
+    D.add(cfg, kc);
     at += mb;
     sat += sb;
   }
@@ -1194,7 +1199,7 @@ int zipnn_b200_decode_plan_create(const zipnn_b200_slice_item* items, int n, voi
   s.coded = P.seg_base[np] / kSegPerItem;
   s.mode = P.replay ? kSyncReplay : kSyncDecode;
   {
-    int rc = batch_prepare(cfgs, starts, np, meta, max_ovf, st, s.B, s.grid);
+    int rc = batch_prepare(D, meta, st, s.B, s.grid);
     if (!rc) rc = batch_decode(s.B, s.grid, st, P.replay ? kSyncRecord : kSyncDecode, &s.X);
     if (!rc) rc = batch_errors(s.B, st);
     if (!rc) rc = read_ctrl_error(meta, st);
@@ -1214,7 +1219,7 @@ int zipnn_b200_decode_plan_create(const zipnn_b200_slice_item* items, int n, voi
       const bool whole = p.base == 0 && p.rows == 1 && p.len == it.orig;
       g.piece = whole && g.piece == -1 ? j : -2;   // (-2: a box or a split item; the pieces of an item are consecutive)
       g.seg_base = P.seg_base[j];
-      g.d_mode = cfgs[j].mode;
+      g.d_mode = D.cfgs[j].mode;
     }
     for (GatherItem& g : rec.items)
       if (g.piece < 0) g.piece = -1;
@@ -1247,13 +1252,12 @@ int zipnn_b200_decode_plan_run_shifted(const zipnn_b200_decode_plan* plan, int64
   PlanState s;
   if (!plan_state(plan, s) || (out_shift & 15)) return ZIPNN_B200_E_ARG;
   if (s.mode != kSyncReplay) return ZIPNN_B200_E_UNSUPPORTED;
-  if (!smem_attr(k_plan_replay_persistent, kPlanReplaySmemBytes)) return ZIPNN_B200_E_CUDA;
-  const int nb = resident_blocks(k_plan_replay_persistent, kPlanReplaySmemBytes, kSyncThreads);
   // more CTAs than units (or than the overflow CTAs a tensor may use) would only claim nothing
-  const uint64_t limit = (uint64_t)nb * sm_count_cached();
   const uint64_t useful = std::max<uint64_t>(std::max<uint64_t>(1, s.grid.items + s.grid.tiles), s.grid.max_ovf);
-  const uint64_t ctas = std::min<uint64_t>(max_ctas <= 0 ? limit : std::min<uint64_t>((uint64_t)max_ctas, limit), useful);
-  k_plan_replay_persistent<<<(unsigned)ctas, kSyncThreads, kPlanReplaySmemBytes, (cudaStream_t)cuda_stream>>>(s.B, s.X, out_shift);
+  const unsigned ctas = resident_grid(k_plan_replay_persistent, kPlanReplaySmemBytes, kSyncThreads,
+                                      max_ctas <= 0 ? useful : std::min<uint64_t>((uint64_t)max_ctas, useful));
+  if (!ctas) return ZIPNN_B200_E_CUDA;
+  k_plan_replay_persistent<<<ctas, kSyncThreads, kPlanReplaySmemBytes, (cudaStream_t)cuda_stream>>>(s.B, s.X, out_shift);
   ZB_LAUNCHED();
   return ZIPNN_B200_OK;
 }
@@ -1286,11 +1290,8 @@ uint64_t gather_span(uint64_t row_bytes, uint64_t chunk, uint64_t K) { return st
 int gather_item(const zipnn_b200_decode_plan* plan, int item, size_t row_bytes, PlanState& s, GatherItem& gi) {
   if (!plan_state(plan, s)) return ZIPNN_B200_E_ARG;
   {
-    std::lock_guard<std::mutex> lk(g_plan_mu);
-    const auto it = g_plan_items.find((uintptr_t)s.B.error_out);
-    if (it == g_plan_items.end() || it->second.gen != s.gen) return ZIPNN_B200_E_ARG;
-    if (item < 0 || (size_t)item >= it->second.items.size()) return ZIPNN_B200_E_ARG;
-    gi = it->second.items[(size_t)item];
+    const int rc = with_plan_items(s, item, [&](std::vector<GatherItem>& v) { gi = v[(size_t)item]; });
+    if (rc) return rc;
   }
   if (gi.piece < 0 || s.mode != kSyncReplay) return ZIPNN_B200_E_UNSUPPORTED;
   if (row_bytes == 0 || gi.orig % row_bytes) return ZIPNN_B200_E_ARG;
@@ -1352,15 +1353,13 @@ int zipnn_b200_decode_plan_gather(const zipnn_b200_decode_plan* plan, int item, 
   // passes: the distinct chunks are at most min(n * span, K), `slots` per pass (a bound of n alone, not of the ids)
   const uint64_t most = n_ids > gi.K / g.span ? gi.K : std::min<uint64_t>(gi.K, n_ids * g.span);
   const uint64_t passes = (most + slots - 1) / slots;
-  if (!smem_attr(k_gather_decode, kPlanReplaySmemBytes)) return ZIPNN_B200_E_CUDA;
-  const int nb = resident_blocks(k_gather_decode, kPlanReplaySmemBytes, kSyncThreads);
-  const int sms = sm_count_cached();
+  const unsigned dec_blocks = resident_grid(k_gather_decode, kPlanReplaySmemBytes, kSyncThreads, slots * 4 * gi.G);
+  if (!dec_blocks) return ZIPNN_B200_E_CUDA;
   const unsigned inv_blocks = (unsigned)std::max<uint64_t>(1, ((uint64_t)gi.G * gi.K + kGatherIndexThreads - 1) / kGatherIndexThreads);
   k_gather_index<<<1 + inv_blocks, kGatherIndexThreads, 0, st>>>(g);
   ZB_LAUNCHED();
-  const unsigned dec_blocks = (unsigned)std::min<uint64_t>(slots * 4 * gi.G, (uint64_t)nb * sms);
   const uint64_t units = n_ids * ((row_bytes + 15) / 16 + 1);
-  const unsigned row_blocks = (unsigned)std::min<uint64_t>((units + 255) / 256, (uint64_t)sms * 16);
+  const unsigned row_blocks = (unsigned)std::min<uint64_t>((units + 255) / 256, (uint64_t)sm_count_cached() * 16);
   for (uint64_t p = 0; p < passes; p++) {
     k_gather_decode<<<dec_blocks, kSyncThreads, kPlanReplaySmemBytes, st>>>(g, (uint32_t)p);
     ZB_LAUNCHED();
@@ -1395,10 +1394,8 @@ SelectLayout select_layout(const PlanState& s) {
 int select_items(const zipnn_b200_decode_plan* plan, size_t rows, PlanState& s, std::vector<GatherItem>& items) {
   if (!plan_state(plan, s)) return ZIPNN_B200_E_ARG;
   {
-    std::lock_guard<std::mutex> lk(g_plan_mu);
-    const auto it = g_plan_items.find((uintptr_t)s.B.error_out);
-    if (it == g_plan_items.end() || it->second.gen != s.gen) return ZIPNN_B200_E_ARG;
-    items = it->second.items;
+    const int rc = with_plan_items(s, kAllItems, [&](std::vector<GatherItem>& v) { items = v; });
+    if (rc) return rc;
   }
   if (s.mode != kSyncReplay || items.empty() || items.size() > 65535) return ZIPNN_B200_E_UNSUPPORTED;  // (grid.y of the overflow)
   for (const GatherItem& gi : items)
@@ -1456,19 +1453,18 @@ int zipnn_b200_decode_plan_run_select(const zipnn_b200_decode_plan* plan, size_t
     tiles += m * ((gi.chunk + kMergeTile - 1) / kMergeTile);
     most = std::max(most, m);
   }
-  if (!smem_attr(k_select_sync, kSyncSmemBytes)) return ZIPNN_B200_E_CUDA;
-  const int nb = resident_blocks(k_select_sync, kSyncSmemBytes, kSyncThreads);
-  const int sms = sm_count_cached();
+  const unsigned sync_blocks = resident_grid(k_select_sync, kSyncSmemBytes, kSyncThreads, bitstreams);
+  if (!sync_blocks) return ZIPNN_B200_E_CUDA;
   k_select_index<<<1, kGatherIndexThreads, 0, st>>>(s.B, sel);
   ZB_LAUNCHED();
   {
     ScopedTimer tm(kKHufDecodeSync, st);
-    k_select_sync<<<(unsigned)std::min<uint64_t>(bitstreams, (uint64_t)nb * sms), kSyncThreads, kSyncSmemBytes, st>>>(s.B, s.X, sel);
+    k_select_sync<<<sync_blocks, kSyncThreads, kSyncSmemBytes, st>>>(s.B, s.X, sel);
     ZB_LAUNCHED();
   }
   {
     ScopedTimer tm(kKRegroup, st);
-    k_select_regroup<<<(unsigned)std::min<uint64_t>(tiles, (uint64_t)sms * 16), kMergeThreads, 0, st>>>(s.B, sel);
+    k_select_regroup<<<(unsigned)std::min<uint64_t>(tiles, (uint64_t)sm_count_cached() * 16), kMergeThreads, 0, st>>>(s.B, sel);
     ZB_LAUNCHED();
   }
   {
@@ -1479,228 +1475,152 @@ int zipnn_b200_decode_plan_run_select(const zipnn_b200_decode_plan* plan, size_t
   return batch_errors(s.B, st);
 }
 
-// ---- matvec: x W^T from the coded bitstreams of one whole-tensor item, no dense W (matvec.cuh) ------------------
-// Scratch: [32 K blocks][rs rows][n_tokens] fp32 partial sums.
+// ---- matvec and matmul: x W^T from the coded bitstreams of one whole-tensor item, no dense W ------------------------
+// Scratch: fp32 partial sums, for the matvec (matvec.cuh) [32 K blocks][rs rows][n_tokens], for the matmul on tensor
+// cores (matmul.cuh) [4 K quarters][rt row tiles][n_tokens][8 rows].
 namespace {
-struct MatvecGeom {
-  uint64_t in, out, ce, total;
-  uint32_t esize, rs;
-};
-// The host-side checks shared by both calls.  The first call for an item reads its chunk modes (one synchronising copy
-// of K bytes); the answer is kept with the plan's record.
-int matvec_item(const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, cudaStream_t st, PlanState& s, GatherItem& gi,
-                MatvecGeom& M) {
+enum ProductKind { kMatvec, kMatmul };
+size_t max_tokens(ProductKind kind) { return kind == kMatmul ? (size_t)kMatmulMaxTokens : (size_t)kMatvecMaxTokens; }
+
+// The host-side checks shared by all four calls, and the fields of m that the item and the shapes settle.  The first
+// call for an item reads its chunk modes (one synchronising copy of K bytes); the answer is kept with the plan's record.
+// The matmul takes 16-bit weights only: fp32 would need TF32 or a split scheme, so it is left to the decode.
+int product_item(ProductKind kind, const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, cudaStream_t st, ProductCfg& m) {
+  PlanState s;
+  GatherItem gi;
   if (!plan_state(plan, s)) return ZIPNN_B200_E_ARG;
-  const auto record = [&](GatherItem* set) -> int {
-    std::lock_guard<std::mutex> lk(g_plan_mu);
-    const auto it = g_plan_items.find((uintptr_t)s.B.error_out);
-    if (it == g_plan_items.end() || it->second.gen != s.gen) return ZIPNN_B200_E_ARG;
-    if (item < 0 || (size_t)item >= it->second.items.size()) return ZIPNN_B200_E_ARG;
-    if (set) it->second.items[(size_t)item].fused = set->fused;
-    gi = it->second.items[(size_t)item];
-    return ZIPNN_B200_OK;
-  };
   {
-    const int rc = record(nullptr);
+    const int rc = with_plan_items(s, item, [&](std::vector<GatherItem>& v) { gi = v[(size_t)item]; });
     if (rc) return rc;
   }
   if (dtype != kMvBf16 && dtype != kMvFp16 && dtype != kMvFp32) return ZIPNN_B200_E_ARG;
-  M.esize = (uint32_t)matvec_esize(dtype);
-  M.total = gi.orig / M.esize;
-  if (in_features == 0 || gi.orig % M.esize || M.total % in_features) return ZIPNN_B200_E_ARG;
-  if (gi.piece < 0 || s.mode != kSyncReplay || gi.G != (int)M.esize || (in_features * M.esize) % 16) return ZIPNN_B200_E_UNSUPPORTED;
+  const uint32_t esize = (uint32_t)matvec_esize(dtype);
+  const uint64_t total = gi.orig / esize;
+  if (in_features == 0 || gi.orig % esize || total % in_features) return ZIPNN_B200_E_ARG;
+  if (gi.piece < 0 || s.mode != kSyncReplay || gi.G != (int)esize || (in_features * esize) % 16) return ZIPNN_B200_E_UNSUPPORTED;
   if (gi.fused < 0) {
     std::vector<uint8_t> mode((size_t)gi.K);
     ZB_CUDA(cudaMemcpyAsync(mode.data(), gi.d_mode, (size_t)gi.K, cudaMemcpyDeviceToHost, st));
     ZB_CUDA(cudaStreamSynchronize(st));
-    gi.fused = 1;
-    for (const uint8_t m : mode) gi.fused &= m == kModeFused;
-    const int rc = record(&gi);
+    int fused = 1;
+    for (const uint8_t c : mode) fused &= c == kModeFused;
+    const int rc = with_plan_items(s, item, [&](std::vector<GatherItem>& v) {
+      v[(size_t)item].fused = fused;
+      gi = v[(size_t)item];
+    });
     if (rc) return rc;
   }
   if (!gi.fused) return ZIPNN_B200_E_UNSUPPORTED;
-  M.in = in_features;
-  M.out = M.total / in_features;
-  M.ce = gi.chunk / M.esize;
-  M.rs = (uint32_t)matvec_block_rows(matvec_block_elems(std::min<uint64_t>(M.ce, M.total), M.esize), M.in, M.out);
+  if (kind == kMatmul && dtype == kMvFp32) return ZIPNN_B200_E_UNSUPPORTED;
+  memset(&m, 0, sizeof(m));
+  m.cfg = s.B.cfgs + gi.piece;
+  m.seg = s.X.seg + gi.seg_base;
+  m.error = s.B.error_out;
+  m.in = in_features;
+  m.out = total / in_features;
+  m.ce = gi.chunk / esize;
+  m.total = total;
+  m.K = gi.K;
+  m.esize = esize;
+  const uint64_t first = std::min<uint64_t>(m.ce, total);  // elements of the first chunk
+  m.rs = (uint32_t)matvec_block_rows(matvec_block_elems(first, esize), m.in, m.out);
+  m.rt = (uint32_t)matmul_quarter_tiles(first / 4, m.in, m.out);
+  const uint64_t step = 32ull * (16 / esize);
+  m.step_rows = (uint32_t)(step / m.in);
+  m.step_cols = (uint32_t)(step % m.in);
   return ZIPNN_B200_OK;
 }
-size_t matvec_scratch_bytes(const GatherItem& gi, const MatvecGeom& M, size_t n_tokens) { return (size_t)32 * gi.K * M.rs * n_tokens * sizeof(float); }
+size_t product_scratch_bytes(ProductKind kind, const ProductCfg& m, size_t n_tokens) {
+  if (kind == kMatmul) return (size_t)4 * m.K * m.rt * n_tokens * kMatmulTileRows * sizeof(float);
+  return (size_t)32 * m.K * m.rs * n_tokens * sizeof(float);
+}
 
+// The bitstream kernel of a product, by how many tokens its lanes hold (matvec: 1, 2, 4 or 8; matmul: 1, 2 or 4 tiles of
+// 16), and its reduce.
+using ProductKernel = void (*)(ProductCfg);
+struct ProductKernels {
+  ProductKernel streams, reduce;
+};
 extern "C++" template <int DT>
-int matvec_launch(const MatvecCfg& m, cudaStream_t st) {
-  const auto decode = [&](auto nt) -> int {
-    constexpr int NT = decltype(nt)::value;
-    if (!smem_attr(k_matvec<DT, NT>, kSyncSmemBytes)) return ZIPNN_B200_E_CUDA;
-    const int nb = resident_blocks(k_matvec<DT, NT>, kSyncSmemBytes, kSyncThreads);
-    const unsigned blocks = (unsigned)std::min<uint64_t>(4 * m.K, (uint64_t)nb * sm_count_cached());
-    k_matvec<DT, NT><<<blocks, kSyncThreads, kSyncSmemBytes, st>>>(m);
-    ZB_LAUNCHED();
-    return ZIPNN_B200_OK;
-  };
-  int rc;
-  if (m.nt <= 1) rc = decode(std::integral_constant<int, 1>{});
-  else if (m.nt <= 2) rc = decode(std::integral_constant<int, 2>{});
-  else if (m.nt <= 4) rc = decode(std::integral_constant<int, 4>{});
-  else rc = decode(std::integral_constant<int, 8>{});
-  if (rc) return rc;
-  k_matvec_reduce<DT><<<(unsigned)((m.out * m.nt + 255) / 256), 256, 0, st>>>(m);
+ProductKernels product_kernels(ProductKind kind, uint32_t nt) {
+  if constexpr (DT != kMvFp32) {  // (product_item refuses an fp32 matmul)
+    if (kind == kMatmul) return {nt <= 16 ? &k_matmul<DT, 1> : nt <= 32 ? &k_matmul<DT, 2> : &k_matmul<DT, 4>, &k_matmul_reduce<DT>};
+  }
+  return {nt <= 1 ? &k_matvec<DT, 1> : nt <= 2 ? &k_matvec<DT, 2> : nt <= 4 ? &k_matvec<DT, 4> : &k_matvec<DT, 8>, &k_matvec_reduce<DT>};
+}
+int product_launch(const ProductKernels& f, const ProductCfg& m, cudaStream_t st) {
+  const unsigned blocks = resident_grid(f.streams, kSyncSmemBytes, kSyncThreads, 4 * m.K);
+  if (!blocks) return ZIPNN_B200_E_CUDA;
+  f.streams<<<blocks, kSyncThreads, kSyncSmemBytes, st>>>(m);
+  ZB_LAUNCHED();
+  f.reduce<<<(unsigned)((m.out * m.nt + 255) / 256), 256, 0, st>>>(m);
   ZB_LAUNCHED();
   return ZIPNN_B200_OK;
+}
+
+int product_scratch_size(ProductKind kind, const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, size_t n_tokens,
+                         size_t* out) {
+  if (!out || n_tokens > max_tokens(kind)) return ZIPNN_B200_E_ARG;
+  ProductCfg m;
+  const int rc = product_item(kind, plan, item, dtype, in_features, nullptr, m);
+  if (rc) return rc;
+  *out = product_scratch_bytes(kind, m, n_tokens);
+  return ZIPNN_B200_OK;
+}
+
+int product(ProductKind kind, const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, const void* d_x, size_t x_stride,
+            size_t n_tokens, const void* d_bias, void* d_y, size_t y_stride, void* d_scratch, size_t scratch_bytes, cudaStream_t st) {
+  if (n_tokens > max_tokens(kind)) return ZIPNN_B200_E_ARG;
+  ProductCfg m;
+  {
+    const int rc = product_item(kind, plan, item, dtype, in_features, st, m);
+    if (rc) return rc;
+  }
+  if (n_tokens == 0) return ZIPNN_B200_OK;
+  if (!d_x || !d_y || !d_scratch || ((uintptr_t)d_x & 15) || ((uintptr_t)d_scratch & 255) || ((uintptr_t)d_y % m.esize) ||
+      ((uintptr_t)d_bias % m.esize))
+    return ZIPNN_B200_E_ARG;
+  if (n_tokens > 1 && ((x_stride * m.esize) % 16 || x_stride < m.in || y_stride < m.out)) return ZIPNN_B200_E_ARG;
+  if (scratch_bytes < product_scratch_bytes(kind, m, n_tokens)) return ZIPNN_B200_E_ARG;
+  m.x = d_x;
+  m.bias = d_bias;
+  m.y = d_y;
+  m.part = (float*)d_scratch;
+  m.xs = x_stride;
+  m.ys = y_stride;
+  m.nt = (uint32_t)n_tokens;
+  if (dtype == kMvBf16) return product_launch(product_kernels<kMvBf16>(kind, m.nt), m, st);
+  if (dtype == kMvFp16) return product_launch(product_kernels<kMvFp16>(kind, m.nt), m, st);
+  return product_launch(product_kernels<kMvFp32>(kind, m.nt), m, st);
 }
 }  // namespace
 
 static_assert(kMatvecMaxTokens == ZIPNN_B200_MATVEC_MAX_TOKENS && kMvBf16 == ZIPNN_B200_MATVEC_BF16 && kMvFp16 == ZIPNN_B200_MATVEC_FP16 &&
-                  kMvFp32 == ZIPNN_B200_MATVEC_FP32,
+                  kMvFp32 == ZIPNN_B200_MATVEC_FP32 && kMatmulMaxTokens == ZIPNN_B200_MATMUL_MAX_TOKENS,
               "the header's constants are the kernels'");
 
 int zipnn_b200_decode_plan_matvec_scratch_size(const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, size_t n_tokens,
                                                size_t* out) {
-  if (!out || n_tokens > (size_t)kMatvecMaxTokens) return ZIPNN_B200_E_ARG;
-  PlanState s;
-  GatherItem gi;
-  MatvecGeom M;
-  const int rc = matvec_item(plan, item, dtype, in_features, nullptr, s, gi, M);
-  if (rc) return rc;
-  *out = matvec_scratch_bytes(gi, M, n_tokens);
-  return ZIPNN_B200_OK;
+  return product_scratch_size(kMatvec, plan, item, dtype, in_features, n_tokens, out);
 }
 
 int zipnn_b200_decode_plan_matvec(const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, const void* d_x, size_t x_stride,
                                   size_t n_tokens, const void* d_bias, void* d_y, size_t y_stride, void* d_scratch, size_t scratch_bytes,
                                   void* cuda_stream) {
-  if (n_tokens > (size_t)kMatvecMaxTokens) return ZIPNN_B200_E_ARG;
-  cudaStream_t st = (cudaStream_t)cuda_stream;
-  PlanState s;
-  GatherItem gi;
-  MatvecGeom M;
-  {
-    const int rc = matvec_item(plan, item, dtype, in_features, st, s, gi, M);
-    if (rc) return rc;
-  }
-  if (n_tokens == 0) return ZIPNN_B200_OK;
-  if (!d_x || !d_y || !d_scratch || ((uintptr_t)d_x & 15) || ((uintptr_t)d_scratch & 255) || ((uintptr_t)d_y % M.esize) ||
-      ((uintptr_t)d_bias % M.esize))
-    return ZIPNN_B200_E_ARG;
-  if (n_tokens > 1 && ((x_stride * M.esize) % 16 || x_stride < M.in || y_stride < M.out)) return ZIPNN_B200_E_ARG;
-  if (scratch_bytes < matvec_scratch_bytes(gi, M, n_tokens)) return ZIPNN_B200_E_ARG;
-  MatvecCfg m;
-  m.cfg = s.B.cfgs + gi.piece;
-  m.seg = s.X.seg + gi.seg_base;
-  m.error = s.B.error_out;
-  m.x = d_x;
-  m.bias = d_bias;
-  m.y = d_y;
-  m.part = (float*)d_scratch;
-  m.in = M.in;
-  m.out = M.out;
-  m.xs = x_stride;
-  m.ys = y_stride;
-  m.ce = M.ce;
-  m.total = M.total;
-  m.K = gi.K;
-  m.esize = M.esize;
-  m.nt = (uint32_t)n_tokens;
-  m.rs = M.rs;
-  const uint64_t step = 32ull * (16 / M.esize);
-  m.step_rows = (uint32_t)(step / M.in);
-  m.step_cols = (uint32_t)(step % M.in);
-  if (dtype == kMvBf16) return matvec_launch<kMvBf16>(m, st);
-  if (dtype == kMvFp16) return matvec_launch<kMvFp16>(m, st);
-  return matvec_launch<kMvFp32>(m, st);
+  return product(kMatvec, plan, item, dtype, in_features, d_x, x_stride, n_tokens, d_bias, d_y, y_stride, d_scratch, scratch_bytes,
+                 (cudaStream_t)cuda_stream);
 }
-
-// ---- matmul: x W^T for up to 64 rows of x on tensor cores, no dense W (matmul.cuh) --------------------------------
-// Scratch: [4 K quarters][rt row tiles][n_tokens][8 rows] fp32 partial sums.
-namespace {
-// matvec_item's checks, and 16-bit weights only: fp32 would need TF32 or a split scheme, so it is left to the decode.
-int matmul_item(const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, cudaStream_t st, PlanState& s, GatherItem& gi,
-                MatvecGeom& M, uint32_t& rt) {
-  const int rc = matvec_item(plan, item, dtype, in_features, st, s, gi, M);
-  if (rc) return rc;
-  if (dtype == kMvFp32) return ZIPNN_B200_E_UNSUPPORTED;
-  rt = (uint32_t)matmul_quarter_tiles(std::min<uint64_t>(M.ce, M.total) / 4, M.in, M.out);
-  return ZIPNN_B200_OK;
-}
-size_t matmul_scratch_bytes(const GatherItem& gi, uint32_t rt, size_t n_tokens) {
-  return (size_t)4 * gi.K * rt * n_tokens * kMatmulTileRows * sizeof(float);
-}
-
-extern "C++" template <int DT>
-int matmul_launch(const MatmulCfg& m, cudaStream_t st) {
-  const auto decode = [&](auto mt) -> int {
-    constexpr int MT = decltype(mt)::value;
-    if (!smem_attr(k_matmul<DT, MT>, kSyncSmemBytes)) return ZIPNN_B200_E_CUDA;
-    const int nb = resident_blocks(k_matmul<DT, MT>, kSyncSmemBytes, kSyncThreads);
-    const unsigned blocks = (unsigned)std::min<uint64_t>(4 * m.K, (uint64_t)nb * sm_count_cached());
-    k_matmul<DT, MT><<<blocks, kSyncThreads, kSyncSmemBytes, st>>>(m);
-    ZB_LAUNCHED();
-    return ZIPNN_B200_OK;
-  };
-  int rc;
-  if (m.nt <= 16) rc = decode(std::integral_constant<int, 1>{});
-  else if (m.nt <= 32) rc = decode(std::integral_constant<int, 2>{});
-  else rc = decode(std::integral_constant<int, 4>{});
-  if (rc) return rc;
-  k_matmul_reduce<DT><<<(unsigned)((m.out * m.nt + 255) / 256), 256, 0, st>>>(m);
-  ZB_LAUNCHED();
-  return ZIPNN_B200_OK;
-}
-}  // namespace
-
-static_assert(kMatmulMaxTokens == ZIPNN_B200_MATMUL_MAX_TOKENS, "the header's constant is the kernels'");
 
 int zipnn_b200_decode_plan_matmul_scratch_size(const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, size_t n_tokens,
                                                size_t* out) {
-  if (!out || n_tokens > (size_t)kMatmulMaxTokens) return ZIPNN_B200_E_ARG;
-  PlanState s;
-  GatherItem gi;
-  MatvecGeom M;
-  uint32_t rt;
-  const int rc = matmul_item(plan, item, dtype, in_features, nullptr, s, gi, M, rt);
-  if (rc) return rc;
-  *out = matmul_scratch_bytes(gi, rt, n_tokens);
-  return ZIPNN_B200_OK;
+  return product_scratch_size(kMatmul, plan, item, dtype, in_features, n_tokens, out);
 }
 
 int zipnn_b200_decode_plan_matmul(const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, const void* d_x, size_t x_stride,
                                   size_t n_tokens, const void* d_bias, void* d_y, size_t y_stride, void* d_scratch, size_t scratch_bytes,
                                   void* cuda_stream) {
-  if (n_tokens > (size_t)kMatmulMaxTokens) return ZIPNN_B200_E_ARG;
-  cudaStream_t st = (cudaStream_t)cuda_stream;
-  PlanState s;
-  GatherItem gi;
-  MatvecGeom M;
-  uint32_t rt;
-  {
-    const int rc = matmul_item(plan, item, dtype, in_features, st, s, gi, M, rt);
-    if (rc) return rc;
-  }
-  if (n_tokens == 0) return ZIPNN_B200_OK;
-  if (!d_x || !d_y || !d_scratch || ((uintptr_t)d_x & 15) || ((uintptr_t)d_scratch & 255) || ((uintptr_t)d_y % M.esize) ||
-      ((uintptr_t)d_bias % M.esize))
-    return ZIPNN_B200_E_ARG;
-  if (n_tokens > 1 && ((x_stride * M.esize) % 16 || x_stride < M.in || y_stride < M.out)) return ZIPNN_B200_E_ARG;
-  if (scratch_bytes < matmul_scratch_bytes(gi, rt, n_tokens)) return ZIPNN_B200_E_ARG;
-  MatmulCfg m;
-  m.cfg = s.B.cfgs + gi.piece;
-  m.seg = s.X.seg + gi.seg_base;
-  m.error = s.B.error_out;
-  m.x = d_x;
-  m.bias = d_bias;
-  m.y = d_y;
-  m.part = (float*)d_scratch;
-  m.in = M.in;
-  m.out = M.out;
-  m.xs = x_stride;
-  m.ys = y_stride;
-  m.ce = M.ce;
-  m.total = M.total;
-  m.K = gi.K;
-  m.nt = (uint32_t)n_tokens;
-  m.rt = rt;
-  if (dtype == kMvBf16) return matmul_launch<kMvBf16>(m, st);
-  return matmul_launch<kMvFp16>(m, st);
+  return product(kMatmul, plan, item, dtype, in_features, d_x, x_stride, n_tokens, d_bias, d_y, y_stride, d_scratch, scratch_bytes,
+                 (cudaStream_t)cuda_stream);
 }
 
 int zipnn_b200_split(const void* d_in, size_t n, int num_buf, int bits_mode, void* d_planes, size_t stride,

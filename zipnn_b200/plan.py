@@ -338,14 +338,15 @@ class DecodePlan:
         _, _, dt, sh = self._offs[k]
         return dt, sh
 
-    def _matvec_size(self, k: int, in_features: int, n_tokens: int) -> tuple:
+    def _product_size(self, name: str, k: int, in_features: int, n_tokens: int) -> tuple:
+        """-> (status, scratch bytes) of zipnn_b200_decode_plan_{name}_scratch_size, `name` "matvec" or "matmul"."""
         dt, _ = self._matvec_item(k)
         out = C.c_size_t(0)
-        if dt not in _MATVEC_DTYPES or in_features <= 0:
+        if dt not in (_MATMUL_DTYPES if name == "matmul" else _MATVEC_DTYPES) or in_features <= 0:
             return _native.E_UNSUPPORTED, 0
         with torch.cuda.device(self.device):
-            rc = _native.lib().zipnn_b200_decode_plan_matvec_scratch_size(self._ref, k, _MATVEC_DTYPES[dt], int(in_features), int(n_tokens),
-                                                                          C.byref(out))
+            rc = getattr(_native.lib(), f"zipnn_b200_decode_plan_{name}_scratch_size")(self._ref, k, _MATVEC_DTYPES[dt], int(in_features),
+                                                                                      int(n_tokens), C.byref(out))
         return rc, out.value
 
     def matvec_ok(self, k: int, in_features: int) -> bool:
@@ -360,12 +361,12 @@ class DecodePlan:
         if in_features <= 0 or n == 0 or n % in_features:
             return False
         if (k, in_features) not in self._matvec_ok:
-            self._matvec_ok[(k, in_features)] = self._matvec_size(k, in_features, 1)[0] == _native.OK
+            self._matvec_ok[(k, in_features)] = self._product_size("matvec", k, in_features, 1)[0] == _native.OK
         return self._matvec_ok[(k, in_features)]
 
     def matvec_scratch_bytes(self, k: int, in_features: int, n_tokens: int = MATVEC_MAX_TOKENS) -> int:
         """Bytes of a matvec scratch for output `k`, rows of `in_features` elements and `n_tokens` rows of x."""
-        rc, n = self._matvec_size(k, in_features, n_tokens)
+        rc, n = self._product_size("matvec", k, in_features, n_tokens)
         _native.check(rc)
         return n
 
@@ -387,16 +388,6 @@ class DecodePlan:
         -> out.  ValueError for an output `matvec_ok` refuses.  Works without the plan's output buffer."""
         return self._product("matvec", k, x, bias, out, scratch)
 
-    def _matmul_size(self, k: int, in_features: int, n_tokens: int) -> tuple:
-        dt, _ = self._matvec_item(k)
-        out = C.c_size_t(0)
-        if dt not in _MATMUL_DTYPES or in_features <= 0:
-            return _native.E_UNSUPPORTED, 0
-        with torch.cuda.device(self.device):
-            rc = _native.lib().zipnn_b200_decode_plan_matmul_scratch_size(self._ref, k, _MATVEC_DTYPES[dt], int(in_features), int(n_tokens),
-                                                                          C.byref(out))
-        return rc, out.value
-
     def matmul_ok(self, k: int, in_features: int) -> bool:
         """Can `matmul` multiply by output `k` seen as rows of `in_features` elements?  What `matvec_ok` accepts, for
         bf16 and fp16 outputs only (an fp32 output decodes).  Never raises for an output that exists."""
@@ -404,12 +395,12 @@ class DecodePlan:
         if dt not in _MATMUL_DTYPES or not self.matvec_ok(k, in_features):
             return False
         if (k, in_features) not in self._matmul_ok:
-            self._matmul_ok[(k, in_features)] = self._matmul_size(k, in_features, 1)[0] == _native.OK
+            self._matmul_ok[(k, in_features)] = self._product_size("matmul", k, in_features, 1)[0] == _native.OK
         return self._matmul_ok[(k, in_features)]
 
     def matmul_scratch_bytes(self, k: int, in_features: int, n_tokens: int = MATMUL_MAX_TOKENS) -> int:
         """Bytes of a matmul scratch for output `k`, rows of `in_features` elements and `n_tokens` rows of x."""
-        rc, n = self._matmul_size(k, in_features, n_tokens)
+        rc, n = self._product_size("matmul", k, in_features, n_tokens)
         _native.check(rc)
         return n
 
