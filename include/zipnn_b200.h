@@ -46,9 +46,13 @@ extern "C" {
 #define ZIPNN_B200_OK 0
 #define ZIPNN_B200_E_ARG 1        /* bad num_buf / modes / chunk / NULL pointer                 */
 #define ZIPNN_B200_E_CAPACITY 2   /* out_cap or workspace too small                              */
-#define ZIPNN_B200_E_CORRUPT 3    /* stream rejected: bad type byte (zipnn_core.c:986-997), bad
-                                     sizes, invalid weight table (entropy_common.c:189-210),
-                                     bitstream not consumed exactly (huf_decompress.c:348-349)   */
+#define ZIPNN_B200_E_CORRUPT 3    /* stream rejected (DESIGN §6): body shorter than its tables, a
+                                     group total past the payload, a decreasing or out-of-group
+                                     size row, bad type byte (zipnn_core.c:986-997), a stored item
+                                     not exactly its plane's length, a coded item on an empty plane
+                                     or longer than its plane, invalid weight table
+                                     (entropy_common.c:189-210), a bitstream not consumed exactly
+                                     as HUF_decompress4X1 requires (huf_decompress.c:348-349)    */
 #define ZIPNN_B200_E_CUDA 4       /* a CUDA runtime call failed; see zipnn_b200_last_cuda_error  */
 #define ZIPNN_B200_E_UNSUPPORTED 5 /* valid stream using a table log of 12 (never produced by
                                      the reference encoder, which asks for 11)                   */
@@ -127,7 +131,8 @@ int zipnn_b200_decompress(const void* d_body, size_t body_len, int num_buf, int 
  * from vLLM's weight iterator); a GPU wants the whole shard in one go.  Every item is what one
  * zipnn_b200_decompress call would take; all of them are decoded by ONE launch of each kernel
  * (tensors of up to ~3000 chunks; larger ones run one by one on the same stream).
- * Status of the whole batch: OR of the tensors' error words. */
+ * Status of the whole batch: OR of the tensors' error words.  An item whose body is shorter than its own
+ * type and size tables is refused (E_CORRUPT) before anything is enqueued: no item is decoded then. */
 typedef struct zipnn_b200_batch_item {
   const void* d_body;   /* stream after the python header, device memory */
   size_t body_len;

@@ -179,12 +179,13 @@ def ref_core():
 
 
 def ref_cdll():
-    """ctypes view of the same .so: HUF_compress / HUF_decompress are exported."""
+    """ctypes view of the same .so: HUF_compress, HUF_decompress and its two decoders (4X1: one symbol per
+    table cell, 4X2: two) are exported."""
     p = ref_path()
     if not os.path.exists(p):
         return None
     L = C.CDLL(p)
-    for name in ("HUF_compress", "HUF_decompress"):
+    for name in ("HUF_compress", "HUF_decompress", "HUF_decompress4X1", "HUF_decompress4X2"):
         f = getattr(L, name)
         f.restype = C.c_size_t
         f.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
@@ -203,3 +204,16 @@ def ref_huf_compress(src, cap: int = 256 * 1024):
     if r == 0:
         return 0, b""
     return r, dst[:r].tobytes()
+
+
+def ref_huf_decoders(block, n: int) -> dict:
+    """What the reference's HUF_decompress, HUF_decompress4X1 and HUF_decompress4X2 make of one block for an n-byte
+    destination: {name: the decoded bytes, or None when it reports an error}."""
+    L = ref_cdll()
+    s = _u8(block)
+    out = {}
+    for name in ("HUF_decompress", "HUF_decompress4X1", "HUF_decompress4X2"):
+        dst = np.zeros(max(n, 1) + 64, dtype=np.uint8)
+        r = getattr(L, name)(_ptr(dst), n, _ptr(s), s.size)
+        out[name] = None if L.HUF_isError(r) or r != n else dst[:n].tobytes()
+    return out

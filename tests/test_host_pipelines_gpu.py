@@ -165,7 +165,8 @@ def test_slab_decoder_many_general_chunks_per_slab(knob, host_buf):
 
 def test_slab_decoder_corrupt_streams(knob, host_buf):
     """A bad type byte in the last slab (found on the device), a size row that decreases across the edge into the
-    last slab (found by the host check, at the slab the model names) and a truncated body: each is E_CORRUPT, and a
+    last slab (found by the host check, at the slab the model names: the one before, whose last row is now past the
+    group's total) and a truncated body: each is E_CORRUPT, and a
     good decode through the same process cache right after is exact."""
     name = "bf16"
     G, bits, chunk, n = HM.DECODE_LAYOUTS[name]
@@ -181,7 +182,7 @@ def test_slab_decoder_corrupt_streams(knob, host_buf):
     bad_row = body.copy()
     cum = bad_row[G * K: 9 * G * K].view("<u8").reshape(G, K)
     cum[G - 1, K - 1] = cum[G - 1, c_last - 1] - 1
-    cases = [(bad_type, ("ok", None)), (bad_row, ("row", plan.nslabs - 1)), (body[:-7], ("room", None))]
+    cases = [(bad_type, ("ok", None)), (bad_row, ("row", plan.nslabs - 2)), (body[:-7], ("room", None))]
     for bad, where in cases:
         assert HM.decode_host_check(bad, G, chunk, n, per) == where
         out = host_buf(n + PAD, "pinned")
@@ -325,17 +326,19 @@ def test_error_exits_leave_nothing_in_flight(knob):
     K = plan.K
     H = 32
     knob(BIG_SLAB)
-    # decompress: a size row that decreases into the last slab, found by the host check after slabs 0 and 1 are queued
+    # decompress: a size row that decreases into the last slab, which leaves slab 1's last row past the group's
+    # total: found by the host check before any slab is queued
     body = stream[H:].copy()
     cum = body[G * K: 9 * G * K].view("<u8").reshape(G, K)
     c_last = plan.ranges[-1][0]
     cum[G - 1, K - 1] = cum[G - 1, c_last - 1] - 1
-    assert HM.decode_host_check(body, G, chunk, n, plan.per) == ("row", 2)
+    assert HM.decode_host_check(body, G, chunk, n, plan.per) == ("row", 1)
     h_out = torch.full((n,), CANARY, dtype=torch.uint8, pin_memory=True)
     rc = L.zipnn_b200_decompress_host(body.ctypes.data, body.size, G, 1, 10, chunk, n, h_out.data_ptr())
     last = slice(plan.ranges[1][1] * chunk - 4096, plan.ranges[1][1] * chunk)     # the end of slab 1's output
     _settled(h_out, last)
     assert rc == HM.E_CORRUPT
+    assert bool((h_out == CANARY).all()), "a refused stream wrote to h_out"
     # compress with out_cap one byte short: fails at the final check right after the last slab's group-0 copy
     Lw = stream.size
     m = HM.bet_model(stream, H, G, chunk, n, plan.per, Lw - 1)

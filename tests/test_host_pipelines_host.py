@@ -194,10 +194,10 @@ def edge_pairs(classes, plan: SlabPlan):
 
 # ------------------------------------------------------------------ decode: the host-side checks
 def decode_host_check(body, G: int, chunk: int, orig: int, per: int):
-    """Where decompress_host_slabs rejects the stream on the host: ('ok', None) when the host checks pass (the
-    device then sees the rest), ('short' | 'room', None) before any work is enqueued, or ('row', i) when slab i's
-    rows fail (a decreasing row, a slab larger than slab_max, planes larger than the slab) with slabs 0..i-1
-    already enqueued."""
+    """Where decompress_host_slabs rejects the stream on the host, always before any work is enqueued:
+    ('ok', None) when the host checks pass (the device then sees the rest), ('short' | 'room', None), or
+    ('row', i) when slab i is the first whose rows fail (a decreasing row, a row past its group's total, a slab
+    larger than slab_max, planes larger than the slab)."""
     b = np.asarray(body, dtype=np.uint8)
     K = -(-orig // chunk)
     if b.size < 9 * G * K:
@@ -205,11 +205,11 @@ def decode_host_check(body, G: int, chunk: int, orig: int, per: int):
     _, cum, payload0, _ = tables(b, 0, G, K)
     u = cum.astype(np.uint64)
     room = b.size - payload0
+    tot = [int(u[g, K - 1]) for g in range(G)]
     for g in range(G):
-        tot = int(u[g, K - 1])
-        if tot > room:
+        if tot[g] > room:
             return "room", None
-        room -= tot
+        room -= tot[g]
     slab_max, tables_max = per * chunk, 9 * G * per
     for i, c0 in enumerate(range(0, K, per)):
         c1 = min(K, c0 + per)
@@ -217,7 +217,7 @@ def decode_host_check(body, G: int, chunk: int, orig: int, per: int):
         for g in range(G):
             lo = int(u[g, c0 - 1]) if c0 else 0
             hi = int(u[g, c1 - 1])
-            if hi < lo or hi - lo > slab_max:
+            if hi < lo or hi > tot[g] or hi - lo > slab_max:
                 return "row", i
             total += hi - lo
         if total > slab_max + tables_max:
@@ -371,8 +371,8 @@ def test_decode_host_check_model():
     cum = body[G * K: 9 * G * K].view("<u8").reshape(G, K)
     bad = body.copy()
     bcum = bad[G * K: 9 * G * K].view("<u8").reshape(G, K)
-    bcum[1, K - 1] = cum[1, 5] - 1        # decreases across the edge into the last slab (chunks 6..6)
-    assert decode_host_check(bad, G, chunk, n, 2) == ("row", 3)
+    bcum[1, K - 1] = cum[1, 5] - 1        # decreases across the edge into the last slab (chunks 6..6) ...
+    assert decode_host_check(bad, G, chunk, n, 2) == ("row", 2)   # ... so slab 2's last row is past the total
     assert decode_host_check(body[:-1], G, chunk, n, 2) == ("room", None)
     assert decode_host_check(body[: 9 * G * K - 1], G, chunk, n, 2) == ("short", None)
 

@@ -220,11 +220,9 @@ __device__ __forceinline__ void decode_meta_body(const DecodeCfg& cfg, uint64_t 
         d.kind = kRaw;
         bad = bad || (slen != dlen);
       } else {
-        // HUF_decompress (huf_decompress.c:1056-1081): csize > dst -> error; == -> copy; 1 -> RLE
-        if (dlen == 0) {
-          d.kind = kRaw;
-          d.src_len = 0;
-        } else if (slen > dlen || slen == 0) {
+        // HUF_decompress (huf_decompress.c:1056-1081): no room -> error (an empty plane cannot be coded);
+        // csize > dst -> error; == -> copy; 1 -> RLE
+        if (dlen == 0 || slen > dlen || slen == 0) {
           bad = true;
           d.kind = kRaw;
         } else if (slen == dlen) {

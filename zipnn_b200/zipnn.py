@@ -518,6 +518,7 @@ class ZipNN:
         total = stream.numel() if isinstance(stream, torch.Tensor) else stream.size
         if total < after_header:
             raise RuntimeError("corrupt ZipNN stream: truncated header")
+        _refuse_header(num_buf, self._byte_reorder, chunk, total - after_header, n)
         if isinstance(stream, torch.Tensor):
             tdt = torch_dtype_of_code(code) if self.input_format == EnumFormat.TORCH.value else None
             if tdt is not None and math.prod(self.shape_bytes) * tdt.itemsize == n:
@@ -692,6 +693,8 @@ class DecodePipe:
         tdt = torch_dtype_of_code(znn.dtype)
         shape = znn.shape_bytes
         blen = total_len - after
+        _refuse_header(num_buf, znn._byte_reorder, chunk, blen, n)
+        _refuse_shape(shape, tdt, n)
         L = _native.lib()
         cur = torch.cuda.current_stream(self.device)
         with torch.cuda.device(self.device):
@@ -802,6 +805,8 @@ class DecodePipe:
                     continue
                 num_buf = znn._num_buf_of_dtype()
                 chunk = znn.compression_chunk if num_buf != 1 else min(HUF_MAX_BLOCK, znn.compression_chunk)
+                _refuse_header(num_buf, znn._byte_reorder, chunk, nbytes - after, znn.original_len)
+                _refuse_shape(znn.shape_bytes, torch_dtype_of_code(znn.dtype), znn.original_len)
                 items.append((j, off - lo + after, nbytes - after, num_buf, znn._bit_reorder, znn._byte_reorder, chunk, znn.original_len,
                               torch_dtype_of_code(znn.dtype), znn.shape_bytes))
             if not items:
@@ -979,10 +984,34 @@ def _compress_device_batch(flats: list, plans: list) -> list:
     return [out[o: o + lens[i]] for i, o in enumerate(offs)]
 
 
+def _refuse_header(num_buf: int, byte_reorder: int, chunk: int, body_len: int, orig: int) -> None:
+    """The checks of a stream header that come before any allocation of its `orig` bytes: a chunk size or byte
+    reorder code the library does not take (ValueError), and a body that cannot back `orig` (corrupt)."""
+    if chunk > 1 << 31 or byte_reorder != (220 if num_buf == 4 else 10):
+        raise ValueError(f"Unsupported chunk size or byte reorder in the header: 2**{chunk.bit_length() - 1}, {byte_reorder}")
+    _refuse_unbacked(body_len, num_buf, chunk, orig)
+
+
+def _refuse_shape(shape, dtype: torch.dtype, orig: int) -> None:
+    """The file-load paths hand out the decoded bytes as a tensor of the header's shape: a shape that does not hold
+    `orig` bytes is a corrupt header, refused before the decode."""
+    if dtype is not None and math.prod(shape) * dtype.itemsize != orig:
+        raise RuntimeError("corrupt ZipNN stream: the header's shape does not match its length")
+
+
+def _refuse_unbacked(body_len: int, num_buf: int, chunk: int, orig: int) -> None:
+    """A body shorter than its type and size tables (9 bytes per group and chunk) cannot back the `orig` bytes its
+    header claims: refused before anything of that size is allocated, so a crafted length is reported as a
+    corrupt stream rather than as an out-of-memory error."""
+    if orig and body_len < 9 * num_buf * -(-orig // chunk):
+        raise RuntimeError("Thread processing failed: corrupt ZipNN stream")
+
+
 def _decompress_device(body: torch.Tensor, num_buf: int, bits_mode: int, bytes_mode: int, chunk: int,
                        orig: int, body_off: int = 0, out: torch.Tensor = None) -> torch.Tensor:
     """Decode body[body_off:] (a flat uint8 CUDA tensor) into `out` (a contiguous tensor of orig bytes on the same
     device; by default a new uint8 one) and return `out`."""
+    _refuse_unbacked(body.numel() - body_off, num_buf, chunk, orig)
     dev = body.device
     with _on_device(dev):
         if out is None:
@@ -1065,6 +1094,7 @@ def _decompress_host(body: np.ndarray, num_buf: int, bits_mode: int, bytes_mode:
     stream of their own once their table rows are rebased, so the library decodes slab by slab on two
     CUDA streams with the H2D copy, the kernels and the D2H copy of neighbouring slabs overlapped."""
     _native.require_cuda()
+    _refuse_unbacked(body.size, num_buf, chunk, orig)
     host = _host_out(orig, out)
     if orig == 0:
         return host
