@@ -313,6 +313,33 @@ int zipnn_b200_decode_plan_matmul(const zipnn_b200_decode_plan* plan, int item, 
                                   const void* d_x, size_t x_stride, size_t n_tokens, const void* d_bias, void* d_y,
                                   size_t y_stride, void* d_scratch, size_t scratch_bytes, void* cuda_stream);
 
+/* _matvec_fp8: y = x (S . W)^T (+ bias) for fp8 weights with an fp32 scale grid, straight from the coded bitstreams of
+ * item `item` as _matvec does it: W is the item's decoded tensor, row-major [out_features][in_features] of
+ * float8_e4m3fn (fp8_format ZIPNN_B200_FP8_E4M3) or float8_e5m2 (ZIPNN_B200_FP8_E5M2); d_scale is the contiguous fp32
+ * grid [ceil(out_features / block_rows)][ceil(in_features / block_cols)], and the weight the product uses is
+ * float(W[o][i]) * S[o / block_rows][i / block_cols] (the stored scale multiplies, as `weight_scale_inv` in fp8
+ * checkpoints).  (out_features, in_features) is one scale for the tensor, (1, in_features) one per row, (128, 128)
+ * DeepSeek's blocks, ragged at the edges.  x, y and the optional d_bias have x_dtype, ZIPNN_B200_MATVEC_BF16 or _FP16.
+ * Each lane of the kernel adds the products of 16 consecutive weights of a row with x in ascending column order (fp32
+ * FMAs), multiplies the sum by the block's scale once, and from there the sums, their order, the rounding, the launches
+ * (2; none for n_tokens == 0), graph capture, determinism and the first call's read of the chunk modes are _matvec's.
+ * An e4m3fn NaN or an e5m2 infinity or NaN in W gives what the dense product of the dequantized matrix gives: NaN or
+ * an infinity in that row of y.
+ * Eligible items (else E_UNSUPPORTED): those _matvec takes, with num_buf 1 (fp8 streams).
+ * Host-side rejections launch and write nothing: E_ARG as for _matvec (x_dtype in place of dtype, the alignments of x,
+ * y and d_bias those of x_dtype), and for an fp8_format other than the two below, an x_dtype other than BF16 or FP16,
+ * block_rows 0, block_cols below 16 or not a multiple of 16, and with n_tokens > 0 a NULL or not 4-byte aligned
+ * d_scale.  _matvec_fp8_scratch_size: the scratch bytes (_matvec's formula), the same item checks. */
+#define ZIPNN_B200_FP8_E4M3 0
+#define ZIPNN_B200_FP8_E5M2 1
+int zipnn_b200_decode_plan_matvec_fp8_scratch_size(const zipnn_b200_decode_plan* plan, int item, size_t in_features,
+                                                   size_t n_tokens, size_t* out);
+int zipnn_b200_decode_plan_matvec_fp8(const zipnn_b200_decode_plan* plan, int item, int fp8_format, int x_dtype,
+                                      size_t in_features, const void* d_x, size_t x_stride, size_t n_tokens,
+                                      const float* d_scale, size_t block_rows, size_t block_cols,
+                                      const void* d_bias, void* d_y, size_t y_stride,
+                                      void* d_scratch, size_t scratch_bytes, void* cuda_stream);
+
 /* ---- stage 1 alone ------------------------------------------------------------ */
 /* d_planes: num_buf planes of `stride` bytes each; plane g receives byte g of every element
  * of the (optionally rotated) input.  Lengths as in the reference: n/num_buf, the first

@@ -9,6 +9,9 @@
 //   k_matvec_reduce  one thread per (token, output row) adds the row's partial sums in ascending element order, adds the
 //                    bias, rounds once to the output type and stores.
 //
+// k_matvec_fp8 is k_matvec for fp8 weights with an fp32 scale grid and bf16 / fp16 x (MatvecFp8Ep, below); its partial
+// sums go through k_matvec_reduce unchanged.
+//
 // Thread mapping.  The run's store loop gives thread t the vectors t, t + 256, ...: fine for stores, but it scatters a
 // row of W over all threads, so every row would end in a CTA-wide reduction.  Here a warp owns a contiguous BLOCK of
 // the quarter plane (an eighth of it, rounded up to whole 32-vector steps) and its lanes take consecutive vectors:
@@ -25,6 +28,7 @@
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <cuda_fp8.h>
 
 #include "decode_sync.cuh"
 
@@ -49,6 +53,11 @@ struct ProductCfg {
   uint32_t esize, nt, rs; // element bytes, tokens, slots (rows) per block of the matvec
   uint32_t step_rows, step_cols;  // one 32-vector step of the matvec as whole rows + columns
   uint32_t rt;            // row tiles per quarter in the matmul's slot layout
+  // the fp8 matvec's scale grid S [ceil(out / bn)][scols]: the block of element (row, col) is
+  // (matvec_fp8_div(row, srow), matvec_fp8_div(col, scol)), srow / scol the reciprocals of bn / bk (matvec_fp8_recip)
+  const float* scale;
+  uint64_t srow, scol;
+  uint32_t scols;
 };
 
 // Elements of a block of a chunk with n elements: a quarter's vectors split over 8 warps, in whole 32-vector steps.
@@ -187,6 +196,120 @@ struct MatvecEp {
   }
 };
 
+// ---- fp8 weights with an fp32 scale grid (k_matvec_fp8) -------------------------------------------------------------
+// y[t][o] = sum_i x[t][i] * (float(W[o][i]) * S[o / bn][i / bk]) (+ bias[o]), W of float8_e4m3fn or float8_e5m2 in one
+// byte plane (G = 1), x, bias and y of bf16 or fp16.  bk % 16 == 0, so a lane's 16 weights (one vector) lie in one row
+// and one scale block: the lane forms s = fma(w15, x15, ... fma(w0, x0, 0)) in fp32, in ascending column order, and
+// p = s * S[block] with one multiply; from there on everything is MatvecEp's (per-lane row accumulators, the butterfly,
+// one slot per (block, row, token), k_matvec_reduce).  fp8 -> fp32 is exact in both formats, subnormals included; an
+// e4m3fn NaN or an e5m2 infinity or NaN acts as in the dense product of the dequantized matrix.
+enum : int { kFp8E4m3 = 0, kFp8E5m2 = 1 };
+
+// floor(n / d) for n, d < 2^31 as one 64-bit multiply-high by r = ceil(2^64 / (2 d)), no division: 2n * r / 2^64 =
+// n / d + 2n * e / 2^64 with 0 <= e < 1, and 2n * e / 2^64 < 1 / (2d) because 2n * 2d < 2^64, so the floor is n / d's.
+__host__ __device__ constexpr uint64_t matvec_fp8_recip(uint64_t d) { return ~0ull / (2 * d) + 1; }
+__device__ __forceinline__ uint32_t matvec_fp8_div(uint32_t n, uint64_t r) { return (uint32_t)__umul64hi(2ull * n, r); }
+
+// The 8 fp8 weights of two words as fp32 (exact: every e4m3fn and e5m2 value, NaN and infinities too, is an fp16 one).
+template <int FMT>
+__device__ __forceinline__ void fp8_floats(uint32_t a, uint32_t b, float (&f)[8]) {
+#pragma unroll
+  for (int i = 0; i < 4; i++) {
+    const uint32_t word = i < 2 ? a : b;
+    const __half2_raw hr = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(word >> (16 * (i & 1))), FMT == kFp8E4m3 ? __NV_E4M3 : __NV_E5M2);
+    const float2 v = __half22float2(*reinterpret_cast<const __half2*>(&hr));
+    f[2 * i] = v.x;
+    f[2 * i + 1] = v.y;
+  }
+}
+
+// The warp-owns-a-block mapping and the row walk are MatvecEp's (its flush is reused); a step is 32 lanes x 16 weights,
+// and a lane reads 32 bytes of x per token and one scale per step (the grid is small and stays in L1 / L2).
+template <int FMT, int XDT, int NT>
+struct MatvecFp8Ep : MatvecEp<XDT, NT> {
+  static constexpr int EPV = 16;
+  using MatvecEp<XDT, NT>::m;
+  using MatvecEp<XDT, NT>::flush;
+
+  template <int G>
+  __device__ __forceinline__ void quarter(const SyncShared& S, uint64_t c, int stream, uint32_t out_off, uint32_t count, bool rot) const {
+    static_assert(G == 1 && XDT != kMvFp32, "fp8 weights: one byte plane; x of bf16 or fp16");
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint32_t nv = count / EPV;
+    const uint32_t vpw = ((nv + 255u) >> 8) << 5;
+    const uint32_t v0 = (uint32_t)wid * vpw, v1 = min(nv, v0 + vpw);
+    if (v0 >= v1) return;  // (warp-uniform) a short last chunk leaves the upper warps without a block
+    const uint64_t in = m.in;
+    const uint64_t e0 = c * m.ce + out_off + (uint64_t)v0 * EPV;
+    uint64_t row0 = e0 / in, col0 = e0 - row0 * in;  // of the step's first element: the same in every lane
+    float* const slots = m.part + ((c * 4 + (uint32_t)stream) * 8 + (uint32_t)wid) * m.rs * m.nt;  // the block's, from its first row
+    const uint64_t first = row0;
+    const uint8_t* const xb = reinterpret_cast<const uint8_t*>(m.x);
+    float acc[NT];
+#pragma unroll
+    for (int t = 0; t < NT; t++) acc[t] = 0.f;
+    uint64_t cur = row0;
+    for (uint32_t v = v0; v < v1; v += 32) {
+      const uint32_t nvalid = min(32u, v1 - v);
+      const bool valid = (uint32_t)lane < nvalid;
+      uint64_t lrow = row0, lcol = col0 + (uint32_t)lane * EPV;
+      uint64_t last = row0;
+      if (col0 + 32u * EPV > in) {  // (uniform) the step straddles rows
+        const uint64_t q = lcol / in;
+        lrow += q;
+        lcol -= q * in;
+        last += (col0 + nvalid * EPV - 1) / in;
+      }
+      float p[NT];
+#pragma unroll
+      for (int t = 0; t < NT; t++) p[t] = 0.f;
+      if (valid) {
+        uint32_t r[4];
+        const uint32_t o = (v + (uint32_t)lane) * 16u;
+        ZB_FUSED_VECTOR(G, S, out_off, o, rot, r);
+        const float sc = __ldg(m.scale + matvec_fp8_div((uint32_t)lrow, m.srow) * m.scols + matvec_fp8_div((uint32_t)lcol, m.scol));
+        // in two halves of 8 columns, every token's sum carried from the first to the second (the order of each sum
+        // is the same), the half loop not unrolled: only 16 bytes of x per token are in flight at once.  Unrolled, the
+        // compiler issues all 32 bytes of every token together and NT = 8 spills at 80 registers.
+#pragma unroll 1
+        for (int h = 0; h < 2; h++) {
+          float w[8];
+          fp8_floats<FMT>(h ? r[2] : r[0], h ? r[3] : r[1], w);
+#pragma unroll
+          for (int t = 0; t < NT; t++) {
+            const uint64_t tt = min((uint32_t)t, m.nt - 1u);
+            const uint4 xv = __ldg(reinterpret_cast<const uint4*>(xb + (tt * m.xs + lcol) * 2) + h);
+            const uint32_t xr[4] = {xv.x, xv.y, xv.z, xv.w};
+            float xf[8];
+            matvec_floats<XDT, 8>(xr, xf);
+#pragma unroll
+            for (int i = 0; i < 8; i++) p[t] = fmaf(w[i], xf[i], p[t]);
+          }
+        }
+#pragma unroll
+        for (int t = 0; t < NT; t++) p[t] *= sc;
+      }
+      for (uint64_t rr = row0; rr <= last; rr++) {
+        if (rr != cur) {
+          flush(acc, slots + (cur - first) * m.nt, lane);
+          cur = rr;
+        }
+        if (lrow == rr) {
+#pragma unroll
+          for (int t = 0; t < NT; t++) acc[t] += p[t];
+        }
+      }
+      row0 += m.step_rows;
+      col0 += m.step_cols;
+      if (col0 >= in) {
+        col0 -= in;
+        row0++;
+      }
+    }
+    flush(acc, slots + (cur - first) * m.nt, lane);
+  }
+};
+
 // The bitstream loop of k_matvec and k_matmul: one CTA per coded bitstream of the item (every chunk is fused: its one
 // coded item is the top byte plane), each decoded as by a plan run, with the epilogue's `quarter` in place of its stores.
 template <int G, typename Ep>
@@ -242,6 +365,12 @@ __global__ void __launch_bounds__(256) k_matvec_reduce(ProductCfg m) {
     }
     return s;
   });
+}
+
+// fp8 weights: the partial sums are k_matvec_reduce<XDT>'s, whose block geometry comes from m.esize (1).
+template <int FMT, int XDT, int NT>
+__global__ void __launch_bounds__(kSyncThreads, 3) k_matvec_fp8(ProductCfg m) {
+  product_streams<1>(m, MatvecFp8Ep<FMT, XDT, NT>{{m}});
 }
 
 }  // namespace zb

@@ -1477,14 +1477,16 @@ int zipnn_b200_decode_plan_run_select(const zipnn_b200_decode_plan* plan, size_t
 
 // ---- matvec and matmul: x W^T from the coded bitstreams of one whole-tensor item, no dense W ------------------------
 // Scratch: fp32 partial sums, for the matvec (matvec.cuh) [32 K blocks][rs rows][n_tokens], for the matmul on tensor
-// cores (matmul.cuh) [4 K quarters][rt row tiles][n_tokens][8 rows].
+// cores (matmul.cuh) [4 K quarters][rt row tiles][n_tokens][8 rows].  The fp8 matvec's are the matvec's.
 namespace {
-enum ProductKind { kMatvec, kMatmul };
+enum ProductKind { kMatvec, kMatmul, kMatvecFp8 };
 size_t max_tokens(ProductKind kind) { return kind == kMatmul ? (size_t)kMatmulMaxTokens : (size_t)kMatvecMaxTokens; }
 
 // The host-side checks shared by all four calls, and the fields of m that the item and the shapes settle.  The first
 // call for an item reads its chunk modes (one synchronising copy of K bytes); the answer is kept with the plan's record.
-// The matmul takes 16-bit weights only: fp32 would need TF32 or a split scheme, so it is left to the decode.
+// The matmul takes 16-bit weights only: fp32 would need TF32 or a split scheme, so it is left to the decode.  For the
+// fp8 matvec, `dtype` is x's (bf16 or fp16) and the weights are one byte: its scale lookup takes element indices in 32
+// bits, which every fp8 piece has (at most 16383 chunks of 128 KiB).
 int product_item(ProductKind kind, const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, cudaStream_t st, ProductCfg& m) {
   PlanState s;
   GatherItem gi;
@@ -1493,8 +1495,8 @@ int product_item(ProductKind kind, const zipnn_b200_decode_plan* plan, int item,
     const int rc = with_plan_items(s, item, [&](std::vector<GatherItem>& v) { gi = v[(size_t)item]; });
     if (rc) return rc;
   }
-  if (dtype != kMvBf16 && dtype != kMvFp16 && dtype != kMvFp32) return ZIPNN_B200_E_ARG;
-  const uint32_t esize = (uint32_t)matvec_esize(dtype);
+  if (dtype != kMvBf16 && dtype != kMvFp16 && (dtype != kMvFp32 || kind == kMatvecFp8)) return ZIPNN_B200_E_ARG;
+  const uint32_t esize = kind == kMatvecFp8 ? 1u : (uint32_t)matvec_esize(dtype);
   const uint64_t total = gi.orig / esize;
   if (in_features == 0 || gi.orig % esize || total % in_features) return ZIPNN_B200_E_ARG;
   if (gi.piece < 0 || s.mode != kSyncReplay || gi.G != (int)esize || (in_features * esize) % 16) return ZIPNN_B200_E_UNSUPPORTED;
@@ -1512,6 +1514,7 @@ int product_item(ProductKind kind, const zipnn_b200_decode_plan* plan, int item,
   }
   if (!gi.fused) return ZIPNN_B200_E_UNSUPPORTED;
   if (kind == kMatmul && dtype == kMvFp32) return ZIPNN_B200_E_UNSUPPORTED;
+  if (kind == kMatvecFp8 && total > (uint64_t)INT32_MAX) return ZIPNN_B200_E_UNSUPPORTED;
   memset(&m, 0, sizeof(m));
   m.cfg = s.B.cfgs + gi.piece;
   m.seg = s.X.seg + gi.seg_base;
@@ -1548,6 +1551,14 @@ ProductKernels product_kernels(ProductKind kind, uint32_t nt) {
   }
   return {nt <= 1 ? &k_matvec<DT, 1> : nt <= 2 ? &k_matvec<DT, 2> : nt <= 4 ? &k_matvec<DT, 4> : &k_matvec<DT, 8>, &k_matvec_reduce<DT>};
 }
+extern "C++" template <int FMT, int XDT>
+ProductKernels fp8_kernels(uint32_t nt) {
+  return {nt <= 1   ? &k_matvec_fp8<FMT, XDT, 1>
+          : nt <= 2 ? &k_matvec_fp8<FMT, XDT, 2>
+          : nt <= 4 ? &k_matvec_fp8<FMT, XDT, 4>
+                    : &k_matvec_fp8<FMT, XDT, 8>,
+          &k_matvec_reduce<XDT>};
+}
 int product_launch(const ProductKernels& f, const ProductCfg& m, cudaStream_t st) {
   const unsigned blocks = resident_grid(f.streams, kSyncSmemBytes, kSyncThreads, 4 * m.K);
   if (!blocks) return ZIPNN_B200_E_CUDA;
@@ -1568,8 +1579,16 @@ int product_scratch_size(ProductKind kind, const zipnn_b200_decode_plan* plan, i
   return ZIPNN_B200_OK;
 }
 
+// The fp8 matvec's weight format and scale grid (zipnn_b200_decode_plan_matvec_fp8 has checked all but the pointer).
+struct Fp8Scale {
+  int format;
+  const float* d_scale;
+  size_t block_rows, block_cols;
+};
+
 int product(ProductKind kind, const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, const void* d_x, size_t x_stride,
-            size_t n_tokens, const void* d_bias, void* d_y, size_t y_stride, void* d_scratch, size_t scratch_bytes, cudaStream_t st) {
+            size_t n_tokens, const void* d_bias, void* d_y, size_t y_stride, void* d_scratch, size_t scratch_bytes, cudaStream_t st,
+            const Fp8Scale* f8 = nullptr) {
   if (n_tokens > max_tokens(kind)) return ZIPNN_B200_E_ARG;
   ProductCfg m;
   {
@@ -1577,10 +1596,12 @@ int product(ProductKind kind, const zipnn_b200_decode_plan* plan, int item, int 
     if (rc) return rc;
   }
   if (n_tokens == 0) return ZIPNN_B200_OK;
-  if (!d_x || !d_y || !d_scratch || ((uintptr_t)d_x & 15) || ((uintptr_t)d_scratch & 255) || ((uintptr_t)d_y % m.esize) ||
-      ((uintptr_t)d_bias % m.esize))
+  const uint32_t xes = f8 ? (uint32_t)matvec_esize(dtype) : m.esize;  // bytes of an element of x, y and the bias
+  if (!d_x || !d_y || !d_scratch || ((uintptr_t)d_x & 15) || ((uintptr_t)d_scratch & 255) || ((uintptr_t)d_y % xes) ||
+      ((uintptr_t)d_bias % xes))
     return ZIPNN_B200_E_ARG;
-  if (n_tokens > 1 && ((x_stride * m.esize) % 16 || x_stride < m.in || y_stride < m.out)) return ZIPNN_B200_E_ARG;
+  if (f8 && (!f8->d_scale || ((uintptr_t)f8->d_scale & 3))) return ZIPNN_B200_E_ARG;
+  if (n_tokens > 1 && ((x_stride * xes) % 16 || x_stride < m.in || y_stride < m.out)) return ZIPNN_B200_E_ARG;
   if (scratch_bytes < product_scratch_bytes(kind, m, n_tokens)) return ZIPNN_B200_E_ARG;
   m.x = d_x;
   m.bias = d_bias;
@@ -1589,6 +1610,17 @@ int product(ProductKind kind, const zipnn_b200_decode_plan* plan, int item, int 
   m.xs = x_stride;
   m.ys = y_stride;
   m.nt = (uint32_t)n_tokens;
+  if (f8) {
+    // a block at least as tall or wide as the matrix is the whole of it: clamped, bn and bk stay below 2^31
+    const uint64_t bn = std::min<uint64_t>(f8->block_rows, m.out), bk = std::min<uint64_t>(f8->block_cols, m.in);
+    m.scale = f8->d_scale;
+    m.srow = matvec_fp8_recip(bn);
+    m.scol = matvec_fp8_recip(bk);
+    m.scols = (uint32_t)((m.in + bk - 1) / bk);
+    const bool e4 = f8->format == kFp8E4m3;
+    if (dtype == kMvBf16) return product_launch(e4 ? fp8_kernels<kFp8E4m3, kMvBf16>(m.nt) : fp8_kernels<kFp8E5m2, kMvBf16>(m.nt), m, st);
+    return product_launch(e4 ? fp8_kernels<kFp8E4m3, kMvFp16>(m.nt) : fp8_kernels<kFp8E5m2, kMvFp16>(m.nt), m, st);
+  }
   if (dtype == kMvBf16) return product_launch(product_kernels<kMvBf16>(kind, m.nt), m, st);
   if (dtype == kMvFp16) return product_launch(product_kernels<kMvFp16>(kind, m.nt), m, st);
   return product_launch(product_kernels<kMvFp32>(kind, m.nt), m, st);
@@ -1596,7 +1628,8 @@ int product(ProductKind kind, const zipnn_b200_decode_plan* plan, int item, int 
 }  // namespace
 
 static_assert(kMatvecMaxTokens == ZIPNN_B200_MATVEC_MAX_TOKENS && kMvBf16 == ZIPNN_B200_MATVEC_BF16 && kMvFp16 == ZIPNN_B200_MATVEC_FP16 &&
-                  kMvFp32 == ZIPNN_B200_MATVEC_FP32 && kMatmulMaxTokens == ZIPNN_B200_MATMUL_MAX_TOKENS,
+                  kMvFp32 == ZIPNN_B200_MATVEC_FP32 && kMatmulMaxTokens == ZIPNN_B200_MATMUL_MAX_TOKENS &&
+                  kFp8E4m3 == ZIPNN_B200_FP8_E4M3 && kFp8E5m2 == ZIPNN_B200_FP8_E5M2,
               "the header's constants are the kernels'");
 
 int zipnn_b200_decode_plan_matvec_scratch_size(const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, size_t n_tokens,
@@ -1621,6 +1654,21 @@ int zipnn_b200_decode_plan_matmul(const zipnn_b200_decode_plan* plan, int item, 
                                   void* cuda_stream) {
   return product(kMatmul, plan, item, dtype, in_features, d_x, x_stride, n_tokens, d_bias, d_y, y_stride, d_scratch, scratch_bytes,
                  (cudaStream_t)cuda_stream);
+}
+
+int zipnn_b200_decode_plan_matvec_fp8_scratch_size(const zipnn_b200_decode_plan* plan, int item, size_t in_features, size_t n_tokens,
+                                                   size_t* out) {
+  return product_scratch_size(kMatvecFp8, plan, item, kMvBf16, in_features, n_tokens, out);
+}
+
+int zipnn_b200_decode_plan_matvec_fp8(const zipnn_b200_decode_plan* plan, int item, int fp8_format, int x_dtype, size_t in_features,
+                                      const void* d_x, size_t x_stride, size_t n_tokens, const float* d_scale, size_t block_rows,
+                                      size_t block_cols, const void* d_bias, void* d_y, size_t y_stride, void* d_scratch,
+                                      size_t scratch_bytes, void* cuda_stream) {
+  if ((fp8_format != kFp8E4m3 && fp8_format != kFp8E5m2) || block_rows == 0 || block_cols < 16 || block_cols % 16) return ZIPNN_B200_E_ARG;
+  const Fp8Scale f8{fp8_format, d_scale, block_rows, block_cols};
+  return product(kMatvecFp8, plan, item, x_dtype, in_features, d_x, x_stride, n_tokens, d_bias, d_y, y_stride, d_scratch, scratch_bytes,
+                 (cudaStream_t)cuda_stream, &f8);
 }
 
 int zipnn_b200_split(const void* d_in, size_t n, int num_buf, int bits_mode, void* d_planes, size_t stride,

@@ -30,6 +30,7 @@ MATVEC_MAX_TOKENS = _native.MATVEC_MAX_TOKENS
 MATMUL_MAX_TOKENS = _native.MATMUL_MAX_TOKENS
 _MATVEC_DTYPES = {torch.bfloat16: 0, torch.float16: 1, torch.float32: 2}   # ZIPNN_B200_MATVEC_*
 _MATMUL_DTYPES = (torch.bfloat16, torch.float16)
+_FP8_FORMATS = {torch.float8_e4m3fn: _native.FP8_E4M3, torch.float8_e5m2: _native.FP8_E5M2}   # ZIPNN_B200_FP8_*
 
 
 def _round(n: int, a: int) -> int:
@@ -170,9 +171,11 @@ class DecodePlan:
         self._gather_scratch = None   # gather's default scratch, grown on demand
         self._matvec = _native.lib().zipnn_b200_decode_plan_matvec
         self._matmul = _native.lib().zipnn_b200_decode_plan_matmul
-        self._scratches = {}          # "matvec" / "matmul" -> that call's default scratch, grown on demand
+        self._matvec_fp8 = _native.lib().zipnn_b200_decode_plan_matvec_fp8
+        self._scratches = {}          # "matvec" / "matmul" / "matvec_fp8" -> that call's default scratch, grown on demand
         self._matvec_ok = {}          # (output, in_features) -> eligible?
         self._matmul_ok = {}
+        self._matvec_fp8_ok = {}
         self._select_ok = None        # select_ok(), once asked
         self._select_scratch = None   # run_select's default scratch
 
@@ -339,14 +342,19 @@ class DecodePlan:
         return dt, sh
 
     def _product_size(self, name: str, k: int, in_features: int, n_tokens: int) -> tuple:
-        """-> (status, scratch bytes) of zipnn_b200_decode_plan_{name}_scratch_size, `name` "matvec" or "matmul"."""
+        """-> (status, scratch bytes) of zipnn_b200_decode_plan_{name}_scratch_size, `name` "matvec", "matmul" or
+        "matvec_fp8"."""
         dt, _ = self._matvec_item(k)
         out = C.c_size_t(0)
-        if dt not in (_MATMUL_DTYPES if name == "matmul" else _MATVEC_DTYPES) or in_features <= 0:
+        dtypes = {"matvec": _MATVEC_DTYPES, "matmul": _MATMUL_DTYPES, "matvec_fp8": _FP8_FORMATS}[name]
+        if dt not in dtypes or in_features <= 0:
             return _native.E_UNSUPPORTED, 0
         with torch.cuda.device(self.device):
-            rc = getattr(_native.lib(), f"zipnn_b200_decode_plan_{name}_scratch_size")(self._ref, k, _MATVEC_DTYPES[dt], int(in_features),
-                                                                                      int(n_tokens), C.byref(out))
+            if name == "matvec_fp8":
+                rc = _native.lib().zipnn_b200_decode_plan_matvec_fp8_scratch_size(self._ref, k, int(in_features), int(n_tokens), C.byref(out))
+            else:
+                rc = getattr(_native.lib(), f"zipnn_b200_decode_plan_{name}_scratch_size")(self._ref, k, _MATVEC_DTYPES[dt], int(in_features),
+                                                                                          int(n_tokens), C.byref(out))
         return rc, out.value
 
     def matvec_ok(self, k: int, in_features: int) -> bool:
@@ -415,14 +423,79 @@ class DecodePlan:
         subnormal products) returns each weight bit for bit, as the matvec and decode + F.linear do."""
         return self._product("matmul", k, x, bias, out, scratch)
 
-    def _product(self, name: str, k: int, x, bias, out, scratch) -> torch.Tensor:
-        """matvec and matmul: the checks and the call, `name` choosing the limit, eligibility, scratch and function."""
-        mm = name == "matmul"
-        limit = MATMUL_MAX_TOKENS if mm else MATVEC_MAX_TOKENS
-        ok, scratch_bytes = (self.matmul_ok, self.matmul_scratch_bytes) if mm else (self.matvec_ok, self.matvec_scratch_bytes)
+    def matvec_fp8_ok(self, k: int, in_features: int) -> bool:
+        """Can `matvec_fp8` multiply by output `k` seen as rows of `in_features` elements?  True for a float8_e4m3fn or
+        float8_e5m2 output in one piece whose rows are a multiple of 16 elements and whose chunks all decode in the
+        fused mode (what fp8 weights produce).  The first call for an output synchronises (it reads the chunk modes);
+        never raises for an output that exists."""
         dt, sh = self._matvec_item(k)
+        n = 1
+        for d in sh:
+            n *= d
+        if dt not in _FP8_FORMATS or in_features <= 0 or n == 0 or n % in_features:
+            return False
+        if (k, in_features) not in self._matvec_fp8_ok:
+            self._matvec_fp8_ok[(k, in_features)] = self._product_size("matvec_fp8", k, in_features, 1)[0] == _native.OK
+        return self._matvec_fp8_ok[(k, in_features)]
+
+    def matvec_fp8_scratch_bytes(self, k: int, in_features: int, n_tokens: int = MATVEC_MAX_TOKENS) -> int:
+        """Bytes of a matvec_fp8 scratch for output `k`, rows of `in_features` elements and `n_tokens` rows of x."""
+        rc, n = self._product_size("matvec_fp8", k, in_features, n_tokens)
+        _native.check(rc)
+        return n
+
+    def matvec_fp8(self, k: int, x: torch.Tensor, scale: torch.Tensor, block: tuple = None, bias: torch.Tensor = None,
+                   out: torch.Tensor = None, scratch: torch.Tensor = None) -> torch.Tensor:
+        """`x @ (S * W).T (+ bias)` with W = output `k`, an fp8 tensor (float8_e4m3fn or float8_e5m2) seen as
+        [out_features, in_features], in_features = x.shape[-1], and S its fp32 scale grid, computed from the coded
+        streams: W is neither written nor read dense (zipnn_b200_decode_plan_matvec_fp8).  The weight the product uses
+        is float(W[o][i]) * scale[o // bn][i // bk] -- the stored scale multiplies, as `weight_scale_inv` does in fp8
+        checkpoints.  Two launches on the current CUDA stream, no host read: capturable in a CUDA graph.  Each group of
+        16 consecutive weights of a row is multiplied with x in fp32 and scaled once; the sums and the single rounding
+        are `matvec`'s, and two calls with the same inputs give the same bits.  An e4m3fn NaN or an e5m2 infinity or NaN
+        gives what the dense product of the dequantized matrix gives: NaN or an infinity in that row.
+
+        x:       CUDA bf16 or fp16 tensor [..., in_features] on the plan's device, at most MATVEC_MAX_TOKENS rows;
+                 rows that are not 16-byte aligned are copied first.
+        scale:   contiguous CUDA float32 tensor of ceil(out_features / bn) * ceil(in_features / bk) elements, row-major.
+        block:   (bn, bk), bn >= 1, bk >= 16 and a multiple of 16: (out_features, in_features) is one scale for the
+                 tensor, (1, in_features) one per row, (128, 128) DeepSeek's blocks.  None: a one-element scale, per
+                 tensor.
+        bias, out, scratch: as for `matvec`, in x's dtype; the scratch at least `matvec_fp8_scratch_bytes(k,
+                 in_features, rows)` bytes.
+        -> out.  ValueError for an output `matvec_fp8_ok` refuses.  Works without the plan's output buffer."""
+        return self._product("matvec_fp8", k, x, bias, out, scratch, scale=scale, block=block)
+
+    def _fp8_grid(self, x, scale, block, out_features: int) -> tuple:
+        """-> (bn, bk) after checking `scale` against the grid the block implies."""
+        in_features = x.shape[-1]
+        if not (isinstance(scale, torch.Tensor) and scale.is_cuda and scale.device == self.device and scale.dtype == torch.float32
+                and scale.is_contiguous()):
+            raise ValueError("matvec_fp8's scale must be a contiguous CUDA float32 tensor on the plan's device")
+        if block is None:
+            if scale.numel() != 1:
+                raise ValueError(f"matvec_fp8 takes block=None for a one-element scale only, not {scale.numel()} elements")
+            return out_features, in_features
+        bn, bk = (int(b) for b in block)
+        if bn < 1 or bk < 16 or bk % 16:
+            raise ValueError(f"matvec_fp8's block (bn, bk) needs bn >= 1 and bk a multiple of 16 of at least 16, not {(bn, bk)}")
+        grid = -(-out_features // bn) * -(-in_features // bk)
+        if scale.numel() != grid:
+            raise ValueError(f"matvec_fp8's scale for block {(bn, bk)} of a [{out_features}, {in_features}] weight has {grid} "
+                             f"elements, not {scale.numel()}")
+        return bn, bk
+
+    def _product(self, name: str, k: int, x, bias, out, scratch, scale=None, block=None) -> torch.Tensor:
+        """matvec, matmul and matvec_fp8: the checks and the call, `name` choosing the limit, eligibility, scratch and
+        function."""
+        mm, f8 = name == "matmul", name == "matvec_fp8"
+        limit = MATMUL_MAX_TOKENS if mm else MATVEC_MAX_TOKENS
+        ok, scratch_bytes = {"matvec": (self.matvec_ok, self.matvec_scratch_bytes), "matmul": (self.matmul_ok, self.matmul_scratch_bytes),
+                             "matvec_fp8": (self.matvec_fp8_ok, self.matvec_fp8_scratch_bytes)}[name]
+        wdt, sh = self._matvec_item(k)
+        dt = x.dtype if f8 and isinstance(x, torch.Tensor) and x.dtype in _MATMUL_DTYPES else wdt
         if not (isinstance(x, torch.Tensor) and x.is_cuda and x.device == self.device and x.dtype == dt and x.dim() >= 1):
-            raise ValueError(f"{name} takes a CUDA {dt} tensor [..., in_features] on the plan's device")
+            raise ValueError(f"{name} takes a CUDA {'bf16 or fp16' if f8 else dt} tensor [..., in_features] on the plan's device")
         in_features = x.shape[-1]
         lead = tuple(x.shape[:-1])
         n = 1
@@ -436,6 +509,8 @@ class DecodePlan:
         for d in sh:
             total *= d
         out_features = total // in_features
+        if f8:
+            bn, bk = self._fp8_grid(x, scale, block, out_features)
         es = x.element_size()
         x2 = x.reshape(max(n, 1), in_features) if n else x.reshape(0, in_features)
         if n and (x2.stride(1) != 1 or x2.data_ptr() % 16 or (n > 1 and (x2.stride(0) * es) % 16)):
@@ -468,9 +543,14 @@ class DecodePlan:
         elif not (isinstance(scratch, torch.Tensor) and scratch.is_cuda and scratch.device == self.device
                   and scratch.dtype == torch.uint8 and scratch.is_contiguous()):
             raise ValueError(f"{name}'s scratch must be a contiguous CUDA uint8 tensor on the plan's device")
-        rc = (self._matmul if mm else self._matvec)(self._ref, k, _MATVEC_DTYPES[dt], in_features, x2.data_ptr(), x2.stride(0), n,
-                                                    bias.data_ptr() if bias is not None else None, y2.data_ptr(), y2.stride(0),
-                                                    scratch.data_ptr(), scratch.numel(), torch.cuda.current_stream(self.device).cuda_stream)
+        if f8:
+            rc = self._matvec_fp8(self._ref, k, _FP8_FORMATS[wdt], _MATVEC_DTYPES[dt], in_features, x2.data_ptr(), x2.stride(0), n,
+                                  scale.data_ptr(), bn, bk, bias.data_ptr() if bias is not None else None, y2.data_ptr(), y2.stride(0),
+                                  scratch.data_ptr(), scratch.numel(), torch.cuda.current_stream(self.device).cuda_stream)
+        else:
+            rc = (self._matmul if mm else self._matvec)(self._ref, k, _MATVEC_DTYPES[dt], in_features, x2.data_ptr(), x2.stride(0), n,
+                                                        bias.data_ptr() if bias is not None else None, y2.data_ptr(), y2.stride(0),
+                                                        scratch.data_ptr(), scratch.numel(), torch.cuda.current_stream(self.device).cuda_stream)
         if rc:
             _native.check(rc)
         return out
