@@ -1,8 +1,8 @@
 """fp8 weights for the fp8 matvec tests (test_matvec_fp8_host.py, _gpu.py), and a numpy model of its numerics.
 
-A case is an fp8 tensor [out, in] (float8_e4m3fn or float8_e5m2), its bytes and an oracle-made stream body at num_buf 1
-(one byte plane per element, the plane is the bytes).  Every case is fused in every chunk (asserted from the stream
-with `plane_inputs.predict`).  The inventory:
+A case is a product_streams.Case of an fp8 tensor [out, in] (float8_e4m3fn or float8_e5m2): its bytes and an
+oracle-made stream body at num_buf 1 (one byte plane per element, the plane is the bytes), built by product_streams'
+builders.  Every case is fused in every chunk (asserted from the stream with `plane_inputs.predict`).  The inventory:
 
   shapes      every fused chunk size from 512 B to 128 KiB (the largest fp8 chunk) on rows shorter than a quarter,
               rows spanning chunks, in = 16, 48, 144 and 528, out = 1, a one-chunk tensor and a short last chunk;
@@ -16,19 +16,19 @@ Outside `special` no weight is NaN or infinite: one would turn its whole product
 """
 from __future__ import annotations
 
+import functools
+
 import numpy as np
 import torch
 
-import plane_inputs as P
-import test_decoder_tables_gpu as D
-from oracle import oracle as O
+import product_streams as S
 
 FORMATS = ("e4m3", "e5m2")
-TORCH = {"e4m3": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2}
-CODE = {"e4m3": 0, "e5m2": 1}                 # ZIPNN_B200_FP8_E4M3 / _E5M2
+TORCH = {f: S.TORCH[f] for f in FORMATS}
+CODE = {f: S.CODE[f] for f in FORMATS}        # ZIPNN_B200_FP8_E4M3 / _E5M2
 XDTYPES = {"bf16": torch.bfloat16, "fp16": torch.float16}
 XCODE = {"bf16": 0, "fp16": 1}                # ZIPNN_B200_MATVEC_BF16 / _FP16
-BITS, BYTES_MODE = 1, 10                      # what ZipNN writes for fp8 (the bit order is ignored at num_buf 1)
+BITS = 1                                      # what ZipNN writes for fp8 (the bit order is ignored at num_buf 1)
 CHUNKS = tuple(512 << i for i in range(9))    # every fused fp8 chunk size: 512 B .. 128 KiB
 
 
@@ -44,44 +44,6 @@ def safe(fmt: str, plane: np.ndarray) -> np.ndarray:
     bad = not_finite(fmt, out)
     out[bad] ^= 0x40
     return out
-
-
-def safe_lengths(fmt: str, nb: np.ndarray) -> np.ndarray:
-    """Code lengths with every coded NaN / infinity symbol moved to an uncoded finite one below 129."""
-    nb = np.asarray(nb, dtype=np.uint8).copy()
-    free = [v for v in range(129) if nb[v] == 0 and not not_finite(fmt, v)]
-    for v in np.nonzero((nb > 0) & not_finite(fmt, np.arange(256)))[0]:
-        to = free.pop(0)
-        nb[to], nb[v] = nb[v], 0
-    return nb
-
-
-class Case:
-    def __init__(self, name, fmt, chunk, shape, data, body=None, special=False):
-        self.name, self.fmt, self.chunk, self.special = name, fmt, chunk, special
-        self.G, self.bits, self.bm = 1, BITS, BYTES_MODE
-        self.data = np.ascontiguousarray(data, dtype=np.uint8).reshape(-1)
-        self.out, self.inn = shape
-        assert self.out * self.inn == self.data.size, (name, shape, self.data.size)
-        if body is None:
-            body = O.zipnn_compress(bytes(32), self.data, 1, BITS, BYTES_MODE, chunk, 0.95, threads=8)[32:]
-        self.body = np.ascontiguousarray(body, dtype=np.uint8)
-        self.pr = P.predict(self.body, 1, BITS, chunk, self.data.size)
-        assert self.pr["mode"] == ["fused"] * self.pr["K"], (name, self.pr["mode"])
-        if not special:
-            assert not not_finite(fmt, self.data).any(), f"{name}: a weight that is not finite"
-
-    @property
-    def shape(self):
-        return (self.out, self.inn)
-
-    def weights(self) -> torch.Tensor:
-        """W [out, in] on the host, in its fp8 dtype."""
-        return torch.from_numpy(self.data.copy()).view(TORCH[self.fmt]).reshape(self.out, self.inn)
-
-    def floats(self) -> np.ndarray:
-        """W as float32 (exact)."""
-        return self.weights().float().numpy()
 
 
 # ---------------------------------------------------------------- shapes
@@ -113,78 +75,28 @@ def shape_cases(chunk: int) -> list:
     out = []
     for k, (name, o, i) in enumerate(shapes(chunk)):
         fmt = FORMATS[(k + k0) % 2]
-        out.append(Case(f"{name}_{fmt}_c{chunk}", fmt, chunk, (o, i), laplace_bytes(fmt, o * i, 1000 * k0 + k)))
+        out.append(S.Case(f"{name}_{fmt}_c{chunk}", fmt, BITS, chunk, (o, i), laplace_bytes(fmt, o * i, 1000 * k0 + k)))
     return out
 
 
 # ---------------------------------------------------------------- crafted tables, rings, fixed-length codes
-def crafted_case(fmt: str) -> Case:
-    """Random Kraft-complete tables of every log from 1 to 11, each twice (once with a hot longest code), and a hot
-    symbol on an 11-bit code: one 4 KiB chunk per table, rows of 128."""
+def crafted_case(fmt: str) -> S.Case:
+    """product_streams.kraft_blocks: one 4 KiB chunk per table, rows of 128."""
     rng = np.random.default_rng(20 + CODE[fmt])
-    specs = []
-    for lg in range(1, 12):
-        for hot in (False, True):
-            nb = P.kraft_lengths(rng, int(rng.integers(lg + 1, min(100, 1 << lg) + 1)), lg)
-            specs.append((nb, int(np.nonzero(nb == nb.max())[0][0]) if hot else None))
-    nb = P.kraft_lengths(rng, 100, 11)
-    specs.append((nb, int(np.nonzero(nb == 11)[0][0])))
-    chunk, chunks, items = 4096, [], [[]]
-    for spec, hot in specs:
-        nb = safe_lengths(fmt, spec)
-        if hot is not None and nb[hot] == 0:   # the hot symbol was moved: follow it
-            hot = int(np.nonzero(nb == np.asarray(spec)[hot])[0][-1])
-        top = P.plane_for_lengths(rng, nb, chunk, hot)
-        blk = P.huf_block(nb, top)
-        assert len(blk) < chunk - 1
-        items[0].append((1, blk))
-        chunks.append(top)
-    data = np.concatenate(chunks)
-    return Case(f"crafted_{fmt}", fmt, chunk, (data.size // 128, 128), data, body=P.assemble_body(items, 1))
+    return S.crafted(f"crafted_{fmt}", fmt, BITS, 4096, S.kraft_blocks(rng), rng, 128, bad=functools.partial(not_finite, fmt))
 
 
-def from_tops(name, fmt, chunk, tops, seed, inn, last=None) -> Case:
-    rng = np.random.default_rng(seed)
-    parts = []
-    for c, fam in enumerate(tops):
-        n = last if (last and c == len(tops) - 1) else chunk
-        parts.append(safe(fmt, P.FAMILIES[fam](rng, n)))
-    data = np.concatenate(parts)
-    assert data.size % inn == 0, (name, data.size, inn)
-    return Case(name, fmt, chunk, (data.size // inn, inn), data)
-
-
-def ring_case(fmt: str) -> Case:
+def ring_case(fmt: str) -> S.Case:
     """128 KiB chunks whose quarter bitstreams are 28672 bytes (eq128) and about 30.8 KiB (heavy256): the second take
     the ring fallback of the sync decoder."""
-    return from_tops(f"ring_{fmt}", fmt, 131072, ["heavy256", "eq128", "heavy256"], 50 + CODE[fmt], 2048)
-
-
-def misaligned_quarter(L: int, lo: int, hi: int) -> int:
-    """Symbols per bitstream s (a multiple of 128, so that the chunk is a multiple of 512 bytes) with s * L > 192 * 256
-    bits and a CTA segment of ceil(s * L / 256) bits that is not a multiple of L."""
-    s = -(-lo // 128) * 128
-    while s <= hi:
-        if s * L > 192 * 256 and (-(-s * L // 256)) % L:
-            return s
-        s += 128
-    raise AssertionError((L, lo, hi))
-
-
-def fixed_length_cases(fmt: str) -> list:
-    """2^L equiprobable symbols, L = 2, 4, 6: a full 128 KiB chunk and a last chunk whose four quarters all start
-    their CTA segments off a code boundary."""
-    out = []
-    for fam, L in (("eq4", 2), ("eq16", 4), ("eq64", 6)):
-        s = misaligned_quarter(L, 12000, 131072 // 4)
-        out.append(from_tops(f"fixed{L}_{fmt}", fmt, 131072, [fam, fam], 60 + L, 64, last=4 * s))
-    return out
+    return S.from_planes(f"ring_{fmt}", fmt, BITS, 131072, ["heavy256", "eq128", "heavy256"], 50 + CODE[fmt], 2048,
+                         safe=functools.partial(safe, fmt))
 
 
 def stream_cases() -> list:
     out = []
     for fmt in FORMATS:
-        out += [crafted_case(fmt), ring_case(fmt)] + fixed_length_cases(fmt)
+        out += [crafted_case(fmt), ring_case(fmt)] + S.fixed_length_cases(fmt, BITS, safe=functools.partial(safe, fmt))
     return out
 
 
@@ -207,18 +119,18 @@ def special_case(fmt: str) -> tuple:
     mant = 8 if fmt == "e4m3" else 4   # exponent field 0, mantissa not 0
     for r, c in at["subnormal"]:
         w[r, c] = int(rng.integers(1, mant)) | (0x80 if rng.integers(0, 2) else 0)
-    return Case(f"special_{fmt}", fmt, 4096, (out, inn), w, special=True), at
+    return S.Case(f"special_{fmt}", fmt, BITS, 4096, (out, inn), w, special=True), at
 
 
 # ---------------------------------------------------------------- integer weights for exact sums
-def integer_case(fmt: str, chunk: int, shape, seed: int) -> Case:
+def integer_case(fmt: str, chunk: int, shape, seed: int) -> S.Case:
     """Integer weights that both formats hold exactly: e4m3fn -16..16, e5m2 -7..7."""
     top = 16 if fmt == "e4m3" else 7
     rng = np.random.default_rng(seed)
     v = np.clip(np.round(rng.normal(0, top / 3, shape)), -top, top)
     w = torch.from_numpy(v).to(TORCH[fmt])
     assert torch.equal(w.double(), torch.from_numpy(v))
-    return Case(f"int_{fmt}_{shape[0]}x{shape[1]}_c{chunk}", fmt, chunk, shape, w.view(torch.uint8).numpy())
+    return S.Case(f"int_{fmt}_{shape[0]}x{shape[1]}_c{chunk}", fmt, BITS, chunk, shape, w.view(torch.uint8).numpy())
 
 
 # ---------------------------------------------------------------- scale grids

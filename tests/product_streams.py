@@ -1,5 +1,6 @@
 """Compressed weights for the product tests (test_product_streams_host.py, _gpu.py): streams of every kind the
-decoder tests use, each one a matrix the matvec and the matmul must multiply by.
+decoder tests use, each one a matrix the matvec and the matmul must multiply by.  The builders also make the fp8
+corpus (fp8_streams.py): a Case takes any weight dtype of the products, fp8 ones included.
 
 A case is a tensor [out, in] of bf16, fp16 or fp32 in either byte layout (`bits`: 1 = the sign bit rotated next to
 the mantissa, 0 = not; a stream's layout comes from its header, not from the dtype, so every dtype is built in
@@ -23,6 +24,8 @@ would check nothing.
 from __future__ import annotations
 
 
+import functools
+
 import numpy as np
 import torch
 
@@ -30,10 +33,11 @@ import plane_inputs as P
 import test_decoder_tables_gpu as D
 from oracle import oracle as O
 
-TORCH = {"bf16": torch.bfloat16, "fp16": torch.float16, "fp32": torch.float32}
-ES = {"bf16": 2, "fp16": 2, "fp32": 4}
-CODE = {"bf16": 0, "fp16": 1, "fp32": 2}   # ZIPNN_B200_MATVEC_BF16 / FP16 / FP32
-BYTES_MODE = {2: 10, 4: 220}
+TORCH = {"bf16": torch.bfloat16, "fp16": torch.float16, "fp32": torch.float32, "e4m3": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2}
+ES = {"bf16": 2, "fp16": 2, "fp32": 4, "e4m3": 1, "e5m2": 1}
+# the weights' code in their product call: ZIPNN_B200_MATVEC_BF16 / FP16 / FP32, ZIPNN_B200_FP8_E4M3 / E5M2
+CODE = {"bf16": 0, "fp16": 1, "fp32": 2, "e4m3": 0, "e5m2": 1}
+BYTES_MODE = {1: 10, 2: 10, 4: 220}
 CHUNKS = tuple(512 << i for i in range(10))   # every chunk size a fused chunk can have: 512 B .. 256 KiB
 LAYOUTS16 = (("bf16", 1), ("bf16", 0), ("fp16", 1), ("fp16", 0))
 LAYOUTS = LAYOUTS16 + (("fp32", 1), ("fp32", 0))
@@ -66,18 +70,24 @@ def safe_top(dtype: str, bits: int, plane: np.ndarray) -> np.ndarray:
     return out
 
 
-def safe_lengths(dtype: str, bits: int, nb: np.ndarray) -> np.ndarray:
-    """Code lengths with every coded symbol that could encode an all-ones exponent swapped with an uncoded one below
-    129 (raw 4-bit weights describe at most 129 symbols)."""
+def safe_lengths(nb: np.ndarray, bad) -> np.ndarray:
+    """Code lengths with every coded symbol that `bad` marks (one that could make a weight that is not finite, as
+    `exp_all_ones` does) swapped with an uncoded one below 129 that it does not (raw 4-bit weights describe at most
+    129 symbols)."""
     nb = np.asarray(nb, dtype=np.uint8).copy()
-    free = [v for v in range(129) if nb[v] == 0 and not exp_all_ones(dtype, bits, np.uint8(v))]
-    for v in np.nonzero((nb > 0) & exp_all_ones(dtype, bits, np.arange(256)))[0]:
+    free = [v for v in range(129) if nb[v] == 0 and not bad(np.uint8(v))]
+    for v in np.nonzero((nb > 0) & bad(np.arange(256)))[0]:
         to = free.pop(0)
         nb[to], nb[v] = nb[v], 0
     return nb
 
 
 # ---------------------------------------------------------------- a case
+def tag(dtype: str, bits: int) -> str:
+    """A layout in case names: dtype and bit order, or the dtype alone for one-byte weights (num_buf 1 has no bit order)."""
+    return dtype if ES[dtype] == 1 else f"{dtype}b{bits}"
+
+
 class Case:
     def __init__(self, name, dtype, bits, chunk, shape, data, body=None, special=False):
         self.name, self.dtype, self.bits, self.chunk, self.special = name, dtype, bits, chunk, special
@@ -92,7 +102,7 @@ class Case:
         self.pr = P.predict(self.body, self.G, bits, chunk, self.data.size)
         assert self.pr["mode"] == ["fused"] * self.pr["K"], (name, self.pr["mode"])
         if not special:
-            assert bool(torch.isfinite(self.weights()).all()), f"{name}: a weight that is not finite"
+            assert bool(torch.isfinite(self.weights().float()).all()), f"{name}: a weight that is not finite"
 
     @property
     def shape(self):
@@ -102,6 +112,10 @@ class Case:
         """W [out, in] on the host."""
         return torch.from_numpy(self.data.copy()).view(TORCH[self.dtype]).reshape(self.out, self.inn)
 
+    def floats(self) -> np.ndarray:
+        """W as float32 (exact)."""
+        return self.weights().float().numpy()
+
     def top_items(self):
         return [self.pr["items"][self.G - 1][c] for c in range(self.pr["K"])]
 
@@ -110,10 +124,12 @@ class Case:
         return P.planes_of(self.data, self.G, self.bits, self.chunk)
 
 
-def from_planes(name, dtype, bits, chunk, tops, seed, shape_in, side=None, last=None):
-    """A tensor whose chunk c has the top plane tops[c] (a family name or an array; `safe_top` is applied) and the other
-    planes side(c, g), a family name or function (default: uniform bytes, stored raw); rows of `shape_in` elements."""
+def from_planes(name, dtype, bits, chunk, tops, seed, shape_in, side=None, last=None, safe=None):
+    """A tensor whose chunk c has the top plane tops[c] (a family name or an array; `safe`, default `safe_top`, is
+    applied) and the other planes side(c, g), a family name or function (default: uniform bytes, stored raw); rows of
+    `shape_in` elements."""
     G = ES[dtype]
+    safe = safe or functools.partial(safe_top, dtype, bits)
     rng = np.random.default_rng(seed)
     chunks = []
     for c, top in enumerate(tops):
@@ -122,7 +138,7 @@ def from_planes(name, dtype, bits, chunk, tops, seed, shape_in, side=None, last=
         for g in range(G):
             m = P.plane_len(n, G, g)
             if g == G - 1:
-                planes.append(safe_top(dtype, bits, top[:m] if isinstance(top, np.ndarray) else P.FAMILIES[top](rng, m)))
+                planes.append(safe(top[:m] if isinstance(top, np.ndarray) else P.FAMILIES[top](rng, m)))
             else:
                 fam = side(c, g) if side else "raw"
                 planes.append((fam if callable(fam) else P.FAMILIES[fam])(rng, m))
@@ -133,10 +149,12 @@ def from_planes(name, dtype, bits, chunk, tops, seed, shape_in, side=None, last=
     return Case(name, dtype, bits, chunk, (n // shape_in, shape_in), data)
 
 
-def crafted(name, dtype, bits, chunk, blocks, seed, shape_in, last=None):
+def crafted(name, dtype, bits, chunk, blocks, seed, shape_in, last=None, bad=None):
     """test_decoder_tables_gpu.crafted_case in any layout: blocks[c] = code lengths of chunk c's top plane, or
-    (lengths, a hot symbol), or a family name (the oracle's block).  Lengths go through `safe_lengths` first."""
+    (lengths, a hot symbol), or a family name (the oracle's block).  Lengths go through `safe_lengths` with `bad`
+    (default `exp_all_ones`) first.  `seed` may be a numpy Generator, which goes on drawing."""
     G = ES[dtype]
+    bad = bad or functools.partial(exp_all_ones, dtype, bits)
     rng = np.random.default_rng(seed)
     chunks, items = [], [[] for _ in range(G)]
     for c, spec in enumerate(blocks):
@@ -149,7 +167,7 @@ def crafted(name, dtype, bits, chunk, blocks, seed, shape_in, last=None):
         if isinstance(spec, str):
             top = safe_top(dtype, bits, P.FAMILIES[spec](rng, m))
         else:
-            nb = safe_lengths(dtype, bits, spec)
+            nb = safe_lengths(spec, bad)
             if hot is not None and nb[hot] == 0:   # the hot symbol was moved: follow it
                 hot = int(np.nonzero(nb == np.asarray(spec)[hot])[0][-1])
             top = P.plane_for_lengths(rng, nb, m, hot)
@@ -264,10 +282,9 @@ def family_case(dtype: str, bits: int) -> Case:
                        shape_in=256 if ES[dtype] == 2 else 128)
 
 
-def crafted_case(dtype: str, bits: int) -> Case:
-    """Random Kraft-complete tables of every log from 1 to 11, each twice (once with a hot longest code), and a hot
-    symbol on an 11-bit code."""
-    rng = np.random.default_rng(20 + 2 * CODE[dtype] + bits)
+def kraft_blocks(rng) -> list:
+    """`crafted` blocks: random Kraft-complete tables of every log from 1 to 11, each twice (once with a hot longest
+    code), and a hot symbol on an 11-bit code."""
     blocks = []
     for lg in range(1, 12):
         for hot in (False, True):
@@ -275,6 +292,12 @@ def crafted_case(dtype: str, bits: int) -> Case:
             blocks.append((nb, int(np.nonzero(nb == nb.max())[0][0])) if hot else nb)
     nb = P.kraft_lengths(rng, 100, 11)
     blocks.append((nb, int(np.nonzero(nb == 11)[0][0])))
+    return blocks
+
+
+def crafted_case(dtype: str, bits: int) -> Case:
+    """The `kraft_blocks` tables, one 4 KiB chunk each."""
+    blocks = kraft_blocks(np.random.default_rng(20 + 2 * CODE[dtype] + bits))
     return crafted(f"crafted_{dtype}b{bits}", dtype, bits, 4096, blocks, seed=30 + bits, shape_in=128)
 
 
@@ -314,28 +337,30 @@ def warp_mix_case(dtype: str, bits: int) -> Case:
     return from_planes(f"warps_{dtype}b{bits}", dtype, bits, chunk, tops, seed=40 + bits, shape_in=128, last=chunk - 512)
 
 
-def misaligned_quarter(L: int, lo: int, hi: int) -> int:
-    """Symbols per bitstream s (a multiple of 64, so the chunk is a multiple of 512 bytes for 16-bit weights) with
-    s * L > 192 * 256 bits and a CTA segment of ceil(s * L / 256) bits that is not a multiple of L."""
-    s = -(-lo // 64) * 64
+def misaligned_quarter(L: int, lo: int, hi: int, step: int) -> int:
+    """Symbols per bitstream s (a multiple of `step`: 64 for 16-bit weights and 128 for fp8, so that the chunk is a
+    multiple of 512 bytes) with s * L > 192 * 256 bits and a CTA segment of ceil(s * L / 256) bits that is not a
+    multiple of L."""
+    s = -(-lo // step) * step
     while s <= hi:
         if s * L > 192 * 256 and (-(-s * L // 256)) % L:
             return s
-        s += 64
+        s += step
     raise AssertionError((L, lo, hi))
 
 
-def fixed_length_cases(dtype: str, bits: int) -> list:
-    """2^L equiprobable symbols (fixed-length codes, which never resynchronise), L = 2, 4, 6: a full 256 KiB chunk and a
-    last chunk whose four quarters all start their CTA segments off a code boundary (16-bit weights: an fp32 top plane
-    of a 256 KiB chunk is too short for L = 2)."""
+def fixed_length_cases(dtype: str, bits: int, safe=None) -> list:
+    """2^L equiprobable symbols (fixed-length codes, which never resynchronise), L = 2, 4, 6: a full chunk (256 KiB for
+    16-bit weights, 128 KiB for fp8: the largest) and a last chunk whose four quarters all start their CTA segments
+    off a code boundary (not fp32: its top plane of a 256 KiB chunk is too short for L = 2).  `safe` as for
+    `from_planes`."""
     G = ES[dtype]
-    chunk = 262144
+    chunk = 131072 * G
     out = []
     for fam, L in (("eq4", 2), ("eq16", 4), ("eq64", 6)):
-        s = misaligned_quarter(L, 12000, chunk // G // 4)
-        out.append(from_planes(f"fixed{L}_{dtype}b{bits}", dtype, bits, chunk, [fam, fam], seed=60 + L, shape_in=64,
-                               last=4 * s * G))
+        s = misaligned_quarter(L, 12000, chunk // G // 4, 128 // G)
+        out.append(from_planes(f"fixed{L}_{tag(dtype, bits)}", dtype, bits, chunk, [fam, fam], seed=60 + L, shape_in=64,
+                               last=4 * s * G, safe=safe))
     return out
 
 

@@ -19,57 +19,26 @@ import torch
 import corrupt_streams as CS
 import fp8_streams as F
 import test_decode_plan_gpu as DP
+from test_product_streams_gpu import POISON, SCRATCH, _first_bad, _st, raw_plan, same_bits, scratch_size
 from zipnn_b200 import DecodePlan, ZipNN, _native
 from zipnn_b200.plan import MATVEC_MAX_TOKENS
 
 pytestmark = pytest.mark.gpu
 
-POISON = 0xFF   # fp32 NaN in every scratch slot
 LAYOUT_NAMES = ("tensor", "row", "block128", "bk16")
 
 
-def _st():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _scratch(need):
-    s = torch.full((need + 256,), POISON, dtype=torch.uint8, device="cuda")
-    return s[:need]
-
-
-def raw_plan(cases) -> DP.Plan:
-    p = DP.Plan([DP.Item(c.name, c.body, 1, c.bits, c.chunk, c.data.size, c.data) for c in cases])
-    assert p.rc == 0, [c.name for c in cases]
-    return p
-
-
-def scratch_size(ref, item, inf, nt):
-    sz = C.c_size_t(0)
-    rc = _native.lib().zipnn_b200_decode_plan_matvec_fp8_scratch_size(ref, item, inf, nt, C.byref(sz))
-    return rc, sz.value
-
-
-def call(ref, item, fmt, xdt, x, scale, bn, bk, y_ptr, ys, bias=None):
+def call(p, item, fmt, xdt, x, scale, bn, bk, y_ptr, ys, bias=None):
     """One raw call on a poisoned scratch: asserts success and two launches."""
     nt, inf = x.shape
-    rc, need = scratch_size(ref, item, inf, nt)
+    rc, need = scratch_size("matvec_fp8", p, item, None, inf, nt)
     assert rc == 0, (item, rc)
-    s = _scratch(need)
+    s = SCRATCH.get(need)
     before = _native.launch_count()
-    rc = _native.lib().zipnn_b200_decode_plan_matvec_fp8(ref, item, F.CODE[fmt], F.XCODE[xdt], inf, x.data_ptr(), x.stride(0), nt,
-                                                         scale.data_ptr(), bn, bk, None if bias is None else bias.data_ptr(), y_ptr, ys,
-                                                         s.data_ptr(), need, _st())
+    rc = _native.lib().zipnn_b200_decode_plan_matvec_fp8(C.byref(p.plan), item, F.CODE[fmt], F.XCODE[xdt], inf, x.data_ptr(), x.stride(0),
+                                                         nt, scale.data_ptr(), bn, bk, None if bias is None else bias.data_ptr(), y_ptr,
+                                                         ys, s.data_ptr(), need, _st())
     assert rc == 0 and _native.launch_count() - before == 2, (item, rc)
-
-
-def same_bits(got, want):
-    """Elementwise on float tensors: equal, or both NaN (+0 == -0)."""
-    return (got == want) | (torch.isnan(got) & torch.isnan(want))
-
-
-def _first_bad(ok):
-    bad = (~ok).nonzero()
-    return None if bad.numel() == 0 else tuple(bad[0].tolist())
 
 
 def _scale(case, layout, seed):
@@ -91,7 +60,7 @@ def check_one_hot(p, item, case, xdt, layout, k=0):
         n = min(MATVEC_MAX_TOKENS, inn - i0)
         x.zero_()
         x.view(-1).index_fill_(0, ar[:n] * (inn + 1) + i0, 2.0 ** k)
-        call(p.plan_ref, item, case.fmt, xdt, x[:n], sd, bn, bk, ybuf[1 + i0].data_ptr() + 3 * ybuf.element_size(), out + 6)
+        call(p, item, case.dtype, xdt, x[:n], sd, bn, bk, ybuf[1 + i0].data_ptr() + 3 * ybuf.element_size(), out + 6)
     mask = torch.ones_like(ybuf, dtype=torch.bool)
     mask[1: inn + 1, 3: 3 + out] = False
     assert torch.all(torch.isnan(ybuf[mask])), f"{case.name}: wrote outside y"
@@ -109,22 +78,16 @@ def check_model(p, item, case, xdt, layout, nt, seed):
     x = torch.randn(nt, case.inn, generator=g).to(dt)
     bias = torch.randn(case.out, generator=g).to(dt) * 2.0 ** -10
     y = torch.full((nt, case.out), float("nan"), dtype=dt, device="cuda")
-    call(p.plan_ref, item, case.fmt, xdt, x.cuda(), sd, bn, bk, y.data_ptr(), case.out, bias=bias.cuda())
+    call(p, item, case.dtype, xdt, x.cuda(), sd, bn, bk, y.data_ptr(), case.out, bias=bias.cuda())
     want = F.model(case.floats(), s, bn, bk, x.float().numpy(), case.chunk, xdt, bias=bias.float().numpy())
     ok = same_bits(y.float().cpu(), torch.from_numpy(want))
     assert bool(ok.all()), (case.name, xdt, layout, nt, _first_bad(ok))
 
 
-def _plan(cases):
-    p = raw_plan(cases)
-    p.plan_ref = C.byref(p.plan)
-    return p
-
-
 @pytest.mark.parametrize("chunk", F.CHUNKS)
 def test_shapes_at_every_chunk_size(chunk):
     cases = F.shape_cases(chunk)
-    p = _plan(cases)   # one plan: items of different shapes and formats in turn
+    p = raw_plan(cases)   # one plan: items of different shapes and formats in turn
     k0 = F.CHUNKS.index(chunk)
     for i, case in enumerate(cases):
         xdt = ("bf16", "fp16")[(i + k0) % 2]
@@ -138,7 +101,7 @@ def test_shapes_at_every_chunk_size(chunk):
 
 def test_stream_kinds():
     for j, case in enumerate(F.stream_cases()):
-        p = _plan([case])
+        p = raw_plan([case])
         for xdt in ("bf16", "fp16"):
             check_one_hot(p, 0, case, xdt, LAYOUT_NAMES[(j + (xdt == "fp16")) % 4])
         check_model(p, 0, case, "bf16", LAYOUT_NAMES[(j + 2) % 4], 8, j)
@@ -153,7 +116,7 @@ def test_exact_integer_sums():
     for j, (fmt, chunk, shape) in enumerate((("e4m3", 512, (160, 400)), ("e5m2", 4096, (5, 8192)), ("e4m3", 131072, (64, 4096)),
                                              ("e5m2", 2048, (48, 160)))):
         case = F.integer_case(fmt, chunk, shape, j)
-        p = _plan([case])
+        p = raw_plan([case])
         for layout in LAYOUT_NAMES:
             bn, bk = F.layouts(case.out, case.inn)[layout]
             s = (2.0 ** rng.integers(-2, 3, F.grid_shape(case.out, case.inn, bn, bk))).astype(np.float32)
@@ -162,7 +125,7 @@ def test_exact_integer_sums():
                 for nt in (1, 3, 8):
                     x = torch.from_numpy(rng.integers(-2, 3, (nt, case.inn)).astype(np.float32)).to(F.XDTYPES[xdt])
                     y = torch.full((nt, case.out), float("nan"), dtype=F.XDTYPES[xdt], device="cuda")
-                    call(p.plan_ref, 0, fmt, xdt, x.cuda(), torch.from_numpy(s).cuda(), bn, bk, y.data_ptr(), case.out)
+                    call(p, 0, fmt, xdt, x.cuda(), torch.from_numpy(s).cuda(), bn, bk, y.data_ptr(), case.out)
                     want = torch.from_numpy(x.double().numpy() @ wd.T).to(y.dtype)
                     assert torch.equal(y.cpu(), want), (case.name, layout, xdt, nt)
 
@@ -283,7 +246,7 @@ def test_every_item_of_a_multi_item_plan_interleaved_with_runs():
 @pytest.mark.parametrize("fmt", F.FORMATS)
 def test_special_values(fmt):
     case, at = F.special_case(fmt)
-    p = _plan([case])
+    p = raw_plan([case])
     w = case.weights().double().cuda()
     bad_rows = ~torch.isfinite(w).all(1)
     assert int(bad_rows.sum()) == (2 if fmt == "e4m3" else 5)
@@ -297,7 +260,7 @@ def test_special_values(fmt):
         for i0 in range(0, case.inn, 8):
             x.zero_()
             x[torch.arange(8), i0 + torch.arange(8)] = 1.0
-            call(p.plan_ref, 0, fmt, xdt, x, sd, case.out, case.inn, ybuf[i0].data_ptr(), case.out)
+            call(p, 0, fmt, xdt, x, sd, case.out, case.inn, ybuf[i0].data_ptr(), case.out)
         ref = (torch.eye(case.inn, dtype=torch.float64, device="cuda") @ (w * 0.25).T)   # NaN and inf where fp64 gives them
         want = torch.from_numpy(F.one_hot_model(case.floats(), s, case.out, case.inn, np.arange(case.inn), 0, xdt)).cuda()
         want = torch.where(bad_rows[None, :], ref.float(), want).to(dt)
@@ -306,7 +269,7 @@ def test_special_values(fmt):
         # random x: NaN exactly where the fp64 product is NaN, the same infinity where it is infinite
         xr = torch.randn(5, case.inn, generator=torch.Generator("cuda").manual_seed(1), device="cuda").to(dt)
         y = torch.zeros(5, case.out, dtype=dt, device="cuda")
-        call(p.plan_ref, 0, fmt, xdt, xr, sd, case.out, case.inn, y.data_ptr(), case.out)
+        call(p, 0, fmt, xdt, xr, sd, case.out, case.inn, y.data_ptr(), case.out)
         ref = xr.double() @ (w * 0.25).T
         assert torch.equal(torch.isnan(y), torch.isnan(ref)), (fmt, xdt, "NaN")
         inf = torch.isinf(ref)
@@ -378,7 +341,7 @@ def test_host_rejections_write_nothing(monkeypatch):
     assert boxed.rc == 0
     for p_ref in (pl._ref, C.byref(boxed.plan)):
         before = _native.launch_count()
-        assert scratch_size(p_ref, 0, 16, 1)[0] == U
+        assert L.zipnn_b200_decode_plan_matvec_fp8_scratch_size(p_ref, 0, 16, 1, C.byref(C.c_size_t(0))) == U
         assert L.zipnn_b200_decode_plan_matvec_fp8(p_ref, 0, 0, 0, 16, x.data_ptr(), 16, 1, scale.data_ptr(), 1, 16, None,
                                                    y.data_ptr(), 64, scratch.data_ptr(), need, _st()) == U
         assert _native.launch_count() == before

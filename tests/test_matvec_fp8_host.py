@@ -107,7 +107,7 @@ def test_fp8_conversion_is_exact_in_fp32():
 @pytest.mark.parametrize("chunk", F.CHUNKS)
 def test_shape_cases_are_what_they_claim(chunk):
     cases = F.shape_cases(chunk)   # (Case asserts that every chunk is fused and every weight finite)
-    assert {c.fmt for c in cases} == set(F.FORMATS)
+    assert {c.dtype for c in cases} == set(F.FORMATS)
     inns = {c.inn for c in cases}
     assert {16, 48, 144, 528} <= inns
     assert any(c.out == 1 for c in cases)
@@ -123,14 +123,14 @@ def test_shape_cases_are_what_they_claim(chunk):
 
 def test_stream_cases_are_what_they_claim():
     cases = F.stream_cases()
-    assert {c.fmt for c in cases} == set(F.FORMATS)
+    assert {c.dtype for c in cases} == set(F.FORMATS)
     for fmt in F.FORMATS:
         crafted = [c for c in cases if c.name == f"crafted_{fmt}"][0]
         logs = {crafted.pr["items"][0][k].lg for k in range(crafted.pr["K"])}
         assert logs == set(range(1, 12)), (fmt, logs)
         ring = [c for c in cases if c.name == f"ring_{fmt}"][0]
         assert max(max(it.s_len) for it in (ring.pr["items"][0][k] for k in range(ring.pr["K"]))) > P.SYNC_STREAM_CAP
-        fixed = [c for c in cases if c.name.startswith("fixed") and c.fmt == fmt]
+        fixed = [c for c in cases if c.name.startswith("fixed") and c.dtype == fmt]
         assert sorted(c.pr["items"][0][0].fixed_len for c in fixed) == [2, 4, 6]
         for c in fixed:
             assert P.misaligned_sync_guesses(c.pr["items"][0][-1]) == 4, c.name

@@ -61,8 +61,11 @@ def raw_plan(cases) -> DP.Plan:
 
 
 def scratch_size(kind, p, item, code, inf, nt):
+    """-> (status, bytes) of zipnn_b200_decode_plan_{kind}_scratch_size; `code` the weights' dtype, None for
+    matvec_fp8, which takes none."""
     sz = C.c_size_t(0)
-    rc = getattr(_native.lib(), f"zipnn_b200_decode_plan_{kind}_scratch_size")(C.byref(p.plan), item, code, inf, nt, C.byref(sz))
+    codes = () if code is None else (code,)
+    rc = getattr(_native.lib(), f"zipnn_b200_decode_plan_{kind}_scratch_size")(C.byref(p.plan), item, *codes, inf, nt, C.byref(sz))
     return rc, sz.value
 
 
@@ -80,7 +83,7 @@ def product(kind, p, item, code, x, y_ptr, ys, bias=None, scratch=None):
 
 
 def same_bits(got, want, mask=None):
-    """Elementwise: equal bits, or both zero, or both NaN (where mask)."""
+    """Elementwise on float tensors: equal bits, or both zero (+0 == -0), or both NaN (where mask)."""
     it = {2: torch.int16, 4: torch.int32}[got.element_size()]
     ok = (got.view(it) == want.view(it)) | ((got == 0) & (want == 0)) | (torch.isnan(got) & torch.isnan(want))
     return ok if mask is None else ok | ~mask

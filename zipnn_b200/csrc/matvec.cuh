@@ -9,8 +9,8 @@
 //   k_matvec_reduce  one thread per (token, output row) adds the row's partial sums in ascending element order, adds the
 //                    bias, rounds once to the output type and stores.
 //
-// k_matvec_fp8 is k_matvec for fp8 weights with an fp32 scale grid and bf16 / fp16 x (MatvecFp8Ep, below); its partial
-// sums go through k_matvec_reduce unchanged.
+// k_matvec_fp8 is k_matvec for fp8 weights with an fp32 scale grid and bf16 / fp16 x: the same epilogue, MatvecEp, with
+// the fp8 product of a lane's vector (below); its partial sums go through k_matvec_reduce unchanged.
 //
 // Thread mapping.  The run's store loop gives thread t the vectors t, t + 256, ...: fine for stores, but it scatters a
 // row of W over all threads, so every row would end in a CTA-wide reduction.  Here a warp owns a contiguous BLOCK of
@@ -103,106 +103,14 @@ __device__ __forceinline__ void matvec_floats(const uint32_t (&r)[4], float (&f)
   }
 }
 
-// NT: the accumulators a lane holds, n_tokens rounded up to a power of two.  Tokens past n_tokens repeat the last one
-// and are not stored: 3 and 5 to 7 tokens pay for 4 and 8.  A uniform `t < n_tokens` exit from the token loop was
-// measured instead: it keeps the loads of the tokens from being issued together, and 8 tokens took 1.3 to 1.5 times as long.
-template <int DT, int NT>
-struct MatvecEp {
-  static constexpr bool on = true;
-  static constexpr int EPV = 16 / matvec_esize(DT);
-  ProductCfg m;
-
-  __device__ __forceinline__ void flush(float (&acc)[NT], float* slot, int lane) const {
-#pragma unroll
-    for (int t = 0; t < NT; t++) {
-      float v = acc[t];
-#pragma unroll
-      for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-      if (lane == t && (uint32_t)t < m.nt) slot[t] = v;
-      acc[t] = 0.f;
-    }
-  }
-
-  // The quarter plane of bitstream `stream` of chunk c is in S.plane (count elements from plane byte out_off).
-  template <int G>
-  __device__ __forceinline__ void quarter(const SyncShared& S, uint64_t c, int stream, uint32_t out_off, uint32_t count, bool rot) const {
-    static_assert(G == matvec_esize(DT), "one byte plane per byte of the element");
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const uint32_t nv = count / EPV;
-    const uint32_t vpw = ((nv + 255u) >> 8) << 5;
-    const uint32_t v0 = (uint32_t)wid * vpw, v1 = min(nv, v0 + vpw);
-    if (v0 >= v1) return;  // (warp-uniform) a short last chunk leaves the upper warps without a block
-    const uint64_t in = m.in;
-    const uint64_t e0 = c * m.ce + out_off + (uint64_t)v0 * EPV;
-    uint64_t row0 = e0 / in, col0 = e0 - row0 * in;  // of the step's first element: the same in every lane
-    float* const slots = m.part + ((c * 4 + (uint32_t)stream) * 8 + (uint32_t)wid) * m.rs * m.nt;  // the block's, from its first row
-    const uint64_t first = row0;
-    const uint8_t* const xb = reinterpret_cast<const uint8_t*>(m.x);
-    float acc[NT];
-#pragma unroll
-    for (int t = 0; t < NT; t++) acc[t] = 0.f;
-    uint64_t cur = row0;
-    for (uint32_t v = v0; v < v1; v += 32) {
-      const uint32_t nvalid = min(32u, v1 - v);
-      const bool valid = (uint32_t)lane < nvalid;
-      uint64_t lrow = row0, lcol = col0 + (uint32_t)lane * EPV;
-      uint64_t last = row0;
-      if (col0 + 32u * EPV > in) {  // (uniform) the step straddles rows
-        const uint64_t q = lcol / in;
-        lrow += q;
-        lcol -= q * in;
-        last += (col0 + nvalid * EPV - 1) / in;
-      }
-      float p[NT];
-#pragma unroll
-      for (int t = 0; t < NT; t++) p[t] = 0.f;
-      if (valid) {
-        uint32_t r[4];
-        const uint32_t o = (v + (uint32_t)lane) * 16u;
-        ZB_FUSED_VECTOR(G, S, out_off, o, rot, r);
-        float w[EPV];
-        matvec_floats<DT, EPV>(r, w);
-#pragma unroll
-        for (int t = 0; t < NT; t++) {
-          const uint64_t tt = min((uint32_t)t, m.nt - 1u);
-          const uint4 xv = __ldg(reinterpret_cast<const uint4*>(xb + (tt * m.xs + lcol) * matvec_esize(DT)));
-          const uint32_t xr[4] = {xv.x, xv.y, xv.z, xv.w};
-          float xf[EPV];
-          matvec_floats<DT, EPV>(xr, xf);
-          float s = 0.f;
-#pragma unroll
-          for (int i = 0; i < EPV; i++) s = fmaf(w[i], xf[i], s);
-          p[t] = s;
-        }
-      }
-      for (uint64_t rr = row0; rr <= last; rr++) {
-        if (rr != cur) {
-          flush(acc, slots + (cur - first) * m.nt, lane);
-          cur = rr;
-        }
-        if (lrow == rr) {
-#pragma unroll
-          for (int t = 0; t < NT; t++) acc[t] += p[t];
-        }
-      }
-      row0 += m.step_rows;
-      col0 += m.step_cols;
-      if (col0 >= in) {
-        col0 -= in;
-        row0++;
-      }
-    }
-    flush(acc, slots + (cur - first) * m.nt, lane);
-  }
-};
-
 // ---- fp8 weights with an fp32 scale grid (k_matvec_fp8) -------------------------------------------------------------
 // y[t][o] = sum_i x[t][i] * (float(W[o][i]) * S[o / bn][i / bk]) (+ bias[o]), W of float8_e4m3fn or float8_e5m2 in one
 // byte plane (G = 1), x, bias and y of bf16 or fp16.  bk % 16 == 0, so a lane's 16 weights (one vector) lie in one row
 // and one scale block: the lane forms s = fma(w15, x15, ... fma(w0, x0, 0)) in fp32, in ascending column order, and
-// p = s * S[block] with one multiply; from there on everything is MatvecEp's (per-lane row accumulators, the butterfly,
-// one slot per (block, row, token), k_matvec_reduce).  fp8 -> fp32 is exact in both formats, subnormals included; an
-// e4m3fn NaN or an e5m2 infinity or NaN acts as in the dense product of the dequantized matrix.
+// p = s * S[block] with one multiply; everything else is the matvec's (per-lane row accumulators, the butterfly, one
+// slot per (block, row, token), k_matvec_reduce).  A step is 32 lanes x 16 weights, and a lane reads 32 bytes of x per
+// token and one scale per step (the grid is small and stays in L1 / L2).  fp8 -> fp32 is exact in both formats,
+// subnormals included; an e4m3fn NaN or an e5m2 infinity or NaN acts as in the dense product of the dequantized matrix.
 enum : int { kFp8E4m3 = 0, kFp8E5m2 = 1 };
 
 // floor(n / d) for n, d < 2^31 as one 64-bit multiply-high by r = ceil(2^64 / (2 d)), no division: 2n * r / 2^64 =
@@ -223,17 +131,36 @@ __device__ __forceinline__ void fp8_floats(uint32_t a, uint32_t b, float (&f)[8]
   }
 }
 
-// The warp-owns-a-block mapping and the row walk are MatvecEp's (its flush is reused); a step is 32 lanes x 16 weights,
-// and a lane reads 32 bytes of x per token and one scale per step (the grid is small and stays in L1 / L2).
-template <int FMT, int XDT, int NT>
-struct MatvecFp8Ep : MatvecEp<XDT, NT> {
-  static constexpr int EPV = 16;
-  using MatvecEp<XDT, NT>::m;
-  using MatvecEp<XDT, NT>::flush;
+// The matvec epilogue of sync_process: the warp-owns-a-block mapping and the row walk.  Only the product of a lane's
+// 16 decoded bytes differs between weight types: FMT < 0, weights of DT, one FMA chain over the vector's EPV elements;
+// FMT = kFp8E4m3 / kFp8E5m2, fp8 weights with a scale grid and x of DT (bf16 or fp16), the FMA chain over 16 weights
+// and one multiply by the scale (above).
+//
+// NT: the accumulators a lane holds, n_tokens rounded up to a power of two.  Tokens past n_tokens repeat the last one
+// and are not stored: 3 and 5 to 7 tokens pay for 4 and 8.  A uniform `t < n_tokens` exit from the token loop was
+// measured instead: it keeps the loads of the tokens from being issued together, and 8 tokens took 1.3 to 1.5 times as long.
+template <int DT, int NT, int FMT = -1>
+struct MatvecEp {
+  static_assert(FMT < 0 || DT != kMvFp32, "fp8 weights: x of bf16 or fp16");
+  static constexpr bool on = true;
+  static constexpr int EPV = FMT < 0 ? 16 / matvec_esize(DT) : 16;
+  ProductCfg m;
 
+  __device__ __forceinline__ void flush(float (&acc)[NT], float* slot, int lane) const {
+#pragma unroll
+    for (int t = 0; t < NT; t++) {
+      float v = acc[t];
+#pragma unroll
+      for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if (lane == t && (uint32_t)t < m.nt) slot[t] = v;
+      acc[t] = 0.f;
+    }
+  }
+
+  // The quarter plane of bitstream `stream` of chunk c is in S.plane (count elements from plane byte out_off).
   template <int G>
   __device__ __forceinline__ void quarter(const SyncShared& S, uint64_t c, int stream, uint32_t out_off, uint32_t count, bool rot) const {
-    static_assert(G == 1 && XDT != kMvFp32, "fp8 weights: one byte plane; x of bf16 or fp16");
+    static_assert(G == 16 / EPV, "one byte plane per byte of the element");
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const uint32_t nv = count / EPV;
     const uint32_t vpw = ((nv + 255u) >> 8) << 5;
@@ -263,7 +190,29 @@ struct MatvecFp8Ep : MatvecEp<XDT, NT> {
       float p[NT];
 #pragma unroll
       for (int t = 0; t < NT; t++) p[t] = 0.f;
-      if (valid) {
+      // The lane's 16 decoded bytes times x.  Each product decodes in a `valid` block of its own: with one block shared
+      // around both, ptxas assigned some k_matvec registers differently.
+      if constexpr (FMT < 0) {
+        if (valid) {
+          uint32_t r[4];
+          const uint32_t o = (v + (uint32_t)lane) * 16u;
+          ZB_FUSED_VECTOR(G, S, out_off, o, rot, r);
+          float w[EPV];
+          matvec_floats<DT, EPV>(r, w);
+#pragma unroll
+          for (int t = 0; t < NT; t++) {
+            const uint64_t tt = min((uint32_t)t, m.nt - 1u);
+            const uint4 xv = __ldg(reinterpret_cast<const uint4*>(xb + (tt * m.xs + lcol) * matvec_esize(DT)));
+            const uint32_t xr[4] = {xv.x, xv.y, xv.z, xv.w};
+            float xf[EPV];
+            matvec_floats<DT, EPV>(xr, xf);
+            float s = 0.f;
+#pragma unroll
+            for (int i = 0; i < EPV; i++) s = fmaf(w[i], xf[i], s);
+            p[t] = s;
+          }
+        }
+      } else if (valid) {
         uint32_t r[4];
         const uint32_t o = (v + (uint32_t)lane) * 16u;
         ZB_FUSED_VECTOR(G, S, out_off, o, rot, r);
@@ -281,7 +230,7 @@ struct MatvecFp8Ep : MatvecEp<XDT, NT> {
             const uint4 xv = __ldg(reinterpret_cast<const uint4*>(xb + (tt * m.xs + lcol) * 2) + h);
             const uint32_t xr[4] = {xv.x, xv.y, xv.z, xv.w};
             float xf[8];
-            matvec_floats<XDT, 8>(xr, xf);
+            matvec_floats<DT, 8>(xr, xf);
 #pragma unroll
             for (int i = 0; i < 8; i++) p[t] = fmaf(w[i], xf[i], p[t]);
           }
@@ -370,7 +319,7 @@ __global__ void __launch_bounds__(256) k_matvec_reduce(ProductCfg m) {
 // fp8 weights: the partial sums are k_matvec_reduce<XDT>'s, whose block geometry comes from m.esize (1).
 template <int FMT, int XDT, int NT>
 __global__ void __launch_bounds__(kSyncThreads, 3) k_matvec_fp8(ProductCfg m) {
-  product_streams<1>(m, MatvecFp8Ep<FMT, XDT, NT>{{m}});
+  product_streams<1>(m, MatvecEp<XDT, NT, FMT>{m});
 }
 
 }  // namespace zb

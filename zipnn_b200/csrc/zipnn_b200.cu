@@ -1539,25 +1539,28 @@ size_t product_scratch_bytes(ProductKind kind, const ProductCfg& m, size_t n_tok
 }
 
 // The bitstream kernel of a product, by how many tokens its lanes hold (matvec: 1, 2, 4 or 8; matmul: 1, 2 or 4 tiles of
-// 16), and its reduce.
+// 16), and its reduce.  DT is the type of x and y; `fmt` the fp8 matvec's weight format (ignored by the others).
 using ProductKernel = void (*)(ProductCfg);
 struct ProductKernels {
   ProductKernel streams, reduce;
 };
+extern "C++" template <int DT, int NT>
+ProductKernel matvec_kernel(ProductKind kind, int fmt) {
+  if constexpr (DT != kMvFp32) {  // (product_item refuses fp32 x for fp8 weights)
+    if (kind == kMatvecFp8) return fmt == kFp8E4m3 ? &k_matvec_fp8<kFp8E4m3, DT, NT> : &k_matvec_fp8<kFp8E5m2, DT, NT>;
+  }
+  return &k_matvec<DT, NT>;
+}
 extern "C++" template <int DT>
-ProductKernels product_kernels(ProductKind kind, uint32_t nt) {
+ProductKernels product_kernels(ProductKind kind, int fmt, uint32_t nt) {
   if constexpr (DT != kMvFp32) {  // (product_item refuses an fp32 matmul)
     if (kind == kMatmul) return {nt <= 16 ? &k_matmul<DT, 1> : nt <= 32 ? &k_matmul<DT, 2> : &k_matmul<DT, 4>, &k_matmul_reduce<DT>};
   }
-  return {nt <= 1 ? &k_matvec<DT, 1> : nt <= 2 ? &k_matvec<DT, 2> : nt <= 4 ? &k_matvec<DT, 4> : &k_matvec<DT, 8>, &k_matvec_reduce<DT>};
-}
-extern "C++" template <int FMT, int XDT>
-ProductKernels fp8_kernels(uint32_t nt) {
-  return {nt <= 1   ? &k_matvec_fp8<FMT, XDT, 1>
-          : nt <= 2 ? &k_matvec_fp8<FMT, XDT, 2>
-          : nt <= 4 ? &k_matvec_fp8<FMT, XDT, 4>
-                    : &k_matvec_fp8<FMT, XDT, 8>,
-          &k_matvec_reduce<XDT>};
+  return {nt <= 1   ? matvec_kernel<DT, 1>(kind, fmt)
+          : nt <= 2 ? matvec_kernel<DT, 2>(kind, fmt)
+          : nt <= 4 ? matvec_kernel<DT, 4>(kind, fmt)
+                    : matvec_kernel<DT, 8>(kind, fmt),
+          &k_matvec_reduce<DT>};
 }
 int product_launch(const ProductKernels& f, const ProductCfg& m, cudaStream_t st) {
   const unsigned blocks = resident_grid(f.streams, kSyncSmemBytes, kSyncThreads, 4 * m.K);
@@ -1596,7 +1599,7 @@ int product(ProductKind kind, const zipnn_b200_decode_plan* plan, int item, int 
     if (rc) return rc;
   }
   if (n_tokens == 0) return ZIPNN_B200_OK;
-  const uint32_t xes = f8 ? (uint32_t)matvec_esize(dtype) : m.esize;  // bytes of an element of x, y and the bias
+  const uint32_t xes = (uint32_t)matvec_esize(dtype);  // bytes of an element of x, y and the bias
   if (!d_x || !d_y || !d_scratch || ((uintptr_t)d_x & 15) || ((uintptr_t)d_scratch & 255) || ((uintptr_t)d_y % xes) ||
       ((uintptr_t)d_bias % xes))
     return ZIPNN_B200_E_ARG;
@@ -1617,13 +1620,11 @@ int product(ProductKind kind, const zipnn_b200_decode_plan* plan, int item, int 
     m.srow = matvec_fp8_recip(bn);
     m.scol = matvec_fp8_recip(bk);
     m.scols = (uint32_t)((m.in + bk - 1) / bk);
-    const bool e4 = f8->format == kFp8E4m3;
-    if (dtype == kMvBf16) return product_launch(e4 ? fp8_kernels<kFp8E4m3, kMvBf16>(m.nt) : fp8_kernels<kFp8E5m2, kMvBf16>(m.nt), m, st);
-    return product_launch(e4 ? fp8_kernels<kFp8E4m3, kMvFp16>(m.nt) : fp8_kernels<kFp8E5m2, kMvFp16>(m.nt), m, st);
   }
-  if (dtype == kMvBf16) return product_launch(product_kernels<kMvBf16>(kind, m.nt), m, st);
-  if (dtype == kMvFp16) return product_launch(product_kernels<kMvFp16>(kind, m.nt), m, st);
-  return product_launch(product_kernels<kMvFp32>(kind, m.nt), m, st);
+  const int fmt = f8 ? f8->format : kFp8E4m3;
+  if (dtype == kMvBf16) return product_launch(product_kernels<kMvBf16>(kind, fmt, m.nt), m, st);
+  if (dtype == kMvFp16) return product_launch(product_kernels<kMvFp16>(kind, fmt, m.nt), m, st);
+  return product_launch(product_kernels<kMvFp32>(kind, fmt, m.nt), m, st);
 }
 }  // namespace
 

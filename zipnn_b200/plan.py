@@ -15,6 +15,8 @@ overwrite each other's outputs.
 from __future__ import annotations
 
 import ctypes as C
+import math
+from typing import NamedTuple
 
 import torch
 
@@ -31,6 +33,23 @@ MATMUL_MAX_TOKENS = _native.MATMUL_MAX_TOKENS
 _MATVEC_DTYPES = {torch.bfloat16: 0, torch.float16: 1, torch.float32: 2}   # ZIPNN_B200_MATVEC_*
 _MATMUL_DTYPES = (torch.bfloat16, torch.float16)
 _FP8_FORMATS = {torch.float8_e4m3fn: _native.FP8_E4M3, torch.float8_e5m2: _native.FP8_E5M2}   # ZIPNN_B200_FP8_*
+
+
+class _Product(NamedTuple):
+    """What sets one product of `DecodePlan` apart from the others."""
+    name: str        # the method's, and zipnn_b200_decode_plan_{name} / _{name}_scratch_size
+    limit: int       # rows of x
+    weights: dict    # weight dtype -> its code in the native calls (the fp8 format, or the dtype)
+    x_dtypes: tuple  # x's dtypes, or None: the weights'
+    scaled: bool     # fp8 weights with a scale grid: the native calls take the format and x's dtype, and the grid
+
+    def native(self, suffix: str = ""):
+        return getattr(_native.lib(), f"zipnn_b200_decode_plan_{self.name}{suffix}")
+
+
+_MATVEC = _Product("matvec", MATVEC_MAX_TOKENS, _MATVEC_DTYPES, None, False)
+_MATMUL = _Product("matmul", MATMUL_MAX_TOKENS, {dt: _MATVEC_DTYPES[dt] for dt in _MATMUL_DTYPES}, None, False)
+_MATVEC_FP8 = _Product("matvec_fp8", MATVEC_MAX_TOKENS, _FP8_FORMATS, _MATMUL_DTYPES, True)
 
 
 def _round(n: int, a: int) -> int:
@@ -168,21 +187,35 @@ class DecodePlan:
         self._gather = _native.lib().zipnn_b200_decode_plan_gather
         self._ref = C.byref(self._plan)
         self._offs = [(o, p.nbytes, p.dtype, p.shape) for p, o in zip(parsed, offs)]
-        self._gather_scratch = None   # gather's default scratch, grown on demand
-        self._matvec = _native.lib().zipnn_b200_decode_plan_matvec
-        self._matmul = _native.lib().zipnn_b200_decode_plan_matmul
-        self._matvec_fp8 = _native.lib().zipnn_b200_decode_plan_matvec_fp8
-        self._scratches = {}          # "matvec" / "matmul" / "matvec_fp8" -> that call's default scratch, grown on demand
-        self._matvec_ok = {}          # (output, in_features) -> eligible?
-        self._matmul_ok = {}
-        self._matvec_fp8_ok = {}
+        self._scratches = {}          # method name -> that call's default scratch, grown on demand
+        self._product_ok = {}         # (method name, output, in_features) -> eligible?
         self._select_ok = None        # select_ok(), once asked
-        self._select_scratch = None   # run_select's default scratch
+
+    def _check_out(self) -> None:
+        if self._out is None:
+            raise RuntimeError("DecodePlan: the output buffer was released (release_out); only gather runs")
+
+    def _check_ids(self, name: str, ids) -> None:
+        if not (isinstance(ids, torch.Tensor) and ids.is_cuda and ids.device == self.device and ids.dtype in (torch.int32, torch.int64)):
+            raise ValueError(f"{name} takes CUDA int32 or int64 ids on the plan's device")
+
+    def _scratch_for(self, name: str, scratch, need) -> torch.Tensor:
+        """The caller's `scratch` for method `name` once checked, or, for None, the plan's default scratch of that
+        method, grown to `need()` bytes."""
+        if scratch is None:
+            n = need()
+            own = self._scratches.get(name)
+            if own is None or own.numel() < n:
+                own = self._scratches[name] = torch.empty(n, dtype=torch.uint8, device=self.device)
+            return own
+        if not (isinstance(scratch, torch.Tensor) and scratch.is_cuda and scratch.device == self.device
+                and scratch.dtype == torch.uint8 and scratch.is_contiguous()):
+            raise ValueError(f"{name}'s scratch must be a contiguous CUDA uint8 tensor on the plan's device")
+        return scratch
 
     def run(self) -> list:
         """Enqueue the decode on the current CUDA stream (launches only) and return `.outputs`."""
-        if self._out is None:
-            raise RuntimeError("DecodePlan: the output buffer was released (release_out); only gather runs")
+        self._check_out()
         rc = self._run(self._ref, torch.cuda.current_stream(self.device).cuda_stream)
         if rc:
             _native.check(rc)
@@ -192,8 +225,7 @@ class DecodePlan:
         """The outputs' views of another buffer `out` (same offsets, dtypes and shapes as `.outputs`); ValueError
         unless `out` is a contiguous CUDA uint8 tensor on the plan's device, 16-byte aligned, of at least
         `nbytes["out"]` bytes."""
-        if self._out is None:
-            raise RuntimeError("DecodePlan: the output buffer was released (release_out); only gather runs")
+        self._check_out()
         if not (isinstance(out, torch.Tensor) and out.is_cuda and out.device == self.device and out.dtype == torch.uint8
                 and out.dim() == 1 and out.is_contiguous()):
             raise ValueError("run_into takes a flat contiguous CUDA uint8 tensor on the plan's device")
@@ -248,8 +280,7 @@ class DecodePlan:
         -> out.  An id outside [0, rows) gets a zero row and makes `check()` raise IndexError (from then on: the
         plan's error word is sticky).  Works without the plan's output buffer (`release_out`)."""
         row, dt, sh = self._gather_row(k)
-        if not (isinstance(ids, torch.Tensor) and ids.is_cuda and ids.device == self.device and ids.dtype in (torch.int32, torch.int64)):
-            raise ValueError("gather takes CUDA int32 or int64 ids on the plan's device")
+        self._check_ids("gather", ids)
         ids_c = ids.contiguous()
         shape = tuple(ids.shape) + tuple(sh[1:])
         if out is None:
@@ -260,14 +291,7 @@ class DecodePlan:
         n = ids_c.numel()
         if n == 0:
             return out
-        if scratch is None:
-            need = self.gather_scratch_bytes(k, GATHER_SLOTS)
-            if self._gather_scratch is None or self._gather_scratch.numel() < need:
-                self._gather_scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
-            scratch = self._gather_scratch
-        elif not (isinstance(scratch, torch.Tensor) and scratch.is_cuda and scratch.device == self.device
-                  and scratch.dtype == torch.uint8 and scratch.is_contiguous()):
-            raise ValueError("gather's scratch must be a contiguous CUDA uint8 tensor on the plan's device")
+        scratch = self._scratch_for("gather", scratch, lambda: self.gather_scratch_bytes(k, GATHER_SLOTS))
         rc = self._gather(self._ref, k, row, ids_c.data_ptr(), n, ids_c.element_size(), out.data_ptr(), scratch.data_ptr(),
                           scratch.numel(), torch.cuda.current_stream(self.device).cuda_stream)
         if rc:
@@ -310,24 +334,15 @@ class DecodePlan:
                  Default: a buffer kept by the plan.
         An id outside [0, shape[0]) selects nothing and makes `check()` raise IndexError (from then on: the plan's
         error word is sticky).  ValueError for a plan `select_ok` refuses."""
-        if self._out is None:
-            raise RuntimeError("DecodePlan: the output buffer was released (release_out); only gather runs")
-        if not (isinstance(ids, torch.Tensor) and ids.is_cuda and ids.device == self.device and ids.dtype in (torch.int32, torch.int64)):
-            raise ValueError("run_select takes CUDA int32 or int64 ids on the plan's device")
+        self._check_out()
+        self._check_ids("run_select", ids)
         if not self.select_ok():
             raise ValueError("run_select needs outputs that share shape[0], each a whole tensor in one piece (see select_ok)")
         ids_c = ids.contiguous()
         n = ids_c.numel()
         if n == 0:
             return self.outputs
-        if scratch is None:
-            need = self.select_scratch_bytes()
-            if self._select_scratch is None or self._select_scratch.numel() < need:
-                self._select_scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
-            scratch = self._select_scratch
-        elif not (isinstance(scratch, torch.Tensor) and scratch.is_cuda and scratch.device == self.device
-                  and scratch.dtype == torch.uint8 and scratch.is_contiguous()):
-            raise ValueError("run_select's scratch must be a contiguous CUDA uint8 tensor on the plan's device")
+        scratch = self._scratch_for("run_select", scratch, self.select_scratch_bytes)
         rc = _native.lib().zipnn_b200_decode_plan_run_select(self._ref, self._offs[0][3][0], ids_c.data_ptr(), n, ids_c.element_size(),
                                                              scratch.data_ptr(), scratch.numel(),
                                                              torch.cuda.current_stream(self.device).cuda_stream)
@@ -335,48 +350,48 @@ class DecodePlan:
             _native.check(rc)
         return self.outputs
 
-    def _matvec_item(self, k: int) -> tuple:
+    def _product_item(self, k: int) -> tuple:
+        """-> (dtype, elements) of output k."""
         if not 0 <= k < len(self._offs):
             raise IndexError(f"DecodePlan has {len(self._offs)} outputs, not {k + 1}")
         _, _, dt, sh = self._offs[k]
-        return dt, sh
+        return dt, math.prod(sh)
 
-    def _product_size(self, name: str, k: int, in_features: int, n_tokens: int) -> tuple:
-        """-> (status, scratch bytes) of zipnn_b200_decode_plan_{name}_scratch_size, `name` "matvec", "matmul" or
-        "matvec_fp8"."""
-        dt, _ = self._matvec_item(k)
+    def _product_size(self, kind: _Product, k: int, in_features: int, n_tokens: int) -> tuple:
+        """-> (status, scratch bytes) of zipnn_b200_decode_plan_{kind.name}_scratch_size."""
+        dt, _ = self._product_item(k)
         out = C.c_size_t(0)
-        dtypes = {"matvec": _MATVEC_DTYPES, "matmul": _MATMUL_DTYPES, "matvec_fp8": _FP8_FORMATS}[name]
-        if dt not in dtypes or in_features <= 0:
+        if dt not in kind.weights or in_features <= 0:
             return _native.E_UNSUPPORTED, 0
+        dtype = () if kind.scaled else (kind.weights[dt],)
         with torch.cuda.device(self.device):
-            if name == "matvec_fp8":
-                rc = _native.lib().zipnn_b200_decode_plan_matvec_fp8_scratch_size(self._ref, k, int(in_features), int(n_tokens), C.byref(out))
-            else:
-                rc = getattr(_native.lib(), f"zipnn_b200_decode_plan_{name}_scratch_size")(self._ref, k, _MATVEC_DTYPES[dt], int(in_features),
-                                                                                          int(n_tokens), C.byref(out))
+            rc = kind.native("_scratch_size")(self._ref, k, *dtype, int(in_features), int(n_tokens), C.byref(out))
         return rc, out.value
+
+    def _ok(self, kind: _Product, k: int, in_features: int) -> bool:
+        dt, n = self._product_item(k)
+        if dt not in kind.weights or in_features <= 0 or n == 0 or n % in_features:
+            return False
+        key = (kind.name, k, in_features)
+        if key not in self._product_ok:
+            self._product_ok[key] = self._product_size(kind, k, in_features, 1)[0] == _native.OK
+        return self._product_ok[key]
+
+    def _scratch_bytes(self, kind: _Product, k: int, in_features: int, n_tokens: int) -> int:
+        rc, n = self._product_size(kind, k, in_features, n_tokens)
+        _native.check(rc)
+        return n
 
     def matvec_ok(self, k: int, in_features: int) -> bool:
         """Can `matvec` multiply by output `k` seen as rows of `in_features` elements?  True for a bf16 / fp16 / fp32
         output in one piece whose rows are a multiple of 16 bytes and whose chunks all decode in the fused mode (what
         float weights produce; a constant tensor or a ragged tail does not).  The first call for an output
         synchronises (it reads the chunk modes); never raises for an output that exists."""
-        _, sh = self._matvec_item(k)
-        n = 1
-        for d in sh:
-            n *= d
-        if in_features <= 0 or n == 0 or n % in_features:
-            return False
-        if (k, in_features) not in self._matvec_ok:
-            self._matvec_ok[(k, in_features)] = self._product_size("matvec", k, in_features, 1)[0] == _native.OK
-        return self._matvec_ok[(k, in_features)]
+        return self._ok(_MATVEC, k, in_features)
 
     def matvec_scratch_bytes(self, k: int, in_features: int, n_tokens: int = MATVEC_MAX_TOKENS) -> int:
         """Bytes of a matvec scratch for output `k`, rows of `in_features` elements and `n_tokens` rows of x."""
-        rc, n = self._product_size("matvec", k, in_features, n_tokens)
-        _native.check(rc)
-        return n
+        return self._scratch_bytes(_MATVEC, k, in_features, n_tokens)
 
     def matvec(self, k: int, x: torch.Tensor, bias: torch.Tensor = None, out: torch.Tensor = None,
                scratch: torch.Tensor = None) -> torch.Tensor:
@@ -394,23 +409,16 @@ class DecodePlan:
                  bytes.  It holds nothing between calls: calls (and plan runs) that share it must be ordered on one
                  stream.  Default: a buffer kept by the plan.
         -> out.  ValueError for an output `matvec_ok` refuses.  Works without the plan's output buffer."""
-        return self._product("matvec", k, x, bias, out, scratch)
+        return self._product(_MATVEC, k, x, bias, out, scratch)
 
     def matmul_ok(self, k: int, in_features: int) -> bool:
         """Can `matmul` multiply by output `k` seen as rows of `in_features` elements?  What `matvec_ok` accepts, for
         bf16 and fp16 outputs only (an fp32 output decodes).  Never raises for an output that exists."""
-        dt, _ = self._matvec_item(k)
-        if dt not in _MATMUL_DTYPES or not self.matvec_ok(k, in_features):
-            return False
-        if (k, in_features) not in self._matmul_ok:
-            self._matmul_ok[(k, in_features)] = self._product_size("matmul", k, in_features, 1)[0] == _native.OK
-        return self._matmul_ok[(k, in_features)]
+        return self._ok(_MATMUL, k, in_features)
 
     def matmul_scratch_bytes(self, k: int, in_features: int, n_tokens: int = MATMUL_MAX_TOKENS) -> int:
         """Bytes of a matmul scratch for output `k`, rows of `in_features` elements and `n_tokens` rows of x."""
-        rc, n = self._product_size("matmul", k, in_features, n_tokens)
-        _native.check(rc)
-        return n
+        return self._scratch_bytes(_MATMUL, k, in_features, n_tokens)
 
     def matmul(self, k: int, x: torch.Tensor, bias: torch.Tensor = None, out: torch.Tensor = None,
                scratch: torch.Tensor = None) -> torch.Tensor:
@@ -421,28 +429,18 @@ class DecodePlan:
         inputs give the same bits.  x must be finite: an infinity may give NaN where the dense product gives one.
         Subnormal weights are kept, not flushed: on an H100 80GB HBM3, x = 1 times bf16 exponent-0 weights (fp32
         subnormal products) returns each weight bit for bit, as the matvec and decode + F.linear do."""
-        return self._product("matmul", k, x, bias, out, scratch)
+        return self._product(_MATMUL, k, x, bias, out, scratch)
 
     def matvec_fp8_ok(self, k: int, in_features: int) -> bool:
         """Can `matvec_fp8` multiply by output `k` seen as rows of `in_features` elements?  True for a float8_e4m3fn or
         float8_e5m2 output in one piece whose rows are a multiple of 16 elements and whose chunks all decode in the
         fused mode (what fp8 weights produce).  The first call for an output synchronises (it reads the chunk modes);
         never raises for an output that exists."""
-        dt, sh = self._matvec_item(k)
-        n = 1
-        for d in sh:
-            n *= d
-        if dt not in _FP8_FORMATS or in_features <= 0 or n == 0 or n % in_features:
-            return False
-        if (k, in_features) not in self._matvec_fp8_ok:
-            self._matvec_fp8_ok[(k, in_features)] = self._product_size("matvec_fp8", k, in_features, 1)[0] == _native.OK
-        return self._matvec_fp8_ok[(k, in_features)]
+        return self._ok(_MATVEC_FP8, k, in_features)
 
     def matvec_fp8_scratch_bytes(self, k: int, in_features: int, n_tokens: int = MATVEC_MAX_TOKENS) -> int:
         """Bytes of a matvec_fp8 scratch for output `k`, rows of `in_features` elements and `n_tokens` rows of x."""
-        rc, n = self._product_size("matvec_fp8", k, in_features, n_tokens)
-        _native.check(rc)
-        return n
+        return self._scratch_bytes(_MATVEC_FP8, k, in_features, n_tokens)
 
     def matvec_fp8(self, k: int, x: torch.Tensor, scale: torch.Tensor, block: tuple = None, bias: torch.Tensor = None,
                    out: torch.Tensor = None, scratch: torch.Tensor = None) -> torch.Tensor:
@@ -464,7 +462,7 @@ class DecodePlan:
         bias, out, scratch: as for `matvec`, in x's dtype; the scratch at least `matvec_fp8_scratch_bytes(k,
                  in_features, rows)` bytes.
         -> out.  ValueError for an output `matvec_fp8_ok` refuses.  Works without the plan's output buffer."""
-        return self._product("matvec_fp8", k, x, bias, out, scratch, scale=scale, block=block)
+        return self._product(_MATVEC_FP8, k, x, bias, out, scratch, scale=scale, block=block)
 
     def _fp8_grid(self, x, scale, block, out_features: int) -> tuple:
         """-> (bn, bk) after checking `scale` against the grid the block implies."""
@@ -485,31 +483,22 @@ class DecodePlan:
                              f"elements, not {scale.numel()}")
         return bn, bk
 
-    def _product(self, name: str, k: int, x, bias, out, scratch, scale=None, block=None) -> torch.Tensor:
-        """matvec, matmul and matvec_fp8: the checks and the call, `name` choosing the limit, eligibility, scratch and
-        function."""
-        mm, f8 = name == "matmul", name == "matvec_fp8"
-        limit = MATMUL_MAX_TOKENS if mm else MATVEC_MAX_TOKENS
-        ok, scratch_bytes = {"matvec": (self.matvec_ok, self.matvec_scratch_bytes), "matmul": (self.matmul_ok, self.matmul_scratch_bytes),
-                             "matvec_fp8": (self.matvec_fp8_ok, self.matvec_fp8_scratch_bytes)}[name]
-        wdt, sh = self._matvec_item(k)
-        dt = x.dtype if f8 and isinstance(x, torch.Tensor) and x.dtype in _MATMUL_DTYPES else wdt
+    def _product(self, kind: _Product, k: int, x, bias, out, scratch, scale=None, block=None) -> torch.Tensor:
+        """matvec, matmul and matvec_fp8: the checks and the call."""
+        name = kind.name
+        wdt, total = self._product_item(k)
+        dt = x.dtype if kind.x_dtypes and isinstance(x, torch.Tensor) and x.dtype in kind.x_dtypes else wdt
         if not (isinstance(x, torch.Tensor) and x.is_cuda and x.device == self.device and x.dtype == dt and x.dim() >= 1):
-            raise ValueError(f"{name} takes a CUDA {'bf16 or fp16' if f8 else dt} tensor [..., in_features] on the plan's device")
+            raise ValueError(f"{name} takes a CUDA {'bf16 or fp16' if kind.x_dtypes else dt} tensor [..., in_features] on the plan's device")
         in_features = x.shape[-1]
         lead = tuple(x.shape[:-1])
-        n = 1
-        for d in lead:
-            n *= d
-        if n > limit:
-            raise ValueError(f"{name} takes at most {limit} rows of x, not {n}")
-        if not ok(k, in_features):
+        n = math.prod(lead)
+        if n > kind.limit:
+            raise ValueError(f"{name} takes at most {kind.limit} rows of x, not {n}")
+        if not self._ok(kind, k, in_features):
             raise ValueError(f"{name} cannot multiply by output {k} with in_features {in_features} (see {name}_ok)")
-        total = 1
-        for d in sh:
-            total *= d
         out_features = total // in_features
-        if f8:
+        if kind.scaled:
             bn, bk = self._fp8_grid(x, scale, block, out_features)
         es = x.element_size()
         x2 = x.reshape(max(n, 1), in_features) if n else x.reshape(0, in_features)
@@ -534,23 +523,14 @@ class DecodePlan:
             y2 = None
         if y2 is None or y2.stride(1) != 1:
             raise ValueError(f"{name}'s out must have contiguous rows, equally spaced")
-        if scratch is None:
-            need = scratch_bytes(k, in_features)
-            own = self._scratches.get(name)
-            if own is None or own.numel() < need:
-                own = self._scratches[name] = torch.empty(need, dtype=torch.uint8, device=self.device)
-            scratch = own
-        elif not (isinstance(scratch, torch.Tensor) and scratch.is_cuda and scratch.device == self.device
-                  and scratch.dtype == torch.uint8 and scratch.is_contiguous()):
-            raise ValueError(f"{name}'s scratch must be a contiguous CUDA uint8 tensor on the plan's device")
-        if f8:
-            rc = self._matvec_fp8(self._ref, k, _FP8_FORMATS[wdt], _MATVEC_DTYPES[dt], in_features, x2.data_ptr(), x2.stride(0), n,
-                                  scale.data_ptr(), bn, bk, bias.data_ptr() if bias is not None else None, y2.data_ptr(), y2.stride(0),
-                                  scratch.data_ptr(), scratch.numel(), torch.cuda.current_stream(self.device).cuda_stream)
+        scratch = self._scratch_for(name, scratch, lambda: self._scratch_bytes(kind, k, in_features, kind.limit))
+        if kind.scaled:
+            dtypes, grid = (kind.weights[wdt], _MATVEC_DTYPES[dt]), (scale.data_ptr(), bn, bk)
         else:
-            rc = (self._matmul if mm else self._matvec)(self._ref, k, _MATVEC_DTYPES[dt], in_features, x2.data_ptr(), x2.stride(0), n,
-                                                        bias.data_ptr() if bias is not None else None, y2.data_ptr(), y2.stride(0),
-                                                        scratch.data_ptr(), scratch.numel(), torch.cuda.current_stream(self.device).cuda_stream)
+            dtypes, grid = (kind.weights[dt],), ()
+        rc = kind.native()(self._ref, k, *dtypes, in_features, x2.data_ptr(), x2.stride(0), n, *grid,
+                           bias.data_ptr() if bias is not None else None, y2.data_ptr(), y2.stride(0), scratch.data_ptr(),
+                           scratch.numel(), torch.cuda.current_stream(self.device).cuda_stream)
         if rc:
             _native.check(rc)
         return out
