@@ -340,6 +340,21 @@ int zipnn_b200_decode_plan_matvec_fp8(const zipnn_b200_decode_plan* plan, int it
                                       const void* d_bias, void* d_y, size_t y_stride,
                                       void* d_scratch, size_t scratch_bytes, void* cuda_stream);
 
+/* _dequant_fp8: the dequantized weight of an item _matvec_fp8 takes, written straight from its coded bitstreams:
+ * d_out[o][i] = out_dtype(float(W[o][i]) * S[o / block_rows][i / block_cols]), W, d_scale and the blocks as for
+ * _matvec_fp8, d_out a contiguous [out_features][in_features] tensor of out_dtype, ZIPNN_B200_MATVEC_BF16 or _FP16.
+ * The values are bit for bit torch's (W.to(float32) * S_expanded).to(out_dtype): fp8 -> fp32 is exact, then one fp32
+ * multiply and one round to nearest even; fp16 overflow gives +-inf, NaN stays NaN (its payload may differ).  Exactly
+ * out_features * in_features elements are written.  Two launches (the decode with the dequantizing store, then the
+ * fold of a decode error into the plan's error word, which _status reports), no scratch, no host read but the first
+ * call's read of the chunk modes (as _matvec): capturable in a CUDA graph.
+ * Eligible items (else E_UNSUPPORTED): those _matvec_fp8 takes.
+ * Host-side rejections launch and write nothing: E_ARG as _matvec_fp8 refuses fp8_format, the blocks, d_scale, the
+ * plan, the item and in_features, and for an out_dtype other than BF16 or FP16 and a NULL or not 16-byte aligned d_out. */
+int zipnn_b200_decode_plan_dequant_fp8(const zipnn_b200_decode_plan* plan, int item, int fp8_format, int out_dtype,
+                                       size_t in_features, const float* d_scale, size_t block_rows, size_t block_cols,
+                                       void* d_out, void* cuda_stream);
+
 /* ---- stage 1 alone ------------------------------------------------------------ */
 /* d_planes: num_buf planes of `stride` bytes each; plane g receives byte g of every element
  * of the (optionally rotated) input.  Lengths as in the reference: n/num_buf, the first

@@ -10,7 +10,8 @@
 //                    bias, rounds once to the output type and stores.
 //
 // k_matvec_fp8 is k_matvec for fp8 weights with an fp32 scale grid and bf16 / fp16 x: the same epilogue, MatvecEp, with
-// the fp8 product of a lane's vector (below); its partial sums go through k_matvec_reduce unchanged.
+// the fp8 product of a lane's vector (below); its partial sums go through k_matvec_reduce unchanged.  k_dequant_fp8
+// (end of file) writes such a weight dequantized to bf16 / fp16 through the same bitstream loop, with no reduce.
 //
 // Thread mapping.  The run's store loop gives thread t the vectors t, t + 256, ...: fine for stores, but it scatters a
 // row of W over all threads, so every row would end in a CTA-wide reduction.  Here a warp owns a contiguous BLOCK of
@@ -320,6 +321,59 @@ __global__ void __launch_bounds__(256) k_matvec_reduce(ProductCfg m) {
 template <int FMT, int XDT, int NT>
 __global__ void __launch_bounds__(kSyncThreads, 3) k_matvec_fp8(ProductCfg m) {
   product_streams<1>(m, MatvecEp<XDT, NT, FMT>{m});
+}
+
+// ---- the dequantized fp8 weight (k_dequant_fp8) ---------------------------------------------------------------------
+// out[o][i] = ODT(float(W[o][i]) * S[o / bn][i / bk]), W and S as for k_matvec_fp8, out the contiguous bf16 / fp16
+// tensor [out][in] at m.y.  Bit for bit torch's (W.to(float32) * S_expanded).to(ODT): fp8 -> fp32 is exact, then one
+// fp32 multiply and one round to nearest even (fp16 overflow to +-inf); NaN stays NaN (its payload may differ).
+// The run's store loop with a different store: thread t takes the vectors t, t + 256, ... of the quarter plane, and
+// since out is contiguous a vector's element index is also its output index.  Only the scale lookup needs (row, col),
+// by multiply-highs (every element index is below 2^31: the host admits total <= INT32_MAX).  A lane converts its 16
+// bytes, multiplies each by the block's one scale (bk % 16 == 0, in % 16 == 0: the vector lies in one row and block)
+// and stores 32 bytes.
+template <int FMT, int ODT>
+struct DequantEp {
+  static_assert(ODT == kMvBf16 || ODT == kMvFp16, "bf16 or fp16 out");
+  static constexpr bool on = true;
+  ProductCfg m;
+
+  template <int G>
+  __device__ __forceinline__ void quarter(const SyncShared& S, uint64_t c, int stream, uint32_t out_off, uint32_t count, bool rot) const {
+    static_assert(G == 1, "fp8: one byte plane");
+    const uint64_t rin = matvec_fp8_recip(m.in);
+    const uint32_t in = (uint32_t)m.in, e0 = (uint32_t)(c * m.ce) + out_off;
+    for (uint32_t o = threadIdx.x * 16u; o < count; o += kSyncThreads * 16u) {
+      uint32_t r[4];
+      ZB_FUSED_VECTOR(G, S, out_off, o, rot, r);
+      const uint32_t e = e0 + o, row = matvec_fp8_div(e, rin), col = e - row * in;
+      const float sc = __ldg(m.scale + matvec_fp8_div(row, m.srow) * m.scols + matvec_fp8_div(col, m.scol));
+      uint32_t h[8];
+#pragma unroll
+      for (int half = 0; half < 2; half++) {
+        float w[8];
+        fp8_floats<FMT>(r[2 * half], r[2 * half + 1], w);
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+          if constexpr (ODT == kMvBf16) {
+            const __nv_bfloat162 v = __floats2bfloat162_rn(w[2 * i] * sc, w[2 * i + 1] * sc);
+            h[4 * half + i] = *reinterpret_cast<const uint32_t*>(&v);
+          } else {
+            const __half2 v = __floats2half2_rn(w[2 * i] * sc, w[2 * i + 1] * sc);
+            h[4 * half + i] = *reinterpret_cast<const uint32_t*>(&v);
+          }
+        }
+      }
+      uint4* const dst = reinterpret_cast<uint4*>(m.y) + (e >> 3);
+      dst[0] = make_uint4(h[0], h[1], h[2], h[3]);
+      dst[1] = make_uint4(h[4], h[5], h[6], h[7]);
+    }
+  }
+};
+
+template <int FMT, int ODT>
+__global__ void __launch_bounds__(kSyncThreads, 3) k_dequant_fp8(ProductCfg m) {
+  product_streams<1>(m, DequantEp<FMT, ODT>{m});
 }
 
 }  // namespace zb

@@ -1582,12 +1582,24 @@ int product_scratch_size(ProductKind kind, const zipnn_b200_decode_plan* plan, i
   return ZIPNN_B200_OK;
 }
 
-// The fp8 matvec's weight format and scale grid (zipnn_b200_decode_plan_matvec_fp8 has checked all but the pointer).
+// The weight format and scale grid of the fp8 matvec and dequantize (fp8_args_ok has checked all but the pointer).
 struct Fp8Scale {
   int format;
   const float* d_scale;
   size_t block_rows, block_cols;
 };
+bool fp8_args_ok(const Fp8Scale& f8) {
+  return (f8.format == kFp8E4m3 || f8.format == kFp8E5m2) && f8.block_rows && f8.block_cols >= 16 && f8.block_cols % 16 == 0;
+}
+// ProductCfg's scale-grid fields.
+void fp8_grid(const Fp8Scale& f8, ProductCfg& m) {
+  // a block at least as tall or wide as the matrix is the whole of it: clamped, bn and bk stay below 2^31
+  const uint64_t bn = std::min<uint64_t>(f8.block_rows, m.out), bk = std::min<uint64_t>(f8.block_cols, m.in);
+  m.scale = f8.d_scale;
+  m.srow = matvec_fp8_recip(bn);
+  m.scol = matvec_fp8_recip(bk);
+  m.scols = (uint32_t)((m.in + bk - 1) / bk);
+}
 
 int product(ProductKind kind, const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, const void* d_x, size_t x_stride,
             size_t n_tokens, const void* d_bias, void* d_y, size_t y_stride, void* d_scratch, size_t scratch_bytes, cudaStream_t st,
@@ -1613,18 +1625,35 @@ int product(ProductKind kind, const zipnn_b200_decode_plan* plan, int item, int 
   m.xs = x_stride;
   m.ys = y_stride;
   m.nt = (uint32_t)n_tokens;
-  if (f8) {
-    // a block at least as tall or wide as the matrix is the whole of it: clamped, bn and bk stay below 2^31
-    const uint64_t bn = std::min<uint64_t>(f8->block_rows, m.out), bk = std::min<uint64_t>(f8->block_cols, m.in);
-    m.scale = f8->d_scale;
-    m.srow = matvec_fp8_recip(bn);
-    m.scol = matvec_fp8_recip(bk);
-    m.scols = (uint32_t)((m.in + bk - 1) / bk);
-  }
+  if (f8) fp8_grid(*f8, m);
   const int fmt = f8 ? f8->format : kFp8E4m3;
   if (dtype == kMvBf16) return product_launch(product_kernels<kMvBf16>(kind, fmt, m.nt), m, st);
   if (dtype == kMvFp16) return product_launch(product_kernels<kMvFp16>(kind, fmt, m.nt), m, st);
   return product_launch(product_kernels<kMvFp32>(kind, fmt, m.nt), m, st);
+}
+
+// The fp8 dequantize: the fp8 matvec's item checks and scale grid, k_dequant_fp8, then the decode error folded into the
+// plan's error word as after a run (k_batch_errors).  No scratch, no host read after the first call for an item.
+int dequant_fp8(const zipnn_b200_decode_plan* plan, int item, const Fp8Scale& f8, int out_dtype, size_t in_features, void* d_out,
+                cudaStream_t st) {
+  ProductCfg m;
+  {
+    const int rc = product_item(kMatvecFp8, plan, item, out_dtype, in_features, st, m);
+    if (rc) return rc;
+  }
+  if (!d_out || ((uintptr_t)d_out & 15) || !f8.d_scale || ((uintptr_t)f8.d_scale & 3)) return ZIPNN_B200_E_ARG;
+  PlanState s;
+  plan_state(plan, s);  // (product_item has checked it)
+  m.y = d_out;
+  fp8_grid(f8, m);
+  const bool e4 = f8.format == kFp8E4m3;
+  const ProductKernel k = out_dtype == kMvBf16 ? (e4 ? &k_dequant_fp8<kFp8E4m3, kMvBf16> : &k_dequant_fp8<kFp8E5m2, kMvBf16>)
+                                               : (e4 ? &k_dequant_fp8<kFp8E4m3, kMvFp16> : &k_dequant_fp8<kFp8E5m2, kMvFp16>);
+  const unsigned blocks = resident_grid(k, kSyncSmemBytes, kSyncThreads, 4 * m.K);
+  if (!blocks) return ZIPNN_B200_E_CUDA;
+  k<<<blocks, kSyncThreads, kSyncSmemBytes, st>>>(m);
+  ZB_LAUNCHED();
+  return batch_errors(s.B, st);
 }
 }  // namespace
 
@@ -1666,10 +1695,17 @@ int zipnn_b200_decode_plan_matvec_fp8(const zipnn_b200_decode_plan* plan, int it
                                       const void* d_x, size_t x_stride, size_t n_tokens, const float* d_scale, size_t block_rows,
                                       size_t block_cols, const void* d_bias, void* d_y, size_t y_stride, void* d_scratch,
                                       size_t scratch_bytes, void* cuda_stream) {
-  if ((fp8_format != kFp8E4m3 && fp8_format != kFp8E5m2) || block_rows == 0 || block_cols < 16 || block_cols % 16) return ZIPNN_B200_E_ARG;
   const Fp8Scale f8{fp8_format, d_scale, block_rows, block_cols};
+  if (!fp8_args_ok(f8)) return ZIPNN_B200_E_ARG;
   return product(kMatvecFp8, plan, item, x_dtype, in_features, d_x, x_stride, n_tokens, d_bias, d_y, y_stride, d_scratch, scratch_bytes,
                  (cudaStream_t)cuda_stream, &f8);
+}
+
+int zipnn_b200_decode_plan_dequant_fp8(const zipnn_b200_decode_plan* plan, int item, int fp8_format, int out_dtype, size_t in_features,
+                                       const float* d_scale, size_t block_rows, size_t block_cols, void* d_out, void* cuda_stream) {
+  const Fp8Scale f8{fp8_format, d_scale, block_rows, block_cols};
+  if (!fp8_args_ok(f8)) return ZIPNN_B200_E_ARG;
+  return dequant_fp8(plan, item, f8, out_dtype, in_features, d_out, (cudaStream_t)cuda_stream);
 }
 
 int zipnn_b200_split(const void* d_in, size_t n, int num_buf, int bits_mode, void* d_planes, size_t stride,

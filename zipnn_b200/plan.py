@@ -464,24 +464,56 @@ class DecodePlan:
         -> out.  ValueError for an output `matvec_fp8_ok` refuses.  Works without the plan's output buffer."""
         return self._product(_MATVEC_FP8, k, x, bias, out, scratch, scale=scale, block=block)
 
-    def _fp8_grid(self, x, scale, block, out_features: int) -> tuple:
-        """-> (bn, bk) after checking `scale` against the grid the block implies."""
-        in_features = x.shape[-1]
+    def _fp8_grid(self, name: str, in_features: int, scale, block, out_features: int) -> tuple:
+        """-> (bn, bk) after checking `scale` against the grid the block implies (for method `name`)."""
         if not (isinstance(scale, torch.Tensor) and scale.is_cuda and scale.device == self.device and scale.dtype == torch.float32
                 and scale.is_contiguous()):
-            raise ValueError("matvec_fp8's scale must be a contiguous CUDA float32 tensor on the plan's device")
+            raise ValueError(f"{name}'s scale must be a contiguous CUDA float32 tensor on the plan's device")
         if block is None:
             if scale.numel() != 1:
-                raise ValueError(f"matvec_fp8 takes block=None for a one-element scale only, not {scale.numel()} elements")
+                raise ValueError(f"{name} takes block=None for a one-element scale only, not {scale.numel()} elements")
             return out_features, in_features
         bn, bk = (int(b) for b in block)
         if bn < 1 or bk < 16 or bk % 16:
-            raise ValueError(f"matvec_fp8's block (bn, bk) needs bn >= 1 and bk a multiple of 16 of at least 16, not {(bn, bk)}")
+            raise ValueError(f"{name}'s block (bn, bk) needs bn >= 1 and bk a multiple of 16 of at least 16, not {(bn, bk)}")
         grid = -(-out_features // bn) * -(-in_features // bk)
         if scale.numel() != grid:
-            raise ValueError(f"matvec_fp8's scale for block {(bn, bk)} of a [{out_features}, {in_features}] weight has {grid} "
+            raise ValueError(f"{name}'s scale for block {(bn, bk)} of a [{out_features}, {in_features}] weight has {grid} "
                              f"elements, not {scale.numel()}")
         return bn, bk
+
+    def dequant_fp8(self, k: int, in_features: int, scale: torch.Tensor, block: tuple = None, dtype: torch.dtype = torch.bfloat16,
+                    out: torch.Tensor = None) -> torch.Tensor:
+        """The dequantized weight S * W as a [out_features, in_features] tensor of `dtype` (bf16 or fp16), W = output `k`
+        (an fp8 tensor that `matvec_fp8_ok(k, in_features)` accepts) and S its fp32 scale grid, written straight from the
+        coded streams: the fp8 bytes are neither written nor read dense (zipnn_b200_decode_plan_dequant_fp8).  Bit for bit
+        torch's `(W.to(torch.float32) * S_expanded).to(dtype)`: one fp32 product per element and one rounding to nearest
+        even (fp16 overflow gives +-inf); NaN stays NaN, its payload may differ.  Two launches on the current CUDA stream,
+        no scratch, no host read: capturable in a CUDA graph and replayable with a new scale.
+
+        scale, block: as for `matvec_fp8`.
+        out:     optional contiguous tensor of shape (out_features, in_features) and `dtype` on the plan's device, 16-byte
+                 aligned; exactly its elements are written.
+        -> out.  ValueError for an output `matvec_fp8_ok` refuses, and for a bad scale, block, dtype or out.  Works
+        without the plan's output buffer.  A decode error surfaces through `check()`."""
+        if dtype not in _MATMUL_DTYPES:
+            raise ValueError(f"dequant_fp8 writes bf16 or fp16, not {dtype}")
+        if not self._ok(_MATVEC_FP8, k, in_features):
+            raise ValueError(f"dequant_fp8 cannot dequantize output {k} with in_features {in_features} (see matvec_fp8_ok)")
+        wdt, total = self._product_item(k)
+        shape = (total // in_features, in_features)
+        bn, bk = self._fp8_grid("dequant_fp8", in_features, scale, block, shape[0])
+        if out is None:
+            out = torch.empty(shape, dtype=dtype, device=self.device)
+        elif not (isinstance(out, torch.Tensor) and out.is_cuda and out.device == self.device and out.dtype == dtype
+                  and tuple(out.shape) == shape and out.is_contiguous() and out.data_ptr() % 16 == 0):
+            raise ValueError(f"dequant_fp8's out must be a contiguous 16-byte aligned {dtype} CUDA tensor of shape {shape} on the plan's device")
+        rc = _native.lib().zipnn_b200_decode_plan_dequant_fp8(self._ref, k, _FP8_FORMATS[wdt], _MATVEC_DTYPES[dtype], in_features,
+                                                              scale.data_ptr(), bn, bk, out.data_ptr(),
+                                                              torch.cuda.current_stream(self.device).cuda_stream)
+        if rc:
+            _native.check(rc)
+        return out
 
     def _product(self, kind: _Product, k: int, x, bias, out, scratch, scale=None, block=None) -> torch.Tensor:
         """matvec, matmul and matvec_fp8: the checks and the call."""
@@ -499,7 +531,7 @@ class DecodePlan:
             raise ValueError(f"{name} cannot multiply by output {k} with in_features {in_features} (see {name}_ok)")
         out_features = total // in_features
         if kind.scaled:
-            bn, bk = self._fp8_grid(x, scale, block, out_features)
+            bn, bk = self._fp8_grid(name, in_features, scale, block, out_features)
         es = x.element_size()
         x2 = x.reshape(max(n, 1), in_features) if n else x.reshape(0, in_features)
         if n and (x2.stride(1) != 1 or x2.data_ptr() % 16 or (n > 1 and (x2.stride(0) * es) % 16)):

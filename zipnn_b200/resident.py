@@ -28,6 +28,9 @@ Rules:
     before for larger inputs; its bias stays a dense parameter;
   * with `matmul=N` such a Linear with a bf16 / fp16 weight multiplies inputs of more rows than the matvec takes and
     at most N on tensor cores (`DecodePlan.matmul`), again without a dense weight;
+  * with `fp8=True` a selected fp8 linear layer (`fp8_linears`: transformers' `FP8Linear`) keeps its scales and bias
+    dense and runs W8A16 from its stream at any number of rows: `DecodePlan.matvec_fp8` for at most `matvec` rows,
+    `DecodePlan.dequant_fp8` + F.linear for more; it needs no downloaded kernel;
   * with `experts=True` the experts module of a mixture-of-experts layer (`experts_module`: 3D weights [E, ...] called
     as experts(hidden_states, top_k_index, top_k_weights)) decodes only the slices [e] of the experts its router
     picked (`DecodePlan.run_select`); its own forward then runs unchanged and reads only those slices;
@@ -44,6 +47,7 @@ import os
 import traceback
 
 import torch
+import torch.nn.functional as F
 
 from . import prefetch as _prefetch
 from .plan import _HEAD, MATMUL_MAX_TOKENS, MATVEC_MAX_TOKENS, DecodePlan, _Stream
@@ -52,6 +56,7 @@ from .util_safetensors import COMPRESSION_METHOD
 from .zipnn import DecodePipe, ZipNN
 
 _DTYPES = (torch.bfloat16, torch.float16, torch.float32, torch.float8_e4m3fn, torch.float8_e5m2)
+_FP8 = (torch.float8_e4m3fn, torch.float8_e5m2)
 _ATTR = "_zipnn_resident"
 
 
@@ -119,6 +124,9 @@ class _Resident:
         self.matmul_scratch_bytes = 0  # what the largest matmul needs of it
         self.experts = set()  # experts=True: id() of the `entries` modules that decode only their routed experts
         self.select_scratch = None  # the experts modules' run_select scratch, sized for the largest
+        self.fp8s = []        # fp8=True: (fp8 linear module, plan, index into the plan's outputs, matvec_fp8 / dequant_fp8 take it?)
+        self.fp8_scratch = None  # the fp8 modules' matvec_fp8 scratch: the plans' one when it is large enough
+        self.fp8_scratch_bytes = 0  # what the largest of them needs of it
 
 
 def _pre_hook(plan, names):
@@ -201,12 +209,44 @@ def _check_experts(experts: bool, prefetch: bool) -> bool:
     return bool(experts)
 
 
-def dense_biases(groups, matvec: int) -> list:
-    """`select`'s groups without the biases that stay dense under matvec=N: those owned by `matvecs` modules only (the
-    matvec adds them after the sum, so they must not need a decode)."""
-    if not matvec:
+def fp8_linears(module: torch.nn.Module) -> bool:
+    """Does `fp8=True` run `module` from its compressed fp8 weight?  A torch.nn.Linear (or subclass) with a 2-D
+    float8_e4m3fn / float8_e5m2 `weight`, an fp32 `weight_scale_inv` and a `block_size` that is None (a one-element
+    scale) or (bn, bk) with the grid's shape [ceil(out / bn), ceil(in / bk)]: transformers' `FP8Linear`, found by these
+    attributes."""
+    w, scale = getattr(module, "weight", None), getattr(module, "weight_scale_inv", None)
+    if not (isinstance(module, torch.nn.Linear) and isinstance(w, torch.Tensor) and w.dim() == 2 and w.dtype in _FP8
+            and isinstance(scale, torch.Tensor) and scale.dtype == torch.float32 and hasattr(module, "block_size")):
+        return False
+    block = module.block_size
+    if block is None:
+        return scale.numel() == 1
+    if not (isinstance(block, (tuple, list)) and len(block) == 2 and all(isinstance(b, int) and b >= 1 for b in block)):
+        return False
+    return tuple(scale.shape) == (-(-w.shape[0] // block[0]), -(-w.shape[1] // block[1]))
+
+
+def dequantize_fp8(weight: torch.Tensor, scale: torch.Tensor, block, dtype: torch.dtype) -> torch.Tensor:
+    """torch's dequantize of an fp8 weight [out, in]: (W.to(float32) * S_expanded).to(dtype), S expanded over its
+    (bn, bk) blocks (block None: one scale for the tensor).  `DecodePlan.dequant_fp8` gives the same bits."""
+    w = weight.to(torch.float32)
+    if block is None:
+        return (w * scale.reshape(())).to(dtype)
+    (out, inn), (bn, bk) = weight.shape, block
+    s = scale.reshape(-(-out // bn), -(-inn // bk)).repeat_interleave(bn, 0)[:out].repeat_interleave(bk, 1)[:, :inn]
+    return (w * s).to(dtype)
+
+
+def dense_biases(groups, matvec: int, fp8: bool = False) -> list:
+    """`select`'s groups without the parameters that stay dense: under matvec=N the biases owned by `matvecs` modules
+    only (the matvec adds them after the sum, so they must not need a decode); under fp8=True every parameter but the
+    weight of `fp8_linears` modules (scales, bias, activation scale: the products read them as they are)."""
+    if not (matvec or fp8):
         return groups
-    return [(p, owners) for p, owners in groups if not all(n == "bias" and matvecs(o) for o, n in owners)]
+
+    def dense(o, n):
+        return (matvec and n == "bias" and matvecs(o)) or (fp8 and n != "weight" and fp8_linears(o))
+    return [(p, owners) for p, owners in groups if not all(dense(o, n) for o, n in owners)]
 
 
 def _check_matvec(matvec: int, prefetch: bool, name: str = "matvec", limit: int = MATVEC_MAX_TOKENS) -> int:
@@ -219,6 +259,54 @@ def _check_matvec(matvec: int, prefetch: bool, name: str = "matvec", limit: int 
 
 def _check_matmul(matmul: int, prefetch: bool) -> int:
     return _check_matvec(matmul, prefetch, "matmul", MATMUL_MAX_TOKENS)
+
+
+def _check_fp8(fp8: bool, prefetch: bool) -> bool:
+    if fp8 and prefetch:
+        raise ValueError("fp8=True and prefetch=True do not combine yet: the prefetch schedule decodes every module")
+    return bool(fp8)
+
+
+def _fp8_block(mod) -> tuple:
+    return None if mod.block_size is None else tuple(mod.block_size)
+
+
+def _fp8_forward(mod, state, plan, k, names, fast: bool):
+    """The forward of an fp8 linear module (W8A16: the activations are not quantized).  A bf16 / fp16 input on the plan's
+    device, outside autocast, is multiplied with the dequantized weight S * W: at most `state.matvec` rows by
+    `plan.matvec_fp8`, more by `plan.dequant_fp8` into the shared output buffer and F.linear; the bias is added as
+    FP8Linear.forward adds it.  A module whose weight `fast` is False for (`matvec_fp8_ok` refuses it) decodes it and
+    dequantizes in torch into a fresh tensor instead (the fp8 bytes occupy the shared buffer), with the same result.
+    Any other input takes the decode, bind, module's own forward, unbind of the other compressed modules."""
+    pre, post = _pre_hook(plan, names), _unbind(names)
+    block = _fp8_block(mod)
+    shape = tuple(plan.outputs[k].shape)
+    nbytes = 2 * shape[0] * shape[1]
+
+    def forward(input):
+        if (input.dtype in (torch.bfloat16, torch.float16) and input.device == plan.device
+                and not torch.is_autocast_enabled(plan.device.type)):
+            if torch.is_grad_enabled():
+                raise RuntimeError(f"{type(mod).__name__} holds compressed weights and runs only under torch.no_grad() or "
+                                   "torch.inference_mode()")
+            width = input.shape[-1] if input.dim() else 0
+            rows = input.numel() // width if width else None
+            scale = mod.weight_scale_inv
+            if fast and rows is not None and rows <= state.matvec:
+                y = plan.matvec_fp8(k, input, scale, block, scratch=state.fp8_scratch)
+            else:
+                if fast:
+                    w = plan.dequant_fp8(k, shape[1], scale, block, input.dtype, out=plan._out[:nbytes].view(input.dtype).view(shape))
+                else:
+                    w = dequantize_fp8(plan.run()[k], scale, block, input.dtype)
+                y = F.linear(input, w)
+            return y if mod.bias is None else (y + mod.bias).to(input.dtype)
+        pre(mod, (input,))
+        try:
+            return type(mod).forward(mod, input)
+        finally:
+            post(mod, (input,), None)
+    return forward
 
 
 def _matvec_forward(mod, state, plan, k, names, dtype, device, matmul: int = 0):
@@ -289,7 +377,7 @@ def _pack(streams: dict, dev) -> tuple:
 
 
 def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: bool = False, matvec: int = 0,
-                    matmul: int = 0, experts: bool = False) -> tuple:
+                    matmul: int = 0, experts: bool = False, fp8: bool = False) -> tuple:
     """The back half of compress_module and load_module: streams {group index: CUDA stream} -> per selected module
     one DecodePlan over its parameters' streams, all sharing one output and one scratch buffer.  Raises like
     `decompress` on a corrupt stream; nothing outside is touched until `_commit`.  -> (_Resident, report).
@@ -301,7 +389,9 @@ def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: 
     matvec=N: a `matvecs` module whose one compressed parameter is a weight that `DecodePlan.matvec_ok` accepts is
     listed in `state.matvecs`; its plan and its room in the shared output buffer stay (larger inputs decode).
     matmul=N: the same for `DecodePlan.matmul_ok`; such a module is also in `state.matmuls`.
-    experts=True: an `experts_module` whose plan passes `DecodePlan.select_ok` is in `state.experts`."""
+    experts=True: an `experts_module` whose plan passes `DecodePlan.select_ok` is in `state.experts`.
+    fp8=True: an `fp8_linears` module whose one compressed parameter is its weight is in `state.fp8s`; the shared output
+    buffer holds at least twice its weight's bytes (its dequantized weight)."""
     where = {id(groups[i][0]): i for i in streams}
     per_module = []
     for m in modules:
@@ -311,7 +401,9 @@ def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: 
     whole, looked, own = split_gathers(per_module, gather)
     sizes = [DecodePlan.sizes([streams[i] for _, i in names]) for _, names in whole]
     own_sizes = [DecodePlan.sizes([streams[i]]) for i in own]
-    out = None if own else torch.empty(max([s[0] for s in sizes] + [1]), dtype=torch.uint8, device=dev)
+    fp8_mods = {id(m) for m, names in whole if fp8 and fp8_linears(m) and [n for n, _ in names] == ["weight"]}
+    out_need = max([s[0] for s in sizes] + [2 * m.weight.numel() for m, _ in whole if id(m) in fp8_mods] + [1])
+    out = None if own else torch.empty(out_need, dtype=torch.uint8, device=dev)
     scratch = torch.empty(max([s[1] for s in sizes + own_sizes] + [1]), dtype=torch.uint8, device=dev)
     state = _Resident()
     state.streams = buffers
@@ -327,7 +419,7 @@ def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: 
         state.gather_plan_bytes += plan.nbytes["plan"]
         index_bytes += plan.nbytes["index"]
     if out is None:
-        out = torch.empty(max([s[0] for s in sizes] + [1]), dtype=torch.uint8, device=dev)
+        out = torch.empty(out_need, dtype=torch.uint8, device=dev)
     for m, names in whole:
         plan = DecodePlan([streams[i] for _, i in names], out=out, scratch=scratch)
         plan_bytes += plan.nbytes["plan"]
@@ -343,6 +435,10 @@ def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: 
                 state.matmuls.add(id(m))
         if experts and experts_module(m, [n for n, _ in names]) and plan.select_ok():
             state.experts.add(id(m))
+        if id(m) in fp8_mods:
+            block = _fp8_block(m)
+            fast = plan.matvec_fp8_ok(0, m.in_features) and (block is None or block[1] % 16 == 0)
+            state.fp8s.append((m, plan, 0, fast))
     state.matvec, state.matmul = matvec, matmul
     for m, i in looked:
         plan, k = by_stream[i]
@@ -392,11 +488,21 @@ def _commit(module: torch.nn.Module, state: _Resident, prefetch: bool = False) -
     if state.experts:
         need = max(plan.select_scratch_bytes() for m, plan, _, _ in state.entries if id(m) in state.experts)
         state.select_scratch = torch.empty(need, dtype=torch.uint8, device=state.scratch.device)
+    if state.matvec and any(fast for _, _, _, fast in state.fp8s):
+        need = max(plan.matvec_fp8_scratch_bytes(k, m.in_features, state.matvec) for m, plan, k, fast in state.fp8s if fast)
+        state.fp8_scratch_bytes = need
+        state.fp8_scratch = state.scratch if need <= state.scratch.numel() else torch.empty(need, dtype=torch.uint8,
+                                                                                             device=state.scratch.device)
     by_matvec = {id(m): (plan, k) for m, plan, k in state.matvecs}
+    by_fp8 = {id(m): (k, fast) for m, _, k, fast in state.fp8s}
     for key, (m, plan, local, hooks) in enumerate(state.entries):
         if id(m) in by_matvec:   # no hooks: its forward decides per input whether anything is decoded
             m.__dict__["forward"] = _matvec_forward(m, state, plan, by_matvec[id(m)][1], local, plan.outputs[by_matvec[id(m)][1]].dtype,
                                                     plan.device, state.matmul if id(m) in state.matmuls else 0)
+            continue
+        if id(m) in by_fp8:   # no hooks either: its forward multiplies from the stream, or decodes
+            k, fast = by_fp8[id(m)]
+            m.__dict__["forward"] = _fp8_forward(m, state, plan, k, local, fast)
             continue
         if id(m) in state.experts:
             hooks.append(m.register_forward_pre_hook(_pre_hook_experts(plan, local, state), with_kwargs=True))
@@ -416,7 +522,7 @@ def _commit(module: torch.nn.Module, state: _Resident, prefetch: bool = False) -
 
 
 def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = False, gather: bool = False, matvec: int = 0,
-                    matmul: int = 0, experts: bool = False) -> dict:
+                    matmul: int = 0, experts: bool = False, fp8: bool = False) -> dict:
     """Compress the weights of `modules` (default: every submodule that directly owns bf16 / fp16 / fp32 / fp8
     parameters) into streams kept in HBM, decoded just before each module's forward.  All parameters are compressed
     in one `compress_batch` call and must be on one CUDA device.
@@ -464,14 +570,28 @@ def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = Fals
     only the slices [e] of the routed experts, so its outputs equal the dense module's bit for bit, whichever experts
     implementation it uses; the other slices of the shared buffer hold stale bytes.  The report gains
     "experts_modules" and "experts_scratch_bytes" (one run_select scratch shared by them all, sized for the largest).
-    ValueError together with prefetch=True."""
+    ValueError together with prefetch=True.
+
+    fp8=True (default False, which changes nothing): the W8A16 reading of fp8 checkpoints.  A selected `fp8_linears`
+    module (transformers' `FP8Linear`) compresses only its weight; `weight_scale_inv`, `bias` and `activation_scale`
+    stay dense parameters.  Its forward multiplies bf16 / fp16 inputs on the weight's device, outside autocast, with the
+    dequantized weight S * W in the input's dtype -- it does not quantize the activations, so it is not FP8Linear's own
+    W8A8 forward, and it needs no downloaded kernel: inputs of at most `matvec` rows go to `DecodePlan.matvec_fp8`
+    (fp32 sums rounded once), larger ones to `DecodePlan.dequant_fp8` into the shared output buffer and F.linear (bit for
+    bit F.linear of torch's dequantize), then the bias is added as FP8Linear adds it.  So fp8=True, matvec=8 is the
+    decode-time setting.  A weight that `DecodePlan.matvec_fp8_ok` refuses (a constant one, say) is decoded and
+    dequantized in torch instead, with the same result.  Other inputs decode and run the module's own forward.  The
+    shared output buffer holds at least twice the largest such weight's bytes.  `matmul` does not apply to fp8 weights.
+    The report gains "fp8_modules" and "fp8_scratch_bytes" (the matvec_fp8 scratch, the plans' one when it is large
+    enough).  ValueError together with prefetch=True."""
     matvec = _check_matvec(matvec, prefetch)
     matmul = _check_matmul(matmul, prefetch)
     experts = _check_experts(experts, prefetch)
+    fp8 = _check_fp8(fp8, prefetch)
     if getattr(module, _ATTR, None) is not None:
         raise ValueError("compress_module: this module is already compressed")
     modules, groups = select(module, modules)
-    groups = dense_biases(groups, max(matvec, matmul))
+    groups = dense_biases(groups, max(matvec, matmul), fp8)
     params = [p for p, _ in groups]
     if not params:
         setattr(module, _ATTR, None)
@@ -484,13 +604,13 @@ def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = Fals
     # the streams move into one tight buffer; the batch's output buffer (sized by the bound) is dropped
     buf, streams = _pack({i: s for i, (p, s) in enumerate(zip(params, coded)) if s.numel() < p.numel() * p.element_size()}, dev)
     del coded, params
-    state, report = _resident_state(modules, groups, streams, [buf], dev, gather, matvec, matmul, experts)
+    state, report = _resident_state(modules, groups, streams, [buf], dev, gather, matvec, matmul, experts, fp8)
     _commit(module, state, prefetch)
-    return _with_prefetch(report, state, prefetch, gather, matvec, matmul, experts)
+    return _with_prefetch(report, state, prefetch, gather, matvec, matmul, experts, fp8)
 
 
 def _with_prefetch(report: dict, state, prefetch: bool, gather: bool = False, matvec: int = 0, matmul: int = 0,
-                   experts: bool = False) -> dict:
+                   experts: bool = False, fp8: bool = False) -> dict:
     if prefetch:
         report = dict(report, prefetch_out_bytes=state.prefetch[1].numel() if state is not None and state.prefetch else 0)
     if gather:
@@ -506,6 +626,9 @@ def _with_prefetch(report: dict, state, prefetch: bool, gather: bool = False, ma
     if experts:
         report = dict(report, experts_modules=len(state.experts) if state is not None else 0,
                       experts_scratch_bytes=state.select_scratch.numel() if state is not None and state.select_scratch is not None else 0)
+    if fp8:
+        report = dict(report, fp8_modules=len(state.fp8s) if state is not None else 0,
+                      fp8_scratch_bytes=state.fp8_scratch_bytes if state is not None else 0)
     return report
 
 
@@ -531,6 +654,8 @@ def decompress_module(module: torch.nn.Module) -> None:
     for m, _, _, _ in state.gathers:
         m.__dict__.pop("forward", None)
     for m, _, _ in state.matvecs:
+        m.__dict__.pop("forward", None)
+    for m, _, _, _ in state.fp8s:
         m.__dict__.pop("forward", None)
     # each module's plan decodes into the shared buffer once more; its parameters are copied out of it, so the
     # model needs its dense size plus that buffer, not twice its dense size
@@ -564,6 +689,7 @@ def decompress_module(module: torch.nn.Module) -> None:
     state.entries.clear()
     state.gathers.clear()
     state.matvecs.clear()
+    state.fp8s.clear()
     state.matmuls.clear()
     state.experts.clear()
     delattr(module, _ATTR)
@@ -639,7 +765,7 @@ def _files(filenames) -> list:
     return [os.fspath(f) for f in filenames]
 
 
-def plan_load(module: torch.nn.Module, filenames, modules=None, matvec: int = 0) -> LoadPlan:
+def plan_load(module: torch.nn.Module, filenames, modules=None, matvec: int = 0, fp8: bool = False) -> LoadPlan:
     """The checks and choices of `load_module`, from the files' headers: ValueError naming the keys for a missing or
     unexpected key, a dtype or shape that differs, a non-persistent buffer on the meta device, and for a module that
     is already compressed."""
@@ -647,7 +773,7 @@ def plan_load(module: torch.nn.Module, filenames, modules=None, matvec: int = 0)
         raise ValueError("load_module: this module is already compressed")
     found = file_entries(_files(filenames))
     modules, groups = select(module, modules)
-    groups = dense_biases(groups, matvec)   # (matvec=N: those biases are read to dense tensors)
+    groups = dense_biases(groups, matvec, fp8)   # (matvec=N, fp8=True: the parameters that stay dense are read so)
     plan = LoadPlan(modules, groups)
     group_of = {id(p): gi for gi, (p, _) in enumerate(groups)}
     by_key = {}
@@ -705,7 +831,8 @@ def plan_load(module: torch.nn.Module, filenames, modules=None, matvec: int = 0)
     return plan
 
 
-def _load_device(plan: LoadPlan, dev, gather: bool = False, matvec: int = 0, matmul: int = 0, experts: bool = False) -> tuple:
+def _load_device(plan: LoadPlan, dev, gather: bool = False, matvec: int = 0, matmul: int = 0, experts: bool = False,
+                 fp8: bool = False) -> tuple:
     """Every device step of load_module; the module is not touched.  -> (_Resident or None, report, dense tensors of
     plan.dense, {group index: dense tensor} of plain entries that did not compress, moved buffers of plan.moves)."""
     pipe = DecodePipe(dev)
@@ -776,7 +903,7 @@ def _load_device(plan: LoadPlan, dev, gather: bool = False, matvec: int = 0, mat
             moved = [m._buffers[n].to(dev) for m, n in plan.moves]
             if plan.groups:
                 state, report = _resident_state(plan.modules, plan.groups, dict(sorted(streams.items())), buffers, dev, gather, matvec,
-                                                matmul, experts)
+                                                matmul, experts, fp8)
             else:
                 state, report = None, dict(_EMPTY_REPORT)
         return state, report, dense, stayed, moved
@@ -787,7 +914,7 @@ def _load_device(plan: LoadPlan, dev, gather: bool = False, matvec: int = 0, mat
 
 
 def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None, prefetch: bool = False,
-                gather: bool = False, matvec: int = 0, matmul: int = 0, experts: bool = False) -> dict:
+                gather: bool = False, matvec: int = 0, matmul: int = 0, experts: bool = False, fp8: bool = False) -> dict:
     """Load a checkpoint into `module` with the weights of `modules` kept compressed on `device`: the state
     `compress_module` leaves (same selection rules, hooks, plans and report), reached without a dense copy of those
     weights on the GPU.
@@ -822,20 +949,21 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None,
     and the batched decode's workspace; plain entries add one group at a time: its input, its streams' bound and the
     compress workspace.  A model loaded from .znn files never has its compressed weights dense on the device.
 
-    prefetch, gather, matvec, matmul, experts: as for `compress_module`.
+    prefetch, gather, matvec, matmul, experts, fp8: as for `compress_module`.
 
     -> the report of `compress_module`."""
     matvec = _check_matvec(matvec, prefetch)
     matmul = _check_matmul(matmul, prefetch)
     experts = _check_experts(experts, prefetch)
+    fp8 = _check_fp8(fp8, prefetch)
     dev = _cuda_device(device)
     if dev is None:
         raise ValueError(f"load_module: {device!r} is not a CUDA device")
     if dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
-    plan = plan_load(module, filenames, modules, max(matvec, matmul))
+    plan = plan_load(module, filenames, modules, max(matvec, matmul), fp8)
     try:
-        state, report, dense, stayed, moved = _load_device(plan, dev, gather, matvec, matmul, experts)
+        state, report, dense, stayed, moved = _load_device(plan, dev, gather, matvec, matmul, experts, fp8)
     except BaseException as e:
         traceback.clear_frames(e.__traceback__)   # the frames' locals would keep the call's device memory alive
         raise
@@ -857,7 +985,7 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None,
         setattr(module, _ATTR, None)
     else:
         _commit(module, state, prefetch)
-    return _with_prefetch(report, state, prefetch, gather, matvec, matmul, experts)
+    return _with_prefetch(report, state, prefetch, gather, matvec, matmul, experts, fp8)
 
 
 def save_module(module: torch.nn.Module, filename, metadata=None) -> None:
