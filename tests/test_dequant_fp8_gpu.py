@@ -375,7 +375,7 @@ def check_against_reference(m, ref, seed):
                 for (_, _, a), (_, _, b) in zip(got_rec, want_rec):
                     assert torch.equal(bits(a), bits(b)), rows
             else:   # matvec_fp8 within the bound; the fallback is the reference's forward on the same input
-                fast = {id(x): f for x, _, _, f in getattr(m, R._ATTR).fp8s}
+                fast = {id(x): mode == "fp8" for x, _, _, mode in getattr(m, R._ATTR).entries if mode in ("fp8", "fp8_torch")}
                 for mod, x, y in got_rec:
                     r = _ref_of(ref, m, mod)
                     if fast[id(mod)]:
@@ -414,7 +414,7 @@ def test_compress_module_fp8_against_the_reference():
     before = dense_state(m)
     report = compress_module(m, fp8=True, matvec=8)
     state = getattr(m, R._ATTR)
-    fast = {id(x): f for x, _, _, f in state.fp8s}
+    fast = {id(x): mode == "fp8" for x, _, _, mode in state.entries if mode in ("fp8", "fp8_torch")}
     down = m.model.layers[1].mlp.down_proj
     assert fast[id(down)] is False and sum(fast.values()) == 14, "the constant weight takes the fallback"
     assert report["out_bytes"] == 2 * 512 * 256   # (twice the largest fp8 weight; the bf16 embedding decodes to as many)

@@ -12,7 +12,7 @@ import pytest
 import torch
 
 import chunk_settings as CS
-from zipnn_b200.resident import _Resident, _with_prefetch, gathers, select, split_gathers
+from zipnn_b200.resident import _Entry, _Resident, _options, _with_prefetch, gathers, select, split_gathers
 
 
 def round_up(v, a):
@@ -164,8 +164,21 @@ def test_report_arithmetic():
     state.gathers = [object(), object()]
     state.gather_plan_bytes = 4096
     base = {"plan_bytes": 1}
-    assert _with_prefetch(base, state, False, False) == base
-    assert _with_prefetch(base, state, False, True) == dict(base, gather_modules=2, gather_bytes=4096)
+    assert _with_prefetch(base, state, _options()) == base
+    assert _with_prefetch(base, state, _options(gather=True)) == dict(base, gather_modules=2, gather_bytes=4096)
     state.gather_scratch = torch.empty(300, dtype=torch.uint8)   # a scratch of its own counts
-    assert _with_prefetch(base, state, False, True)["gather_bytes"] == 4096 + 300
-    assert _with_prefetch(base, None, False, True) == dict(base, gather_modules=0, gather_bytes=0)
+    assert _with_prefetch(base, state, _options(gather=True))["gather_bytes"] == 4096 + 300
+    assert _with_prefetch(base, None, _options(gather=True)) == dict(base, gather_modules=0, gather_bytes=0)
+
+
+def test_mode_report_counts():
+    """Each mode's module count comes from the entries' modes: a "matmul" module is also a matvec module, an fp8 module
+    counts whether its products take its weight or torch dequantizes it."""
+    state = _Resident()
+    state.entries = [_Entry(None, None, [], mode) for mode in ("matmul", "matvec", "fp8", "fp8_torch", "experts", "experts", "decode")]
+    state.select_scratch = torch.empty(7, dtype=torch.uint8)
+    state.matvec_scratch_bytes, state.matmul_scratch_bytes, state.fp8_scratch_bytes = 1, 2, 3
+    got = _with_prefetch({}, state, _options(matvec=8, matmul=64, experts=True, fp8=True))
+    assert got == {"matvec_modules": 2, "matvec_scratch_bytes": 1, "matmul_modules": 1, "matmul_scratch_bytes": 2,
+                   "experts_modules": 2, "experts_scratch_bytes": 7, "fp8_modules": 2, "fp8_scratch_bytes": 3}
+    assert _with_prefetch({}, None, _options(prefetch=True)) == {"prefetch_out_bytes": 0}

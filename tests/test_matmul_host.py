@@ -253,4 +253,5 @@ def test_prefetch_and_bad_counts_are_refused():
     for bad in (-1, R.MATMUL_MAX_TOKENS + 1, 1.5, "4"):
         with pytest.raises(ValueError, match="matmul"):
             R.compress_module(model, matmul=bad)
-    assert R._check_matmul(0, True) == 0 and R._check_matmul(R.MATMUL_MAX_TOKENS, False) == R.MATMUL_MAX_TOKENS
+    assert R._options(prefetch=True, matmul=0).matmul == 0
+    assert R._options(matmul=R.MATMUL_MAX_TOKENS).matmul == R.MATMUL_MAX_TOKENS

@@ -231,4 +231,5 @@ def test_prefetch_and_bad_counts_are_refused():
     for bad in (-1, R.MATVEC_MAX_TOKENS + 1, 1.5, "4"):
         with pytest.raises(ValueError, match="matvec"):
             R.compress_module(model, matvec=bad)
-    assert R._check_matvec(0, True) == 0 and R._check_matvec(R.MATVEC_MAX_TOKENS, False) == R.MATVEC_MAX_TOKENS
+    assert R._options(prefetch=True, matvec=0).matvec == 0
+    assert R._options(matvec=R.MATVEC_MAX_TOKENS).matvec == R.MATVEC_MAX_TOKENS

@@ -424,7 +424,8 @@ def test_transformers_moe_logits_are_exact(which):
     rep = compress_module(model, experts=True)
     # the experts modules, and the routers (weight [E, H], num_experts = E: they pass no ids, so they decode whole)
     experts = [m for m in model.modules() if type(m).__name__.endswith("Experts")]
-    assert len(experts) == cfg.num_hidden_layers and all(id(m) in getattr(model, _ATTR).experts for m in experts)
+    mode = {id(m): mode for m, _, _, mode in getattr(model, _ATTR).entries}
+    assert len(experts) == cfg.num_hidden_layers and all(mode.get(id(m)) == "experts" for m in experts)
     assert rep["experts_modules"] == 2 * cfg.num_hidden_layers
     for impl in impls:
         model.config._experts_implementation = impl

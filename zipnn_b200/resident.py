@@ -45,6 +45,7 @@ from __future__ import annotations
 
 import os
 import traceback
+from typing import NamedTuple
 
 import torch
 import torch.nn.functional as F
@@ -100,11 +101,45 @@ def select(module: torch.nn.Module, modules=None):
     return modules, groups
 
 
+class _Options(NamedTuple):
+    """The run modes of compress_module / load_module, as `_options` checked them."""
+    prefetch: bool
+    gather: bool
+    matvec: int    # the most input rows a matvec module multiplies without decoding (0: none)
+    matmul: int    # the most input rows a matmul module multiplies without decoding (0: none)
+    experts: bool
+    fp8: bool
+
+
+def _options(prefetch=False, gather=False, matvec=0, matmul=0, experts=False, fp8=False) -> _Options:
+    """ValueError for a row count out of range and for a mode that does not combine with prefetch=True."""
+    for name, n, limit in (("matvec", matvec, MATVEC_MAX_TOKENS), ("matmul", matmul, MATMUL_MAX_TOKENS)):
+        if not (isinstance(n, int) and 0 <= n <= limit):
+            raise ValueError(f"{name} must be an integer from 0 to {limit}, not {n!r}")
+        if n and prefetch:
+            raise ValueError(f"{name} and prefetch=True do not combine yet: the prefetch schedule decodes every module")
+    if experts and prefetch:
+        raise ValueError("experts=True and prefetch=True do not combine: the prefetch schedule decodes every module "
+                         "before its router has picked the experts")
+    if fp8 and prefetch:
+        raise ValueError("fp8=True and prefetch=True do not combine yet: the prefetch schedule decodes every module")
+    return _Options(bool(prefetch), bool(gather), matvec, matmul, bool(experts), bool(fp8))
+
+
+class _Entry(NamedTuple):
+    """A module decoded whole and how it runs, as `_resident_state` decided it."""
+    module: torch.nn.Module
+    plan: DecodePlan
+    names: list   # [(name, index into the plan's outputs)]
+    mode: str     # hooks: "decode", "prefetch", "experts"; a forward of its own: "matvec", "matmul", "fp8", "fp8_torch"
+
+
 class _Resident:
     """What compress_module leaves on the root module: per compressed module its plan and parameter names."""
 
     def __init__(self):
-        self.entries = []     # (module, plan, [(name, index into the plan's outputs)], [hook handles])
+        self.entries = []     # _Entry per module decoded whole
+        self.hooks = []       # the entries' hook handles
         self.params = {}      # parameter index -> (requires_grad, dtype, shape, [(module, name)] where it was bound)
         self.stream_of = {}   # parameter index -> its stream (a view of `streams`)
         self.streams = []     # the buffers that hold the streams (one per load group)
@@ -114,29 +149,31 @@ class _Resident:
         self.scratch = None   # the plans' shared scratch
         self.gather_scratch = None  # the gathers' scratch: the plans' one, or a buffer of its own (prefetch)
         self.gather_plan_bytes = 0  # memory of the plans that only serve gathers
-        self.matvec = 0       # matvec=N: the most input rows a matvec module multiplies without decoding
-        self.matvecs = []     # matvec=N: (linear module, plan, index into the plan's outputs)
-        self.matvec_scratch = None  # the matvecs' scratch: the plans' one when it is large enough
-        self.matvec_scratch_bytes = 0  # what the largest matvec needs of it
-        self.matmul = 0       # matmul=N: the most input rows a matmul module multiplies without decoding
-        self.matmuls = set()  # matmul=N: id() of the `matvecs` modules whose weight `DecodePlan.matmul_ok` accepts
-        self.matmul_scratch = None  # the matmuls' scratch: the plans' one when it is large enough
-        self.matmul_scratch_bytes = 0  # what the largest matmul needs of it
-        self.experts = set()  # experts=True: id() of the `entries` modules that decode only their routed experts
-        self.select_scratch = None  # the experts modules' run_select scratch, sized for the largest
-        self.fp8s = []        # fp8=True: (fp8 linear module, plan, index into the plan's outputs, matvec_fp8 / dequant_fp8 take it?)
-        self.fp8_scratch = None  # the fp8 modules' matvec_fp8 scratch: the plans' one when it is large enough
-        self.fp8_scratch_bytes = 0  # what the largest of them needs of it
+        self.matvec = 0       # matvec=N: the most input rows a "matvec" / "matmul" / "fp8" module multiplies by a matvec
+        self.matvec_scratch = None     # the matvecs' scratch and what the largest of them needs of it
+        self.matvec_scratch_bytes = 0
+        self.matmul_scratch = None     # the "matmul" modules' matmul scratch and what the largest needs of it
+        self.matmul_scratch_bytes = 0
+        self.select_scratch = None     # the "experts" modules' run_select scratch, sized for the largest
+        self.fp8_scratch = None        # the "fp8" modules' matvec_fp8 scratch and what the largest needs of it
+        self.fp8_scratch_bytes = 0
+
+
+def _grad_mode_error(mod, shared: bool = False):
+    raise RuntimeError(f"{type(mod).__name__} holds compressed weights and runs only under torch.no_grad() or "
+                       "torch.inference_mode()" + (" (its decoded weights live in a shared buffer)" if shared else ""))
+
+
+def _bind(mod, names, outs) -> None:
+    for name, k in names:
+        object.__setattr__(mod, name, outs[k])
 
 
 def _pre_hook(plan, names):
     def hook(mod, args):
         if torch.is_grad_enabled():
-            raise RuntimeError(f"{type(mod).__name__} holds compressed weights and runs only under torch.no_grad() or "
-                               "torch.inference_mode() (its decoded weights live in a shared buffer)")
-        outs = plan.run()
-        for name, k in names:
-            object.__setattr__(mod, name, outs[k])
+            _grad_mode_error(mod, shared=True)
+        _bind(mod, names, plan.run())
     return hook
 
 
@@ -144,27 +181,21 @@ def _pre_hook_experts(plan, names, state):
     # the ids: experts(hidden_states, top_k_index, top_k_weights), positional or by keyword
     def hook(mod, args, kwargs):
         if torch.is_grad_enabled():
-            raise RuntimeError(f"{type(mod).__name__} holds compressed weights and runs only under torch.no_grad() or "
-                               "torch.inference_mode() (its decoded weights live in a shared buffer)")
+            _grad_mode_error(mod, shared=True)
         ids = args[1] if len(args) > 1 else kwargs.get("top_k_index")
         if (isinstance(ids, torch.Tensor) and ids.is_cuda and ids.device == plan.device
                 and ids.dtype in (torch.int32, torch.int64)):
-            outs = plan.run_select(ids, scratch=state.select_scratch)
+            _bind(mod, names, plan.run_select(ids, scratch=state.select_scratch))
         else:
-            outs = plan.run()
-        for name, k in names:
-            object.__setattr__(mod, name, outs[k])
+            _bind(mod, names, plan.run())
     return hook
 
 
 def _pre_hook_prefetch(sched, key, names, views):
     def hook(mod, args):
         if torch.is_grad_enabled():
-            raise RuntimeError(f"{type(mod).__name__} holds compressed weights and runs only under torch.no_grad() or "
-                               "torch.inference_mode() (its decoded weights live in a shared buffer)")
-        outs = views[sched.before(key)]
-        for name, k in names:
-            object.__setattr__(mod, name, outs[k])
+            _grad_mode_error(mod, shared=True)
+        _bind(mod, names, views[sched.before(key)])
     return hook
 
 
@@ -178,8 +209,7 @@ def _gather_forward(mod, state, plan, k):
     # padding_idx, scale_grad_by_freq and sparse only shape gradients, which a compressed module never has
     def forward(input):
         if torch.is_grad_enabled():
-            raise RuntimeError(f"{type(mod).__name__} holds compressed weights and runs only under torch.no_grad() or "
-                               "torch.inference_mode()")
+            _grad_mode_error(mod)
         return plan.gather(k, input, scratch=state.gather_scratch)
     return forward
 
@@ -200,13 +230,6 @@ def experts_module(module: torch.nn.Module, names=None) -> bool:
         return False
     params = [p for name, p in _own_params(module) if names is None or name in names]
     return bool(params) and all(p.dim() >= 1 and p.shape[0] == n for p in params)
-
-
-def _check_experts(experts: bool, prefetch: bool) -> bool:
-    if experts and prefetch:
-        raise ValueError("experts=True and prefetch=True do not combine: the prefetch schedule decodes every module "
-                         "before its router has picked the experts")
-    return bool(experts)
 
 
 def fp8_linears(module: torch.nn.Module) -> bool:
@@ -249,26 +272,27 @@ def dense_biases(groups, matvec: int, fp8: bool = False) -> list:
     return [(p, owners) for p, owners in groups if not all(dense(o, n) for o, n in owners)]
 
 
-def _check_matvec(matvec: int, prefetch: bool, name: str = "matvec", limit: int = MATVEC_MAX_TOKENS) -> int:
-    if not (isinstance(matvec, int) and 0 <= matvec <= limit):
-        raise ValueError(f"{name} must be an integer from 0 to {limit}, not {matvec!r}")
-    if matvec and prefetch:
-        raise ValueError(f"{name} and prefetch=True do not combine yet: the prefetch schedule decodes every module")
-    return matvec
-
-
-def _check_matmul(matmul: int, prefetch: bool) -> int:
-    return _check_matvec(matmul, prefetch, "matmul", MATMUL_MAX_TOKENS)
-
-
-def _check_fp8(fp8: bool, prefetch: bool) -> bool:
-    if fp8 and prefetch:
-        raise ValueError("fp8=True and prefetch=True do not combine yet: the prefetch schedule decodes every module")
-    return bool(fp8)
-
-
 def _fp8_block(mod) -> tuple:
     return None if mod.block_size is None else tuple(mod.block_size)
+
+
+def _rows(input) -> int:
+    """The rows of an input [..., in_features]: the product of its leading dims (None without a last dim to divide by)."""
+    width = input.shape[-1] if input.dim() else 0
+    return input.numel() // width if width else None
+
+
+def _decoded(mod, plan, names, forward):
+    """-> f(input): the decode, bind, `forward(mod, input)`, unbind of the hooks every other compressed module has."""
+    pre, post = _pre_hook(plan, names), _unbind(names)
+
+    def run(input):
+        pre(mod, (input,))
+        try:
+            return forward(mod, input)
+        finally:
+            post(mod, (input,), None)
+    return run
 
 
 def _fp8_forward(mod, state, plan, k, names, fast: bool):
@@ -278,7 +302,7 @@ def _fp8_forward(mod, state, plan, k, names, fast: bool):
     FP8Linear.forward adds it.  A module whose weight `fast` is False for (`matvec_fp8_ok` refuses it) decodes it and
     dequantizes in torch into a fresh tensor instead (the fp8 bytes occupy the shared buffer), with the same result.
     Any other input takes the decode, bind, module's own forward, unbind of the other compressed modules."""
-    pre, post = _pre_hook(plan, names), _unbind(names)
+    decoded = _decoded(mod, plan, names, type(mod).forward)
     block = _fp8_block(mod)
     shape = tuple(plan.outputs[k].shape)
     nbytes = 2 * shape[0] * shape[1]
@@ -287,10 +311,8 @@ def _fp8_forward(mod, state, plan, k, names, fast: bool):
         if (input.dtype in (torch.bfloat16, torch.float16) and input.device == plan.device
                 and not torch.is_autocast_enabled(plan.device.type)):
             if torch.is_grad_enabled():
-                raise RuntimeError(f"{type(mod).__name__} holds compressed weights and runs only under torch.no_grad() or "
-                                   "torch.inference_mode()")
-            width = input.shape[-1] if input.dim() else 0
-            rows = input.numel() // width if width else None
+                _grad_mode_error(mod)
+            rows = _rows(input)
             scale = mod.weight_scale_inv
             if fast and rows is not None and rows <= state.matvec:
                 y = plan.matvec_fp8(k, input, scale, block, scratch=state.fp8_scratch)
@@ -301,38 +323,28 @@ def _fp8_forward(mod, state, plan, k, names, fast: bool):
                     w = dequantize_fp8(plan.run()[k], scale, block, input.dtype)
                 y = F.linear(input, w)
             return y if mod.bias is None else (y + mod.bias).to(input.dtype)
-        pre(mod, (input,))
-        try:
-            return type(mod).forward(mod, input)
-        finally:
-            post(mod, (input,), None)
+        return decoded(input)
     return forward
 
 
 def _matvec_forward(mod, state, plan, k, names, dtype, device, matmul: int = 0):
     """The forward of a matvec module: an input of at most `state.matvec` rows (a host-side test of its shape) that has
     the weight's `dtype` and `device`, outside autocast, goes to `plan.matvec`; one of more rows and at most `matmul`
-    (the module's limit: `state.matmul` for the modules in `state.matmuls`, else 0) goes to `plan.matmul`.  Then nothing
-    is decoded or bound.  Any other input (a larger one, another dtype, an autocast region: whatever F.linear accepts)
+    (the module's limit: `matmul` for a "matmul" module, 0 for a "matvec" one) goes to `plan.matmul`.  Then nothing is
+    decoded or bound.  Any other input (a larger one, another dtype, an autocast region: whatever F.linear accepts)
     takes the decode, bind, forward, unbind of the hooks every other compressed module has."""
-    pre, post = _pre_hook(plan, names), _unbind(names)
+    decoded = _decoded(mod, plan, names, torch.nn.Linear.forward)
 
     def forward(input):
-        width = input.shape[-1] if input.dim() else 0
-        rows = input.numel() // width if width else None
+        rows = _rows(input)
         if (rows is not None and rows <= max(state.matvec, matmul) and input.dtype == dtype and input.device == device
                 and not torch.is_autocast_enabled(device.type)):
             if torch.is_grad_enabled():
-                raise RuntimeError(f"{type(mod).__name__} holds compressed weights and runs only under torch.no_grad() or "
-                                   "torch.inference_mode()")
+                _grad_mode_error(mod)
             if rows <= state.matvec:
                 return plan.matvec(k, input, bias=mod.bias, scratch=state.matvec_scratch)
             return plan.matmul(k, input, bias=mod.bias, scratch=state.matmul_scratch)
-        pre(mod, (input,))
-        try:
-            return torch.nn.Linear.forward(mod, input)
-        finally:
-            post(mod, (input,), None)
+        return decoded(input)
     return forward
 
 
@@ -361,23 +373,27 @@ def split_gathers(per_module, gather: bool) -> tuple:
     return whole, looked, own
 
 
+def _aligned_views(sizes: list, dev) -> tuple:
+    """Byte sizes -> (one uint8 buffer, a view of each size in it): back to back, each at a 16-byte aligned offset,
+    since the plans' recorded segment starts depend on a stream's address modulo 16."""
+    offs, at = [], 0
+    for n in sizes:
+        offs.append(at)
+        at = (at + n + 15) // 16 * 16
+    buf = torch.empty(max(at, 1), dtype=torch.uint8, device=dev)
+    return buf, [buf[o: o + n] for o, n in zip(offs, sizes)]
+
+
 def _pack(streams: dict, dev) -> tuple:
     """{group index: CUDA uint8 stream} -> (one tight buffer holding them at 16-byte aligned offsets, {index: its
     view}); the sources are only read."""
-    offs, at = {}, 0
-    for i, s in streams.items():
-        offs[i] = at
-        at = (at + s.numel() + 15) // 16 * 16
-    buf = torch.empty(max(at, 1), dtype=torch.uint8, device=dev)
-    views = {}
-    for i, s in streams.items():
-        views[i] = buf[offs[i]: offs[i] + s.numel()]
-        views[i].copy_(s)
-    return buf, views
+    buf, views = _aligned_views([s.numel() for s in streams.values()], dev)
+    for v, s in zip(views, streams.values()):
+        v.copy_(s)
+    return buf, dict(zip(streams, views))
 
 
-def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: bool = False, matvec: int = 0,
-                    matmul: int = 0, experts: bool = False, fp8: bool = False) -> tuple:
+def _resident_state(modules, groups, streams: dict, buffers: list, dev, opts: _Options) -> tuple:
     """The back half of compress_module and load_module: streams {group index: CUDA stream} -> per selected module
     one DecodePlan over its parameters' streams, all sharing one output and one scratch buffer.  Raises like
     `decompress` on a corrupt stream; nothing outside is touched until `_commit`.  -> (_Resident, report).
@@ -386,22 +402,23 @@ def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: 
     tied lm_head) gathers through that module's plan; any other gets a plan of its own, created first, into a
     transient buffer that is freed before the shared output buffer exists (so the peak stays that of gather=False).
 
-    matvec=N: a `matvecs` module whose one compressed parameter is a weight that `DecodePlan.matvec_ok` accepts is
-    listed in `state.matvecs`; its plan and its room in the shared output buffer stay (larger inputs decode).
-    matmul=N: the same for `DecodePlan.matmul_ok`; such a module is also in `state.matmuls`.
-    experts=True: an `experts_module` whose plan passes `DecodePlan.select_ok` is in `state.experts`.
-    fp8=True: an `fp8_linears` module whose one compressed parameter is its weight is in `state.fp8s`; the shared output
-    buffer holds at least twice its weight's bytes (its dequantized weight)."""
+    Every other module is an `_Entry`, its plan and its room in the shared output buffer kept (larger inputs decode),
+    in the first mode that applies: "matmul" for a `matvecs` module whose one compressed parameter is a weight that
+    `DecodePlan.matmul_ok` accepts (matmul=N), "matvec" for one that only `DecodePlan.matvec_ok` accepts (matvec=N);
+    "fp8" for an `fp8_linears` module whose one compressed parameter is its weight and which `DecodePlan.matvec_fp8_ok`
+    accepts, "fp8_torch" for one it refuses (fp8=True; the shared output buffer holds at least twice such a weight's
+    bytes, its dequantized weight); "experts" for an `experts_module` whose plan passes `DecodePlan.select_ok`
+    (experts=True); else "prefetch" with prefetch=True, "decode" without."""
     where = {id(groups[i][0]): i for i in streams}
     per_module = []
     for m in modules:
         names = [(n, where[id(p)]) for n, p in _own_params(m) if id(p) in where]
         if names:
             per_module.append((m, names))
-    whole, looked, own = split_gathers(per_module, gather)
+    whole, looked, own = split_gathers(per_module, opts.gather)
     sizes = [DecodePlan.sizes([streams[i] for _, i in names]) for _, names in whole]
     own_sizes = [DecodePlan.sizes([streams[i]]) for i in own]
-    fp8_mods = {id(m) for m, names in whole if fp8 and fp8_linears(m) and [n for n, _ in names] == ["weight"]}
+    fp8_mods = {id(m) for m, names in whole if opts.fp8 and fp8_linears(m) and [n for n, _ in names] == ["weight"]}
     out_need = max([s[0] for s in sizes] + [2 * m.weight.numel() for m, _ in whole if id(m) in fp8_mods] + [1])
     out = None if own else torch.empty(out_need, dtype=torch.uint8, device=dev)
     scratch = torch.empty(max([s[1] for s in sizes + own_sizes] + [1]), dtype=torch.uint8, device=dev)
@@ -424,22 +441,21 @@ def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: 
         plan = DecodePlan([streams[i] for _, i in names], out=out, scratch=scratch)
         plan_bytes += plan.nbytes["plan"]
         index_bytes += plan.nbytes["index"]
-        state.entries.append((m, plan, [(n, k) for k, (n, _) in enumerate(names)], []))
+        local = [(n, k) for k, (n, _) in enumerate(names)]
         for k, (_, i) in enumerate(names):
             by_stream.setdefault(i, (plan, k))
-        if (matvec or matmul) and matvecs(m) and [n for n, _ in names] == ["weight"]:
-            mm = bool(matmul) and plan.matmul_ok(0, m.in_features)
-            if mm or (matvec and plan.matvec_ok(0, m.in_features)):
-                state.matvecs.append((m, plan, 0))
-            if mm:
-                state.matmuls.add(id(m))
-        if experts and experts_module(m, [n for n, _ in names]) and plan.select_ok():
-            state.experts.add(id(m))
-        if id(m) in fp8_mods:
+        linear = matvecs(m) and local == [("weight", 0)]
+        mm = bool(opts.matmul) and linear and plan.matmul_ok(0, m.in_features)
+        if mm or (opts.matvec and linear and plan.matvec_ok(0, m.in_features)):
+            mode = "matmul" if mm else "matvec"
+        elif id(m) in fp8_mods:
             block = _fp8_block(m)
-            fast = plan.matvec_fp8_ok(0, m.in_features) and (block is None or block[1] % 16 == 0)
-            state.fp8s.append((m, plan, 0, fast))
-    state.matvec, state.matmul = matvec, matmul
+            mode = "fp8" if plan.matvec_fp8_ok(0, m.in_features) and (block is None or block[1] % 16 == 0) else "fp8_torch"
+        elif opts.experts and experts_module(m, [n for n, _ in local]) and plan.select_ok():
+            mode = "experts"
+        else:
+            mode = "prefetch" if opts.prefetch else "decode"
+        state.entries.append(_Entry(m, plan, local, mode))
     for m, i in looked:
         plan, k = by_stream[i]
         state.gathers.append((m, plan, k, i in own))
@@ -454,11 +470,16 @@ def _resident_state(modules, groups, streams: dict, buffers: list, dev, gather: 
                    "params": len(streams), "modules": len(per_module)}
 
 
-def _commit(module: torch.nn.Module, state: _Resident, prefetch: bool = False) -> None:
-    """Hooks on, compressed parameters out: after this the model runs from its streams."""
+def _plans_scratch_or_own(state: _Resident, need: int):
+    """The plans' scratch if it holds `need` bytes, else a buffer of `need` bytes."""
+    return state.scratch if need <= state.scratch.numel() else torch.empty(need, dtype=torch.uint8, device=state.scratch.device)
+
+
+def _commit(module: torch.nn.Module, state: _Resident, opts: _Options) -> None:
+    """Hooks and forwards on, compressed parameters out: after this the model runs from its streams."""
     sched = None
-    if prefetch and state.entries:
-        plans = [plan for _, plan, _, _ in state.entries]
+    if opts.prefetch and state.entries:
+        plans = [e.plan for e in state.entries]
         slot1 = torch.empty_like(plans[0]._out)
         slots = [plans[0]._out, slot1]
         sched = _prefetch.Prefetcher(_prefetch.CudaOps(plans[0].device, plans, slots, _prefetch.prefetch_ctas()))
@@ -467,52 +488,46 @@ def _commit(module: torch.nn.Module, state: _Resident, prefetch: bool = False) -
         state.prefetch = (sched, slot1, roots)
     if state.gathers:
         # the plans' scratch, whose runs share the forward's stream; with prefetch those runs move to the side stream,
-        # so the gathers get a buffer of their own.  One slot at least.
+        # so the gathers get a buffer of their own, of the plans' scratch's size at least.  One slot at least.
         need = max(plan.gather_scratch_bytes(k, 1) for _, plan, k, _ in state.gathers)
-        if prefetch or need > state.scratch.numel():
+        if opts.prefetch or need > state.scratch.numel():
             state.gather_scratch = torch.empty(max(need, state.scratch.numel()), dtype=torch.uint8, device=state.scratch.device)
         else:
             state.gather_scratch = state.scratch
         for m, plan, k, _ in state.gathers:
             m.__dict__["forward"] = _gather_forward(m, state, plan, k)
-    if state.matvecs and state.matvec:
-        need = max(plan.matvec_scratch_bytes(k, m.in_features, state.matvec) for m, plan, k in state.matvecs)
-        state.matvec_scratch_bytes = need
-        state.matvec_scratch = state.scratch if need <= state.scratch.numel() else torch.empty(need, dtype=torch.uint8,
-                                                                                                device=state.scratch.device)
-    if state.matmuls:
-        need = max(plan.matmul_scratch_bytes(k, m.in_features, state.matmul) for m, plan, k in state.matvecs if id(m) in state.matmuls)
-        state.matmul_scratch_bytes = need
-        state.matmul_scratch = state.scratch if need <= state.scratch.numel() else torch.empty(need, dtype=torch.uint8,
-                                                                                                device=state.scratch.device)
-    if state.experts:
-        need = max(plan.select_scratch_bytes() for m, plan, _, _ in state.entries if id(m) in state.experts)
+    state.matvec = opts.matvec
+    matvec = [e for e in state.entries if e.mode in ("matvec", "matmul")]
+    matmul = [e for e in state.entries if e.mode == "matmul"]
+    experts = [e for e in state.entries if e.mode == "experts"]
+    fp8 = [e for e in state.entries if e.mode == "fp8"]
+    if matvec and opts.matvec:
+        state.matvec_scratch_bytes = max(e.plan.matvec_scratch_bytes(0, e.module.in_features, opts.matvec) for e in matvec)
+        state.matvec_scratch = _plans_scratch_or_own(state, state.matvec_scratch_bytes)
+    if matmul:
+        state.matmul_scratch_bytes = max(e.plan.matmul_scratch_bytes(0, e.module.in_features, opts.matmul) for e in matmul)
+        state.matmul_scratch = _plans_scratch_or_own(state, state.matmul_scratch_bytes)
+    if experts:
+        # always a buffer of its own: run_select must not be given the plans' scratch
+        need = max(e.plan.select_scratch_bytes() for e in experts)
         state.select_scratch = torch.empty(need, dtype=torch.uint8, device=state.scratch.device)
-    if state.matvec and any(fast for _, _, _, fast in state.fp8s):
-        need = max(plan.matvec_fp8_scratch_bytes(k, m.in_features, state.matvec) for m, plan, k, fast in state.fp8s if fast)
-        state.fp8_scratch_bytes = need
-        state.fp8_scratch = state.scratch if need <= state.scratch.numel() else torch.empty(need, dtype=torch.uint8,
-                                                                                             device=state.scratch.device)
-    by_matvec = {id(m): (plan, k) for m, plan, k in state.matvecs}
-    by_fp8 = {id(m): (k, fast) for m, _, k, fast in state.fp8s}
-    for key, (m, plan, local, hooks) in enumerate(state.entries):
-        if id(m) in by_matvec:   # no hooks: its forward decides per input whether anything is decoded
-            m.__dict__["forward"] = _matvec_forward(m, state, plan, by_matvec[id(m)][1], local, plan.outputs[by_matvec[id(m)][1]].dtype,
-                                                    plan.device, state.matmul if id(m) in state.matmuls else 0)
-            continue
-        if id(m) in by_fp8:   # no hooks either: its forward multiplies from the stream, or decodes
-            k, fast = by_fp8[id(m)]
-            m.__dict__["forward"] = _fp8_forward(m, state, plan, k, local, fast)
-            continue
-        if id(m) in state.experts:
-            hooks.append(m.register_forward_pre_hook(_pre_hook_experts(plan, local, state), with_kwargs=True))
+    if fp8 and opts.matvec:
+        state.fp8_scratch_bytes = max(e.plan.matvec_fp8_scratch_bytes(0, e.module.in_features, opts.matvec) for e in fp8)
+        state.fp8_scratch = _plans_scratch_or_own(state, state.fp8_scratch_bytes)
+    for key, (m, plan, names, mode) in enumerate(state.entries):
+        if mode in ("matvec", "matmul"):   # no hooks: its forward decides per input whether anything is decoded
+            m.__dict__["forward"] = _matvec_forward(m, state, plan, 0, names, plan.outputs[0].dtype, plan.device,
+                                                    opts.matmul if mode == "matmul" else 0)
+        elif mode in ("fp8", "fp8_torch"):   # no hooks either: its forward multiplies from the stream, or decodes
+            m.__dict__["forward"] = _fp8_forward(m, state, plan, 0, names, mode == "fp8")
         else:
-            if sched is None:
-                pre = _pre_hook(plan, local)
+            if mode == "experts":
+                pre = m.register_forward_pre_hook(_pre_hook_experts(plan, names, state), with_kwargs=True)
+            elif mode == "prefetch":
+                pre = m.register_forward_pre_hook(_pre_hook_prefetch(sched, key, names, [plan.views(b) for b in sched.ops.slots]))
             else:
-                pre = _pre_hook_prefetch(sched, key, local, [plan.views(b) for b in sched.ops.slots])
-            hooks.append(m.register_forward_pre_hook(pre))
-        hooks.append(m.register_forward_hook(_unbind(local), always_call=True))
+                pre = m.register_forward_pre_hook(_pre_hook(plan, names))
+            state.hooks += [pre, m.register_forward_hook(_unbind(names), always_call=True)]
     # the dense parameters go: nothing here keeps their storage alive
     for _, _, _, owners in state.params.values():
         for o, n in owners:
@@ -584,14 +599,11 @@ def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = Fals
     shared output buffer holds at least twice the largest such weight's bytes.  `matmul` does not apply to fp8 weights.
     The report gains "fp8_modules" and "fp8_scratch_bytes" (the matvec_fp8 scratch, the plans' one when it is large
     enough).  ValueError together with prefetch=True."""
-    matvec = _check_matvec(matvec, prefetch)
-    matmul = _check_matmul(matmul, prefetch)
-    experts = _check_experts(experts, prefetch)
-    fp8 = _check_fp8(fp8, prefetch)
+    opts = _options(prefetch, gather, matvec, matmul, experts, fp8)
     if getattr(module, _ATTR, None) is not None:
         raise ValueError("compress_module: this module is already compressed")
     modules, groups = select(module, modules)
-    groups = dense_biases(groups, max(matvec, matmul), fp8)
+    groups = dense_biases(groups, max(opts.matvec, opts.matmul), opts.fp8)
     params = [p for p, _ in groups]
     if not params:
         setattr(module, _ATTR, None)
@@ -604,31 +616,31 @@ def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = Fals
     # the streams move into one tight buffer; the batch's output buffer (sized by the bound) is dropped
     buf, streams = _pack({i: s for i, (p, s) in enumerate(zip(params, coded)) if s.numel() < p.numel() * p.element_size()}, dev)
     del coded, params
-    state, report = _resident_state(modules, groups, streams, [buf], dev, gather, matvec, matmul, experts, fp8)
-    _commit(module, state, prefetch)
-    return _with_prefetch(report, state, prefetch, gather, matvec, matmul, experts, fp8)
+    state, report = _resident_state(modules, groups, streams, [buf], dev, opts)
+    _commit(module, state, opts)
+    return _with_prefetch(report, state, opts)
 
 
-def _with_prefetch(report: dict, state, prefetch: bool, gather: bool = False, matvec: int = 0, matmul: int = 0,
-                   experts: bool = False, fp8: bool = False) -> dict:
-    if prefetch:
-        report = dict(report, prefetch_out_bytes=state.prefetch[1].numel() if state is not None and state.prefetch else 0)
-    if gather:
-        own = state is not None and state.gather_scratch is not None and state.gather_scratch is not state.scratch
-        report = dict(report, gather_modules=len(state.gathers) if state is not None else 0,
-                      gather_bytes=(state.gather_plan_bytes + (state.gather_scratch.numel() if own else 0)) if state is not None else 0)
-    if matvec:
-        report = dict(report, matvec_modules=len(state.matvecs) if state is not None else 0,
-                      matvec_scratch_bytes=state.matvec_scratch_bytes if state is not None else 0)
-    if matmul:
-        report = dict(report, matmul_modules=len(state.matmuls) if state is not None else 0,
-                      matmul_scratch_bytes=state.matmul_scratch_bytes if state is not None else 0)
-    if experts:
-        report = dict(report, experts_modules=len(state.experts) if state is not None else 0,
-                      experts_scratch_bytes=state.select_scratch.numel() if state is not None and state.select_scratch is not None else 0)
-    if fp8:
-        report = dict(report, fp8_modules=len(state.fp8s) if state is not None else 0,
-                      fp8_scratch_bytes=state.fp8_scratch_bytes if state is not None else 0)
+def _with_prefetch(report: dict, state, opts: _Options) -> dict:
+    """`report` with the keys of every mode `opts` turns on, prefetch's and the others'; all 0 for a model with nothing
+    compressed (state None)."""
+    state = _Resident() if state is None else state
+    modes = [e.mode for e in state.entries]
+    report = dict(report)
+    if opts.prefetch:
+        report.update(prefetch_out_bytes=state.prefetch[1].numel() if state.prefetch else 0)
+    if opts.gather:
+        own = state.gather_scratch is not None and state.gather_scratch is not state.scratch
+        report.update(gather_modules=len(state.gathers), gather_bytes=state.gather_plan_bytes + (state.gather_scratch.numel() if own else 0))
+    if opts.matvec:
+        report.update(matvec_modules=modes.count("matvec") + modes.count("matmul"), matvec_scratch_bytes=state.matvec_scratch_bytes)
+    if opts.matmul:
+        report.update(matmul_modules=modes.count("matmul"), matmul_scratch_bytes=state.matmul_scratch_bytes)
+    if opts.experts:
+        report.update(experts_modules=modes.count("experts"),
+                      experts_scratch_bytes=0 if state.select_scratch is None else state.select_scratch.numel())
+    if opts.fp8:
+        report.update(fp8_modules=modes.count("fp8") + modes.count("fp8_torch"), fp8_scratch_bytes=state.fp8_scratch_bytes)
     return report
 
 
@@ -648,14 +660,12 @@ def decompress_module(module: torch.nn.Module) -> None:
             h.remove()
         sched.ops.slots = None   # slot 1 goes with the state
         state.prefetch = None
-    for _, _, _, hooks in state.entries:
-        for h in hooks:
-            h.remove()
+    for h in state.hooks:
+        h.remove()
+    for m, _, _, mode in state.entries:
+        if mode in ("matvec", "matmul", "fp8", "fp8_torch"):   # the modes whose forward _commit replaced
+            m.__dict__.pop("forward", None)
     for m, _, _, _ in state.gathers:
-        m.__dict__.pop("forward", None)
-    for m, _, _ in state.matvecs:
-        m.__dict__.pop("forward", None)
-    for m, _, _, _ in state.fp8s:
         m.__dict__.pop("forward", None)
     # each module's plan decodes into the shared buffer once more; its parameters are copied out of it, so the
     # model needs its dense size plus that buffer, not twice its dense size
@@ -688,10 +698,6 @@ def decompress_module(module: torch.nn.Module) -> None:
         params.update(reordered)
     state.entries.clear()
     state.gathers.clear()
-    state.matvecs.clear()
-    state.fp8s.clear()
-    state.matmuls.clear()
-    state.experts.clear()
     delattr(module, _ATTR)
 
 
@@ -831,8 +837,7 @@ def plan_load(module: torch.nn.Module, filenames, modules=None, matvec: int = 0,
     return plan
 
 
-def _load_device(plan: LoadPlan, dev, gather: bool = False, matvec: int = 0, matmul: int = 0, experts: bool = False,
-                 fp8: bool = False) -> tuple:
+def _load_device(plan: LoadPlan, dev, opts: _Options) -> tuple:
     """Every device step of load_module; the module is not touched.  -> (_Resident or None, report, dense tensors of
     plan.dense, {group index: dense tensor} of plain entries that did not compress, moved buffers of plan.moves)."""
     pipe = DecodePipe(dev)
@@ -850,17 +855,15 @@ def _load_device(plan: LoadPlan, dev, gather: bool = False, matvec: int = 0, mat
     try:
         with torch.cuda.device(dev), torch.no_grad():
             cur = torch.cuda.current_stream()
-            # compressed entries of selected parameters: one buffer, each stream at a 16-byte aligned offset (the
-            # plans' recorded segment starts depend on the address modulo 16), never decoded but by plan create
-            buffers, streams, at, offs = [], {}, 0, []
-            for _, e in plan.streams:
-                offs.append(at)
-                at = (at + e.nbytes + 15) // 16 * 16
+            # compressed entries of selected parameters: one buffer, each stream at a 16-byte aligned offset, never
+            # decoded but by plan create
+            buffers, streams = [], {}
             if plan.streams:
-                buffers.append(torch.empty(at, dtype=torch.uint8, device=dev))
-                for (gi, e), o in zip(plan.streams, offs):
-                    streams[gi] = buffers[0][o: o + e.nbytes]
-                    upload(streams[gi], e)
+                buf, views = _aligned_views([e.nbytes for _, e in plan.streams], dev)
+                buffers.append(buf)
+                for (gi, e), v in zip(plan.streams, views):
+                    streams[gi] = v
+                    upload(v, e)
             # plain floating-point entries of selected parameters: compressed a group at a time, compress_module's rule
             entries = [(gi, _FileRange(fd(e.file), e.offset, e.nbytes, e.dtype, e.shape)) for gi, e in plan.compress]
             stayed = {}
@@ -902,8 +905,7 @@ def _load_device(plan: LoadPlan, dev, gather: bool = False, matvec: int = 0, mat
             pipe.finish()
             moved = [m._buffers[n].to(dev) for m, n in plan.moves]
             if plan.groups:
-                state, report = _resident_state(plan.modules, plan.groups, dict(sorted(streams.items())), buffers, dev, gather, matvec,
-                                                matmul, experts, fp8)
+                state, report = _resident_state(plan.modules, plan.groups, dict(sorted(streams.items())), buffers, dev, opts)
             else:
                 state, report = None, dict(_EMPTY_REPORT)
         return state, report, dense, stayed, moved
@@ -952,18 +954,15 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None,
     prefetch, gather, matvec, matmul, experts, fp8: as for `compress_module`.
 
     -> the report of `compress_module`."""
-    matvec = _check_matvec(matvec, prefetch)
-    matmul = _check_matmul(matmul, prefetch)
-    experts = _check_experts(experts, prefetch)
-    fp8 = _check_fp8(fp8, prefetch)
+    opts = _options(prefetch, gather, matvec, matmul, experts, fp8)
     dev = _cuda_device(device)
     if dev is None:
         raise ValueError(f"load_module: {device!r} is not a CUDA device")
     if dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
-    plan = plan_load(module, filenames, modules, max(matvec, matmul), fp8)
+    plan = plan_load(module, filenames, modules, max(opts.matvec, opts.matmul), opts.fp8)
     try:
-        state, report, dense, stayed, moved = _load_device(plan, dev, gather, matvec, matmul, experts, fp8)
+        state, report, dense, stayed, moved = _load_device(plan, dev, opts)
     except BaseException as e:
         traceback.clear_frames(e.__traceback__)   # the frames' locals would keep the call's device memory alive
         raise
@@ -984,8 +983,8 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None,
     if state is None:
         setattr(module, _ATTR, None)
     else:
-        _commit(module, state, prefetch)
-    return _with_prefetch(report, state, prefetch, gather, matvec, matmul, experts, fp8)
+        _commit(module, state, opts)
+    return _with_prefetch(report, state, opts)
 
 
 def save_module(module: torch.nn.Module, filename, metadata=None) -> None:
