@@ -340,6 +340,25 @@ int zipnn_b200_decode_plan_matvec_fp8(const zipnn_b200_decode_plan* plan, int it
                                       const void* d_bias, void* d_y, size_t y_stride,
                                       void* d_scratch, size_t scratch_bytes, void* cuda_stream);
 
+/* _matmul_fp8: y = x D^T (+ bias) for up to ZIPNN_B200_MATMUL_MAX_TOKENS rows of x, on tensor cores, with D the weight
+ * _dequant_fp8 writes for the same arguments: D[o][i] = x_dtype(float(W[o][i]) * S[o / block_rows][i / block_cols]),
+ * neither written nor read dense.  Arguments, eligible items, the host-side rejections (E_ARG as _matvec_fp8, with
+ * ZIPNN_B200_MATMUL_MAX_TOKENS as the row limit and scratch_bytes below _matmul_fp8_scratch_size; E_UNSUPPORTED for
+ * every item _matvec_fp8 refuses) and the first call's read of the chunk modes are _matvec_fp8's.  Each 16 fp8 weights
+ * the replay decoder forms are dequantized to x_dtype exactly as _dequant_fp8 rounds them, and go to mma.m16n8k16 in
+ * x_dtype with fp32 accumulation as B fragments of 8 rows x 64 columns; from there the partial sums, their order, the
+ * rounding, the launches (2; none for n_tokens == 0), graph capture, determinism and the finite-x rule are _matmul's.
+ * So a result is F.linear of _dequant_fp8's weight up to the order of the fp32 sums.  An e4m3fn NaN or an e5m2
+ * infinity or NaN in W, or an fp16 overflow in D, gives NaN or an infinity in that row of y as that F.linear does.
+ * _matmul_fp8_scratch_size: the scratch bytes (_matmul's formula), the same item checks. */
+int zipnn_b200_decode_plan_matmul_fp8_scratch_size(const zipnn_b200_decode_plan* plan, int item, size_t in_features,
+                                                   size_t n_tokens, size_t* out);
+int zipnn_b200_decode_plan_matmul_fp8(const zipnn_b200_decode_plan* plan, int item, int fp8_format, int x_dtype,
+                                      size_t in_features, const void* d_x, size_t x_stride, size_t n_tokens,
+                                      const float* d_scale, size_t block_rows, size_t block_cols,
+                                      const void* d_bias, void* d_y, size_t y_stride,
+                                      void* d_scratch, size_t scratch_bytes, void* cuda_stream);
+
 /* _dequant_fp8: the dequantized weight of an item _matvec_fp8 takes, written straight from its coded bitstreams:
  * d_out[o][i] = out_dtype(float(W[o][i]) * S[o / block_rows][i / block_cols]), W, d_scale and the blocks as for
  * _matvec_fp8, d_out a contiguous [out_features][in_features] tensor of out_dtype, ZIPNN_B200_MATVEC_BF16 or _FP16.

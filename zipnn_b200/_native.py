@@ -128,6 +128,9 @@ def lib() -> C.CDLL:
                 "zipnn_b200_decode_plan_matvec_fp8_scratch_size": (i32, [C.POINTER(DecodePlanStruct), i32, sz, sz, szp]),
                 "zipnn_b200_decode_plan_matvec_fp8": (i32, [C.POINTER(DecodePlanStruct), i32, i32, i32, sz, vp, sz, sz, vp, sz, sz, vp, vp, sz,
                                                              vp, sz, vp]),
+                "zipnn_b200_decode_plan_matmul_fp8_scratch_size": (i32, [C.POINTER(DecodePlanStruct), i32, sz, sz, szp]),
+                "zipnn_b200_decode_plan_matmul_fp8": (i32, [C.POINTER(DecodePlanStruct), i32, i32, i32, sz, vp, sz, sz, vp, sz, sz, vp, vp, sz,
+                                                             vp, sz, vp]),
                 "zipnn_b200_decode_plan_dequant_fp8": (i32, [C.POINTER(DecodePlanStruct), i32, i32, i32, sz, vp, sz, sz, vp, vp]),
                 "zipnn_b200_split": (i32, [vp, sz, i32, i32, vp, sz, vp]),
                 "zipnn_b200_regroup": (i32, [vp, sz, sz, i32, i32, vp, vp]),
@@ -157,6 +160,7 @@ EXPORTS = [
     "zipnn_b200_decode_plan_matvec_scratch_size", "zipnn_b200_decode_plan_matvec",
     "zipnn_b200_decode_plan_matmul_scratch_size", "zipnn_b200_decode_plan_matmul",
     "zipnn_b200_decode_plan_matvec_fp8_scratch_size", "zipnn_b200_decode_plan_matvec_fp8",
+    "zipnn_b200_decode_plan_matmul_fp8_scratch_size", "zipnn_b200_decode_plan_matmul_fp8",
     "zipnn_b200_decode_plan_dequant_fp8", "zipnn_b200_split", "zipnn_b200_regroup", "zipnn_b200_compress_host", "zipnn_b200_decompress_host",
     "zipnn_b200_timing_enable", "zipnn_b200_timing_kernel_count", "zipnn_b200_timing_kernel_name",
     "zipnn_b200_timing_collect",

@@ -18,6 +18,13 @@
 // order are one 16-byte load of x per token row: columns 8j .. 8j + 7 of tokens g and g + 8 of each 16-row tile, whose
 // words 2s and 2s + 1 are a0a1 / a4a5 (token g) and a2a3 / a6a7 (token g + 8).  D is [token][W row of the tile].
 //
+// k_matmul_fp8 is k_matmul for fp8 weights with an fp32 scale grid and bf16 / fp16 x (MatmulEp with FMT >= 0): a step is
+// 8 rows x 64 columns, lane (g, j) forms the 16 fp8 weights of row g, columns 16j .. 16j + 15, and after the rotation
+// below dequantizes them exactly as k_dequant_fp8 does (fp8_dequant8: one fp32 multiply by the block's scale, one
+// rounding to x's type) into the B fragments of four k16 steps, register 2s / 2s + 1 = columns 16j + 4s + {0, 1} /
+// {2, 3}; x is two 16-byte loads per token row.  The product is F.linear of dequant_fp8's weight, summed in fp32, and
+// its partial sums go through k_matmul_reduce unchanged.
+//
 // Masking.  A vector outside the quarter's range (partial first and last rows, columns past `in`) is zero and reads no
 // shared memory; x columns past `in` and tokens past n_tokens are zero fragments and are not loaded.  The zero B
 // vectors of a row that straddles two quarters meet real x, so an infinite x there gives NaN where the dense product
@@ -45,7 +52,6 @@ namespace zb {
 
 constexpr int kMatmulMaxTokens = 64;
 constexpr int kMatmulTileRows = 8;    // W rows per tile: n of the mma
-constexpr int kMatmulGroupCols = 128;  // 4 column steps of 32
 
 // Row tiles a quarter of q elements may touch, wherever it starts (rows of `in` elements).
 __host__ __device__ inline uint64_t matmul_quarter_tiles(uint64_t q, uint64_t in, uint64_t out) {
@@ -66,14 +72,20 @@ __device__ __forceinline__ void mma_16816(float (&d)[4], uint32_t a0, uint32_t a
 }
 
 // MT: 16-token tiles a lane accumulates, n_tokens rounded up to 16, 32 or 64.  Tiles wholly past n_tokens are skipped.
-template <int DT, int MT>
+// FMT < 0: W of DT (above).  FMT = kFp8E4m3 / kFp8E5m2: fp8 W with a scale grid and x of DT (k_matmul_fp8, below).
+template <int DT, int MT, int FMT = -1>
 struct MatmulEp {
+  static_assert(DT == kMvBf16 || DT == kMvFp16, "x of bf16 or fp16");
   static constexpr bool on = true;
+  static constexpr uint32_t EB = FMT < 0 ? 2 : 1;  // bytes of a W element
+  static constexpr uint32_t VC = 16 / EB;          // columns of a lane's vector
+  static constexpr uint32_t SC = 4 * VC;           // columns of a step
+  static constexpr uint32_t GC = 4 * SC;           // columns of a group
   ProductCfg m;
 
   template <int G>
   __device__ __forceinline__ void quarter(const SyncShared& S, uint64_t c, int stream, uint32_t out_off, uint32_t count, bool rot) const {
-    static_assert(G == 2, "16-bit weights: two byte planes");
+    static_assert(G == (int)EB, "one byte plane per byte of a W element");
     constexpr int TT = 16 * MT;
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const uint32_t g = (uint32_t)lane >> 2, j = (uint32_t)lane & 3u;
@@ -81,26 +93,27 @@ struct MatmulEp {
     const uint64_t e0 = c * m.ce + out_off, e1 = e0 + count;
     const uint64_t r_first = e0 / in;
     const uint32_t tiles = (uint32_t)((e1 - 1) / in - r_first) / kMatmulTileRows + 1;
-    const uint32_t groups = (uint32_t)((in + kMatmulGroupCols - 1) / kMatmulGroupCols);
+    const uint32_t groups = (uint32_t)((in + GC - 1) / GC);
     const uint32_t mts = min((uint32_t)MT, (m.nt + 15u) >> 4);  // token tiles with a token in them
     const uint8_t* const xb = reinterpret_cast<const uint8_t*>(m.x);
     float* const red = reinterpret_cast<float*>(const_cast<uint8_t*>(S.sbuf));  // [warp][row][TT]
     float* const slots = m.part + (c * 4 + (uint32_t)stream) * m.rt * m.nt * kMatmulTileRows;
     const uint32_t rg = g & 3u;
     for (uint32_t tile = 0; tile < tiles; tile++) {
-      const uint64_t rowe = (r_first + (uint64_t)tile * kMatmulTileRows + g) * in;  // this lane's row, as an element
+      const uint64_t row = r_first + (uint64_t)tile * kMatmulTileRows + g;  // this lane's row
+      const uint64_t rowe = row * in;                                        // ... as an element
       float acc[MT][4];
 #pragma unroll
       for (int mt = 0; mt < MT; mt++) acc[mt][0] = acc[mt][1] = acc[mt][2] = acc[mt][3] = 0.f;
       for (uint32_t grp = (uint32_t)wid; grp < groups; grp += kSyncThreads / 32) {
-        const uint64_t k0 = (uint64_t)grp * kMatmulGroupCols;
+        const uint64_t k0 = (uint64_t)grp * GC;
         uint32_t v[4][4];
 #pragma unroll
         for (int i = 0; i < 4; i++) {
-          const uint64_t col = k0 + 32u * (((uint32_t)i + g) & 3u) + 8u * j;
+          const uint64_t col = k0 + SC * (((uint32_t)i + g) & 3u) + VC * j;
           const uint64_t e = rowe + col;
           if (col < in && e >= e0 && e < e1) {
-            const uint32_t vo = (uint32_t)(e - e0) * 2u;
+            const uint32_t vo = (uint32_t)(e - e0) * EB;
             uint32_t fv[4];  // (a plain name: the macro's own loop index is `i`)
             ZB_FUSED_VECTOR(G, S, out_off, vo, rot, fv);
 #pragma unroll
@@ -121,19 +134,44 @@ struct MatmulEp {
           for (int q = 0; q < 4; q++) v[t][q] = (rg & 2u) ? u[(t + 2) & 3][q] : u[t][q];
 #pragma unroll
         for (int t = 0; t < 4; t++) {
-          const uint64_t kc = k0 + 32u * (uint32_t)t;
+          const uint64_t kc = k0 + SC * (uint32_t)t;
           if (kc >= in) break;  // (uniform)
-          const uint64_t col = kc + 8u * j;
+          const uint64_t col = kc + VC * j;
           const bool cv = col < in;
+          if constexpr (FMT < 0) {
 #pragma unroll
-          for (int mt = 0; mt < MT; mt++) {
-            if ((uint32_t)mt >= mts) break;  // (uniform)
-            const uint32_t t0 = 16u * (uint32_t)mt + g, t1 = t0 + 8u;
-            uint4 xa = make_uint4(0u, 0u, 0u, 0u), xc = xa;
-            if (cv && t0 < m.nt) xa = __ldg(reinterpret_cast<const uint4*>(xb + ((uint64_t)t0 * m.xs + col) * 2u));
-            if (cv && t1 < m.nt) xc = __ldg(reinterpret_cast<const uint4*>(xb + ((uint64_t)t1 * m.xs + col) * 2u));
-            mma_16816<DT>(acc[mt], xa.x, xc.x, xa.y, xc.y, v[t][0], v[t][1]);
-            mma_16816<DT>(acc[mt], xa.z, xc.z, xa.w, xc.w, v[t][2], v[t][3]);
+            for (int mt = 0; mt < MT; mt++) {
+              if ((uint32_t)mt >= mts) break;  // (uniform)
+              const uint32_t t0 = 16u * (uint32_t)mt + g, t1 = t0 + 8u;
+              uint4 xa = make_uint4(0u, 0u, 0u, 0u), xc = xa;
+              if (cv && t0 < m.nt) xa = __ldg(reinterpret_cast<const uint4*>(xb + ((uint64_t)t0 * m.xs + col) * 2u));
+              if (cv && t1 < m.nt) xc = __ldg(reinterpret_cast<const uint4*>(xb + ((uint64_t)t1 * m.xs + col) * 2u));
+              mma_16816<DT>(acc[mt], xa.x, xc.x, xa.y, xc.y, v[t][0], v[t][1]);
+              mma_16816<DT>(acc[mt], xa.z, xc.z, xa.w, xc.w, v[t][2], v[t][3]);
+            }
+          } else {
+            // the vector dequantized as k_dequant_fp8 writes it: a zero vector (outside the quarter) is +0 with no scale
+            // read, so a row or column past the matrix reads nothing
+            const uint64_t e = rowe + col;
+            float sc = 0.f;
+            if (cv && e >= e0 && e < e1)
+              sc = __ldg(m.scale + matvec_fp8_div((uint32_t)row, m.srow) * m.scols + matvec_fp8_div((uint32_t)col, m.scol));
+            // in two halves of 8 columns, the half loop not unrolled: only one half's B fragments and 16 bytes of x per
+            // token row are live at once (unrolled, MT = 2 and 4 spill at 80 registers)
+#pragma unroll 1
+            for (int h = 0; h < 2; h++) {  // columns 16j + 8h .. 16j + 8h + 7: k steps 2h, 2h + 1
+              const uint4 b = fp8_dequant8<FMT, DT>(h ? v[t][2] : v[t][0], h ? v[t][3] : v[t][1], sc);
+#pragma unroll
+              for (int mt = 0; mt < MT; mt++) {
+                if ((uint32_t)mt >= mts) break;  // (uniform)
+                const uint32_t t0 = 16u * (uint32_t)mt + g, t1 = t0 + 8u;
+                uint4 xa = make_uint4(0u, 0u, 0u, 0u), xc = xa;
+                if (cv && t0 < m.nt) xa = __ldg(reinterpret_cast<const uint4*>(xb + ((uint64_t)t0 * m.xs + col) * 2u) + h);
+                if (cv && t1 < m.nt) xc = __ldg(reinterpret_cast<const uint4*>(xb + ((uint64_t)t1 * m.xs + col) * 2u) + h);
+                mma_16816<DT>(acc[mt], xa.x, xc.x, xa.y, xc.y, b.x, b.y);
+                mma_16816<DT>(acc[mt], xa.z, xc.z, xa.w, xc.w, b.z, b.w);
+              }
+            }
           }
         }
       }
@@ -165,6 +203,13 @@ static_assert(sizeof(((SyncShared*)0)->sbuf) >= (kSyncThreads / 32) * kMatmulTil
 template <int DT, int MT>
 __global__ void __launch_bounds__(kSyncThreads, 3) k_matmul(ProductCfg m) {
   product_streams<2>(m, MatmulEp<DT, MT>{m});
+}
+
+// fp8 weights: MatmulEp with 16 fp8 weights per vector; the partial sums are k_matmul_reduce<XDT>'s, whose geometry
+// comes from the element counts (esize 1).
+template <int FMT, int XDT, int MT>
+__global__ void __launch_bounds__(kSyncThreads, 3) k_matmul_fp8(ProductCfg m) {
+  product_streams<1>(m, MatmulEp<XDT, MT, FMT>{m});
 }
 
 template <int DT>

@@ -323,6 +323,27 @@ __global__ void __launch_bounds__(kSyncThreads, 3) k_matvec_fp8(ProductCfg m) {
   product_streams<1>(m, MatvecEp<XDT, NT, FMT>{m});
 }
 
+// The 8 fp8 weights of two words a, b as ODT (bf16 or fp16), each converted exactly, multiplied by the scale sc in fp32
+// and rounded once to nearest even: word i of the result holds weights 2i and 2i + 1.  The dequantize's store and the
+// fp8 matmul's B fragments (matmul.cuh).
+template <int FMT, int ODT>
+__device__ __forceinline__ uint4 fp8_dequant8(uint32_t a, uint32_t b, float sc) {
+  float w[8];
+  fp8_floats<FMT>(a, b, w);
+  uint32_t h[4];
+#pragma unroll
+  for (int i = 0; i < 4; i++) {
+    if constexpr (ODT == kMvBf16) {
+      const __nv_bfloat162 v = __floats2bfloat162_rn(w[2 * i] * sc, w[2 * i + 1] * sc);
+      h[i] = *reinterpret_cast<const uint32_t*>(&v);
+    } else {
+      const __half2 v = __floats2half2_rn(w[2 * i] * sc, w[2 * i + 1] * sc);
+      h[i] = *reinterpret_cast<const uint32_t*>(&v);
+    }
+  }
+  return make_uint4(h[0], h[1], h[2], h[3]);
+}
+
 // ---- the dequantized fp8 weight (k_dequant_fp8) ---------------------------------------------------------------------
 // out[o][i] = ODT(float(W[o][i]) * S[o / bn][i / bk]), W and S as for k_matvec_fp8, out the contiguous bf16 / fp16
 // tensor [out][in] at m.y.  Bit for bit torch's (W.to(float32) * S_expanded).to(ODT): fp8 -> fp32 is exact, then one
@@ -348,25 +369,10 @@ struct DequantEp {
       ZB_FUSED_VECTOR(G, S, out_off, o, rot, r);
       const uint32_t e = e0 + o, row = matvec_fp8_div(e, rin), col = e - row * in;
       const float sc = __ldg(m.scale + matvec_fp8_div(row, m.srow) * m.scols + matvec_fp8_div(col, m.scol));
-      uint32_t h[8];
-#pragma unroll
-      for (int half = 0; half < 2; half++) {
-        float w[8];
-        fp8_floats<FMT>(r[2 * half], r[2 * half + 1], w);
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-          if constexpr (ODT == kMvBf16) {
-            const __nv_bfloat162 v = __floats2bfloat162_rn(w[2 * i] * sc, w[2 * i + 1] * sc);
-            h[4 * half + i] = *reinterpret_cast<const uint32_t*>(&v);
-          } else {
-            const __half2 v = __floats2half2_rn(w[2 * i] * sc, w[2 * i + 1] * sc);
-            h[4 * half + i] = *reinterpret_cast<const uint32_t*>(&v);
-          }
-        }
-      }
+      const uint4 lo = fp8_dequant8<FMT, ODT>(r[0], r[1], sc), hi = fp8_dequant8<FMT, ODT>(r[2], r[3], sc);
       uint4* const dst = reinterpret_cast<uint4*>(m.y) + (e >> 3);
-      dst[0] = make_uint4(h[0], h[1], h[2], h[3]);
-      dst[1] = make_uint4(h[4], h[5], h[6], h[7]);
+      dst[0] = lo;
+      dst[1] = hi;
     }
   }
 };

@@ -1477,16 +1477,19 @@ int zipnn_b200_decode_plan_run_select(const zipnn_b200_decode_plan* plan, size_t
 
 // ---- matvec and matmul: x W^T from the coded bitstreams of one whole-tensor item, no dense W ------------------------
 // Scratch: fp32 partial sums, for the matvec (matvec.cuh) [32 K blocks][rs rows][n_tokens], for the matmul on tensor
-// cores (matmul.cuh) [4 K quarters][rt row tiles][n_tokens][8 rows].  The fp8 matvec's are the matvec's.
+// cores (matmul.cuh) [4 K quarters][rt row tiles][n_tokens][8 rows].  The fp8 matvec's are the matvec's, the fp8
+// matmul's the matmul's.
 namespace {
-enum ProductKind { kMatvec, kMatmul, kMatvecFp8 };
-size_t max_tokens(ProductKind kind) { return kind == kMatmul ? (size_t)kMatmulMaxTokens : (size_t)kMatvecMaxTokens; }
+enum ProductKind { kMatvec, kMatmul, kMatvecFp8, kMatmulFp8 };
+bool fp8_kind(ProductKind kind) { return kind == kMatvecFp8 || kind == kMatmulFp8; }
+bool matmul_kind(ProductKind kind) { return kind == kMatmul || kind == kMatmulFp8; }
+size_t max_tokens(ProductKind kind) { return matmul_kind(kind) ? (size_t)kMatmulMaxTokens : (size_t)kMatvecMaxTokens; }
 
 // The host-side checks shared by all four calls, and the fields of m that the item and the shapes settle.  The first
 // call for an item reads its chunk modes (one synchronising copy of K bytes); the answer is kept with the plan's record.
 // The matmul takes 16-bit weights only: fp32 would need TF32 or a split scheme, so it is left to the decode.  For the
-// fp8 matvec, `dtype` is x's (bf16 or fp16) and the weights are one byte: its scale lookup takes element indices in 32
-// bits, which every fp8 piece has (at most 16383 chunks of 128 KiB).
+// fp8 matvec and matmul, `dtype` is x's (bf16 or fp16) and the weights are one byte: their scale lookup takes element
+// indices in 32 bits, which every fp8 piece has (at most 16383 chunks of 128 KiB).
 int product_item(ProductKind kind, const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, cudaStream_t st, ProductCfg& m) {
   PlanState s;
   GatherItem gi;
@@ -1495,8 +1498,8 @@ int product_item(ProductKind kind, const zipnn_b200_decode_plan* plan, int item,
     const int rc = with_plan_items(s, item, [&](std::vector<GatherItem>& v) { gi = v[(size_t)item]; });
     if (rc) return rc;
   }
-  if (dtype != kMvBf16 && dtype != kMvFp16 && (dtype != kMvFp32 || kind == kMatvecFp8)) return ZIPNN_B200_E_ARG;
-  const uint32_t esize = kind == kMatvecFp8 ? 1u : (uint32_t)matvec_esize(dtype);
+  if (dtype != kMvBf16 && dtype != kMvFp16 && (dtype != kMvFp32 || fp8_kind(kind))) return ZIPNN_B200_E_ARG;
+  const uint32_t esize = fp8_kind(kind) ? 1u : (uint32_t)matvec_esize(dtype);
   const uint64_t total = gi.orig / esize;
   if (in_features == 0 || gi.orig % esize || total % in_features) return ZIPNN_B200_E_ARG;
   if (gi.piece < 0 || s.mode != kSyncReplay || gi.G != (int)esize || (in_features * esize) % 16) return ZIPNN_B200_E_UNSUPPORTED;
@@ -1514,7 +1517,7 @@ int product_item(ProductKind kind, const zipnn_b200_decode_plan* plan, int item,
   }
   if (!gi.fused) return ZIPNN_B200_E_UNSUPPORTED;
   if (kind == kMatmul && dtype == kMvFp32) return ZIPNN_B200_E_UNSUPPORTED;
-  if (kind == kMatvecFp8 && total > (uint64_t)INT32_MAX) return ZIPNN_B200_E_UNSUPPORTED;
+  if (fp8_kind(kind) && total > (uint64_t)INT32_MAX) return ZIPNN_B200_E_UNSUPPORTED;
   memset(&m, 0, sizeof(m));
   m.cfg = s.B.cfgs + gi.piece;
   m.seg = s.X.seg + gi.seg_base;
@@ -1534,12 +1537,12 @@ int product_item(ProductKind kind, const zipnn_b200_decode_plan* plan, int item,
   return ZIPNN_B200_OK;
 }
 size_t product_scratch_bytes(ProductKind kind, const ProductCfg& m, size_t n_tokens) {
-  if (kind == kMatmul) return (size_t)4 * m.K * m.rt * n_tokens * kMatmulTileRows * sizeof(float);
+  if (matmul_kind(kind)) return (size_t)4 * m.K * m.rt * n_tokens * kMatmulTileRows * sizeof(float);
   return (size_t)32 * m.K * m.rs * n_tokens * sizeof(float);
 }
 
 // The bitstream kernel of a product, by how many tokens its lanes hold (matvec: 1, 2, 4 or 8; matmul: 1, 2 or 4 tiles of
-// 16), and its reduce.  DT is the type of x and y; `fmt` the fp8 matvec's weight format (ignored by the others).
+// 16), and its reduce.  DT is the type of x and y; `fmt` the fp8 products' weight format (ignored by the others).
 using ProductKernel = void (*)(ProductCfg);
 struct ProductKernels {
   ProductKernel streams, reduce;
@@ -1553,8 +1556,15 @@ ProductKernel matvec_kernel(ProductKind kind, int fmt) {
 }
 extern "C++" template <int DT>
 ProductKernels product_kernels(ProductKind kind, int fmt, uint32_t nt) {
-  if constexpr (DT != kMvFp32) {  // (product_item refuses an fp32 matmul)
+  if constexpr (DT != kMvFp32) {  // (product_item refuses an fp32 matmul, and fp32 x for fp8 weights)
     if (kind == kMatmul) return {nt <= 16 ? &k_matmul<DT, 1> : nt <= 32 ? &k_matmul<DT, 2> : &k_matmul<DT, 4>, &k_matmul_reduce<DT>};
+    if (kind == kMatmulFp8) {
+      if (fmt == kFp8E4m3)
+        return {nt <= 16 ? &k_matmul_fp8<kFp8E4m3, DT, 1> : nt <= 32 ? &k_matmul_fp8<kFp8E4m3, DT, 2> : &k_matmul_fp8<kFp8E4m3, DT, 4>,
+                &k_matmul_reduce<DT>};
+      return {nt <= 16 ? &k_matmul_fp8<kFp8E5m2, DT, 1> : nt <= 32 ? &k_matmul_fp8<kFp8E5m2, DT, 2> : &k_matmul_fp8<kFp8E5m2, DT, 4>,
+              &k_matmul_reduce<DT>};
+    }
   }
   return {nt <= 1   ? matvec_kernel<DT, 1>(kind, fmt)
           : nt <= 2 ? matvec_kernel<DT, 2>(kind, fmt)
@@ -1582,7 +1592,7 @@ int product_scratch_size(ProductKind kind, const zipnn_b200_decode_plan* plan, i
   return ZIPNN_B200_OK;
 }
 
-// The weight format and scale grid of the fp8 matvec and dequantize (fp8_args_ok has checked all but the pointer).
+// The weight format and scale grid of the fp8 matvec, matmul and dequantize (fp8_args_ok has checked all but the pointer).
 struct Fp8Scale {
   int format;
   const float* d_scale;
@@ -1698,6 +1708,21 @@ int zipnn_b200_decode_plan_matvec_fp8(const zipnn_b200_decode_plan* plan, int it
   const Fp8Scale f8{fp8_format, d_scale, block_rows, block_cols};
   if (!fp8_args_ok(f8)) return ZIPNN_B200_E_ARG;
   return product(kMatvecFp8, plan, item, x_dtype, in_features, d_x, x_stride, n_tokens, d_bias, d_y, y_stride, d_scratch, scratch_bytes,
+                 (cudaStream_t)cuda_stream, &f8);
+}
+
+int zipnn_b200_decode_plan_matmul_fp8_scratch_size(const zipnn_b200_decode_plan* plan, int item, size_t in_features, size_t n_tokens,
+                                                   size_t* out) {
+  return product_scratch_size(kMatmulFp8, plan, item, kMvBf16, in_features, n_tokens, out);
+}
+
+int zipnn_b200_decode_plan_matmul_fp8(const zipnn_b200_decode_plan* plan, int item, int fp8_format, int x_dtype, size_t in_features,
+                                      const void* d_x, size_t x_stride, size_t n_tokens, const float* d_scale, size_t block_rows,
+                                      size_t block_cols, const void* d_bias, void* d_y, size_t y_stride, void* d_scratch,
+                                      size_t scratch_bytes, void* cuda_stream) {
+  const Fp8Scale f8{fp8_format, d_scale, block_rows, block_cols};
+  if (!fp8_args_ok(f8)) return ZIPNN_B200_E_ARG;
+  return product(kMatmulFp8, plan, item, x_dtype, in_features, d_x, x_stride, n_tokens, d_bias, d_y, y_stride, d_scratch, scratch_bytes,
                  (cudaStream_t)cuda_stream, &f8);
 }
 

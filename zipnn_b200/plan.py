@@ -50,6 +50,7 @@ class _Product(NamedTuple):
 _MATVEC = _Product("matvec", MATVEC_MAX_TOKENS, _MATVEC_DTYPES, None, False)
 _MATMUL = _Product("matmul", MATMUL_MAX_TOKENS, {dt: _MATVEC_DTYPES[dt] for dt in _MATMUL_DTYPES}, None, False)
 _MATVEC_FP8 = _Product("matvec_fp8", MATVEC_MAX_TOKENS, _FP8_FORMATS, _MATMUL_DTYPES, True)
+_MATMUL_FP8 = _Product("matmul_fp8", MATMUL_MAX_TOKENS, _FP8_FORMATS, _MATMUL_DTYPES, True)
 
 
 def _round(n: int, a: int) -> int:
@@ -464,6 +465,26 @@ class DecodePlan:
         -> out.  ValueError for an output `matvec_fp8_ok` refuses.  Works without the plan's output buffer."""
         return self._product(_MATVEC_FP8, k, x, bias, out, scratch, scale=scale, block=block)
 
+    def matmul_fp8_ok(self, k: int, in_features: int) -> bool:
+        """Can `matmul_fp8` multiply by output `k` seen as rows of `in_features` elements?  What `matvec_fp8_ok`
+        accepts.  Never raises for an output that exists."""
+        return self._ok(_MATMUL_FP8, k, in_features)
+
+    def matmul_fp8_scratch_bytes(self, k: int, in_features: int, n_tokens: int = MATMUL_MAX_TOKENS) -> int:
+        """Bytes of a matmul_fp8 scratch for output `k`, rows of `in_features` elements and `n_tokens` rows of x."""
+        return self._scratch_bytes(_MATMUL_FP8, k, in_features, n_tokens)
+
+    def matmul_fp8(self, k: int, x: torch.Tensor, scale: torch.Tensor, block: tuple = None, bias: torch.Tensor = None,
+                   out: torch.Tensor = None, scratch: torch.Tensor = None) -> torch.Tensor:
+        """`matvec_fp8` for up to MATMUL_MAX_TOKENS rows of x, on tensor cores (zipnn_b200_decode_plan_matmul_fp8): the
+        same arguments and rules, with `matmul_fp8_ok` and `matmul_fp8_scratch_bytes` in place of the matvec's.  Each
+        weight is dequantized to x's dtype exactly as `dequant_fp8` writes it, D = dtype(float(W) * S), and the products
+        and sums are the tensor cores' in fp32 (as `matmul`'s), each result rounded once: F.linear(x, D) up to the order
+        of the fp32 sums, never writing D.  Two calls with the same inputs give the same bits.  x must be finite: an
+        infinity may give NaN where the dense product gives one.  An e4m3fn NaN, an e5m2 infinity or NaN, or an fp16
+        overflow in D gives NaN or an infinity in that row, as F.linear of D does."""
+        return self._product(_MATMUL_FP8, k, x, bias, out, scratch, scale=scale, block=block)
+
     def _fp8_grid(self, name: str, in_features: int, scale, block, out_features: int) -> tuple:
         """-> (bn, bk) after checking `scale` against the grid the block implies (for method `name`)."""
         if not (isinstance(scale, torch.Tensor) and scale.is_cuda and scale.device == self.device and scale.dtype == torch.float32
@@ -516,7 +537,7 @@ class DecodePlan:
         return out
 
     def _product(self, kind: _Product, k: int, x, bias, out, scratch, scale=None, block=None) -> torch.Tensor:
-        """matvec, matmul and matvec_fp8: the checks and the call."""
+        """matvec, matmul, matvec_fp8 and matmul_fp8: the checks and the call."""
         name = kind.name
         wdt, total = self._product_item(k)
         dt = x.dtype if kind.x_dtypes and isinstance(x, torch.Tensor) and x.dtype in kind.x_dtypes else wdt

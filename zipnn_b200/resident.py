@@ -109,11 +109,14 @@ class _Options(NamedTuple):
     matmul: int    # the most input rows a matmul module multiplies without decoding (0: none)
     experts: bool
     fp8: bool
+    fp8_matmul: int  # the most input rows an "fp8" module multiplies on tensor cores without dequantizing (0: none)
 
 
-def _options(prefetch=False, gather=False, matvec=0, matmul=0, experts=False, fp8=False) -> _Options:
-    """ValueError for a row count out of range and for a mode that does not combine with prefetch=True."""
-    for name, n, limit in (("matvec", matvec, MATVEC_MAX_TOKENS), ("matmul", matmul, MATMUL_MAX_TOKENS)):
+def _options(prefetch=False, gather=False, matvec=0, matmul=0, experts=False, fp8=False, fp8_matmul=0) -> _Options:
+    """ValueError for a row count out of range, for fp8_matmul without fp8=True and for a mode that does not combine
+    with prefetch=True."""
+    for name, n, limit in (("matvec", matvec, MATVEC_MAX_TOKENS), ("matmul", matmul, MATMUL_MAX_TOKENS),
+                           ("fp8_matmul", fp8_matmul, MATMUL_MAX_TOKENS)):
         if not (isinstance(n, int) and 0 <= n <= limit):
             raise ValueError(f"{name} must be an integer from 0 to {limit}, not {n!r}")
         if n and prefetch:
@@ -123,7 +126,9 @@ def _options(prefetch=False, gather=False, matvec=0, matmul=0, experts=False, fp
                          "before its router has picked the experts")
     if fp8 and prefetch:
         raise ValueError("fp8=True and prefetch=True do not combine yet: the prefetch schedule decodes every module")
-    return _Options(bool(prefetch), bool(gather), matvec, matmul, bool(experts), bool(fp8))
+    if fp8_matmul and not fp8:
+        raise ValueError("fp8_matmul applies to the fp8 modules of fp8=True: pass fp8=True with it")
+    return _Options(bool(prefetch), bool(gather), matvec, matmul, bool(experts), bool(fp8), fp8_matmul)
 
 
 class _Entry(NamedTuple):
@@ -157,6 +162,9 @@ class _Resident:
         self.select_scratch = None     # the "experts" modules' run_select scratch, sized for the largest
         self.fp8_scratch = None        # the "fp8" modules' matvec_fp8 scratch and what the largest needs of it
         self.fp8_scratch_bytes = 0
+        self.fp8_matmul = 0            # fp8_matmul=N: the most input rows an "fp8" module multiplies by matmul_fp8
+        self.fp8_matmul_scratch = None  # the "fp8" modules' matmul_fp8 scratch and what the largest needs of it
+        self.fp8_matmul_scratch_bytes = 0
 
 
 def _grad_mode_error(mod, shared: bool = False):
@@ -298,8 +306,8 @@ def _decoded(mod, plan, names, forward):
 def _fp8_forward(mod, state, plan, k, names, fast: bool):
     """The forward of an fp8 linear module (W8A16: the activations are not quantized).  A bf16 / fp16 input on the plan's
     device, outside autocast, is multiplied with the dequantized weight S * W: at most `state.matvec` rows by
-    `plan.matvec_fp8`, more by `plan.dequant_fp8` into the shared output buffer and F.linear; the bias is added as
-    FP8Linear.forward adds it.  A module whose weight `fast` is False for (`matvec_fp8_ok` refuses it) decodes it and
+    `plan.matvec_fp8`, more and at most `state.fp8_matmul` by `plan.matmul_fp8`, more by `plan.dequant_fp8` into the
+    shared output buffer and F.linear; the bias is added as FP8Linear.forward adds it.  A module whose weight `fast` is False for (`matvec_fp8_ok` refuses it) decodes it and
     dequantizes in torch into a fresh tensor instead (the fp8 bytes occupy the shared buffer), with the same result.
     Any other input takes the decode, bind, module's own forward, unbind of the other compressed modules."""
     decoded = _decoded(mod, plan, names, type(mod).forward)
@@ -316,6 +324,8 @@ def _fp8_forward(mod, state, plan, k, names, fast: bool):
             scale = mod.weight_scale_inv
             if fast and rows is not None and rows <= state.matvec:
                 y = plan.matvec_fp8(k, input, scale, block, scratch=state.fp8_scratch)
+            elif fast and rows is not None and rows <= state.fp8_matmul:
+                y = plan.matmul_fp8(k, input, scale, block, scratch=state.fp8_matmul_scratch)
             else:
                 if fast:
                     w = plan.dequant_fp8(k, shape[1], scale, block, input.dtype, out=plan._out[:nbytes].view(input.dtype).view(shape))
@@ -514,6 +524,10 @@ def _commit(module: torch.nn.Module, state: _Resident, opts: _Options) -> None:
     if fp8 and opts.matvec:
         state.fp8_scratch_bytes = max(e.plan.matvec_fp8_scratch_bytes(0, e.module.in_features, opts.matvec) for e in fp8)
         state.fp8_scratch = _plans_scratch_or_own(state, state.fp8_scratch_bytes)
+    state.fp8_matmul = opts.fp8_matmul
+    if fp8 and opts.fp8_matmul:
+        state.fp8_matmul_scratch_bytes = max(e.plan.matmul_fp8_scratch_bytes(0, e.module.in_features, opts.fp8_matmul) for e in fp8)
+        state.fp8_matmul_scratch = _plans_scratch_or_own(state, state.fp8_matmul_scratch_bytes)
     for key, (m, plan, names, mode) in enumerate(state.entries):
         if mode in ("matvec", "matmul"):   # no hooks: its forward decides per input whether anything is decoded
             m.__dict__["forward"] = _matvec_forward(m, state, plan, 0, names, plan.outputs[0].dtype, plan.device,
@@ -537,7 +551,7 @@ def _commit(module: torch.nn.Module, state: _Resident, opts: _Options) -> None:
 
 
 def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = False, gather: bool = False, matvec: int = 0,
-                    matmul: int = 0, experts: bool = False, fp8: bool = False) -> dict:
+                    matmul: int = 0, experts: bool = False, fp8: bool = False, fp8_matmul: int = 0) -> dict:
     """Compress the weights of `modules` (default: every submodule that directly owns bf16 / fp16 / fp32 / fp8
     parameters) into streams kept in HBM, decoded just before each module's forward.  All parameters are compressed
     in one `compress_batch` call and must be on one CUDA device.
@@ -596,10 +610,19 @@ def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = Fals
     bit F.linear of torch's dequantize), then the bias is added as FP8Linear adds it.  So fp8=True, matvec=8 is the
     decode-time setting.  A weight that `DecodePlan.matvec_fp8_ok` refuses (a constant one, say) is decoded and
     dequantized in torch instead, with the same result.  Other inputs decode and run the module's own forward.  The
-    shared output buffer holds at least twice the largest such weight's bytes.  `matmul` does not apply to fp8 weights.
+    shared output buffer holds at least twice the largest such weight's bytes.  `matmul` does not apply to fp8 weights;
+    `fp8_matmul` (below) is their tensor-core path.
     The report gains "fp8_modules" and "fp8_scratch_bytes" (the matvec_fp8 scratch, the plans' one when it is large
-    enough).  ValueError together with prefetch=True."""
-    opts = _options(prefetch, gather, matvec, matmul, experts, fp8)
+    enough).  ValueError together with prefetch=True.
+
+    fp8_matmul=N (0 .. MATMUL_MAX_TOKENS; 0, the default, changes nothing): with fp8=True, an fp8 module whose weight
+    `DecodePlan.matvec_fp8_ok` accepts computes bf16 / fp16 inputs of more than `matvec` rows and at most N as
+    `DecodePlan.matmul_fp8` (tensor cores, two launches, the weight neither dequantized into the shared buffer nor
+    read back): F.linear of the same dequantized weight, with the fp32 sums in another order.  Inputs of at most
+    `matvec` rows still take matvec_fp8, larger ones dequant_fp8 + F.linear.  The report gains "fp8_matmul_modules" and
+    "fp8_matmul_scratch_bytes" (one scratch for all of them, the plans' one when it is large enough).  ValueError
+    without fp8=True and together with prefetch=True."""
+    opts = _options(prefetch, gather, matvec, matmul, experts, fp8, fp8_matmul)
     if getattr(module, _ATTR, None) is not None:
         raise ValueError("compress_module: this module is already compressed")
     modules, groups = select(module, modules)
@@ -641,6 +664,8 @@ def _with_prefetch(report: dict, state, opts: _Options) -> dict:
                       experts_scratch_bytes=0 if state.select_scratch is None else state.select_scratch.numel())
     if opts.fp8:
         report.update(fp8_modules=modes.count("fp8") + modes.count("fp8_torch"), fp8_scratch_bytes=state.fp8_scratch_bytes)
+    if opts.fp8_matmul:
+        report.update(fp8_matmul_modules=modes.count("fp8"), fp8_matmul_scratch_bytes=state.fp8_matmul_scratch_bytes)
     return report
 
 
@@ -916,7 +941,8 @@ def _load_device(plan: LoadPlan, dev, opts: _Options) -> tuple:
 
 
 def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None, prefetch: bool = False,
-                gather: bool = False, matvec: int = 0, matmul: int = 0, experts: bool = False, fp8: bool = False) -> dict:
+                gather: bool = False, matvec: int = 0, matmul: int = 0, experts: bool = False, fp8: bool = False,
+                fp8_matmul: int = 0) -> dict:
     """Load a checkpoint into `module` with the weights of `modules` kept compressed on `device`: the state
     `compress_module` leaves (same selection rules, hooks, plans and report), reached without a dense copy of those
     weights on the GPU.
@@ -951,10 +977,10 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None,
     and the batched decode's workspace; plain entries add one group at a time: its input, its streams' bound and the
     compress workspace.  A model loaded from .znn files never has its compressed weights dense on the device.
 
-    prefetch, gather, matvec, matmul, experts, fp8: as for `compress_module`.
+    prefetch, gather, matvec, matmul, experts, fp8, fp8_matmul: as for `compress_module`.
 
     -> the report of `compress_module`."""
-    opts = _options(prefetch, gather, matvec, matmul, experts, fp8)
+    opts = _options(prefetch, gather, matvec, matmul, experts, fp8, fp8_matmul)
     dev = _cuda_device(device)
     if dev is None:
         raise ValueError(f"load_module: {device!r} is not a CUDA device")
