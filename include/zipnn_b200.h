@@ -374,6 +374,37 @@ int zipnn_b200_decode_plan_dequant_fp8(const zipnn_b200_decode_plan* plan, int i
                                        size_t in_features, const float* d_scale, size_t block_rows, size_t block_cols,
                                        void* d_out, void* cuda_stream);
 
+/* _dequant_fp8_select: _dequant_fp8 restricted to the slices that ids select, the selected run of _run_select with
+ * _dequant_fp8's stores (the routed experts of an fp8 mixture-of-experts layer: gate_up_proj [E, 2I, H] and down_proj
+ * [E, H, I] with a scale grid per expert).  Every item is `rows` slices along dim 0 (E experts); item i is seen as
+ * rows * out_i rows of items[i].in_features elements, slice e its rows [e * out_i, (e + 1) * out_i), and
+ * items[i].d_out is a contiguous [rows * out_i][in_features] tensor of out_dtype (ZIPNN_B200_MATVEC_BF16 or _FP16),
+ * 16-byte aligned.  items[i].d_scale is the contiguous fp32 [rows][ceil(out_i / bn)][ceil(in / bk)] of the per-slice
+ * grids, (bn, bk) = (block_rows, block_cols) clamped to (out_i, in_features) as for _dequant_fp8: (out_i, in) is one
+ * scale per slice.  For every chunk of an item that meets a selected slice, every element of the chunk is written,
+ * d_out[r][c] = out_dtype(float(W[r][c]) * S[r / out_i][(r % out_i) / bn][c / bk]): bit for bit torch's dequantize of
+ * each slice, as _dequant_fp8 writes it.  A chunk that straddles two slices writes its neighbour's elements too (with
+ * their own scales), and no other element of any d_out is written.
+ * Three launches whatever the id values are (the index kernel of _run_select, the replay decoder with the dequantizing
+ * stores, the plan run's error pass), no copy and no host read but the first call's read of each item's chunk modes:
+ * capturable in a CUDA graph, replayable with new ids and new scales.  Ids, the scratch (_select_scratch_size bytes,
+ * not the plan's own scratch), E_INDEX and n_ids == 0 as for _run_select.
+ * Eligible plans (else E_UNSUPPORTED): those _run_select takes, with at most 4 items, each of which _dequant_fp8 takes
+ * (fused fp8 chunks, in_features a multiple of 16); all items in one fp8_format.
+ * Host-side rejections launch and write nothing: E_ARG as _run_select refuses rows, ids and scratch, as _dequant_fp8
+ * refuses fp8_format, out_dtype, in_features, the blocks, d_scale and d_out, for NULL items, n_items other than the
+ * plan's item count, and an item whose slices are not whole rows. */
+typedef struct zipnn_b200_fp8_select_item {
+  size_t in_features;
+  const float* d_scale;
+  size_t block_rows, block_cols;
+  void* d_out;
+} zipnn_b200_fp8_select_item;
+int zipnn_b200_decode_plan_dequant_fp8_select(const zipnn_b200_decode_plan* plan, size_t rows, const void* d_ids,
+                                              size_t n_ids, int id_bytes, int fp8_format, int out_dtype, int n_items,
+                                              const zipnn_b200_fp8_select_item* items, void* d_scratch,
+                                              size_t scratch_bytes, void* cuda_stream);
+
 /* ---- stage 1 alone ------------------------------------------------------------ */
 /* d_planes: num_buf planes of `stride` bytes each; plane g receives byte g of every element
  * of the (optionally rotated) input.  Lengths as in the reference: n/num_buf, the first

@@ -47,6 +47,12 @@ class CompressItem(C.Structure):
                 ("threshold", C.c_float), ("d_out", C.c_void_p), ("out_cap", C.c_size_t)]
 
 
+class Fp8SelectItem(C.Structure):
+    """zipnn_b200_fp8_select_item (include/zipnn_b200.h)."""
+    _fields_ = [("in_features", C.c_size_t), ("d_scale", C.c_void_p), ("block_rows", C.c_size_t), ("block_cols", C.c_size_t),
+                ("d_out", C.c_void_p)]
+
+
 class DecodePlanStruct(C.Structure):
     """zipnn_b200_decode_plan (include/zipnn_b200.h): host memory, filled by zipnn_b200_decode_plan_create."""
     _fields_ = [("opaque", C.c_uint64 * 16)]
@@ -132,6 +138,8 @@ def lib() -> C.CDLL:
                 "zipnn_b200_decode_plan_matmul_fp8": (i32, [C.POINTER(DecodePlanStruct), i32, i32, i32, sz, vp, sz, sz, vp, sz, sz, vp, vp, sz,
                                                              vp, sz, vp]),
                 "zipnn_b200_decode_plan_dequant_fp8": (i32, [C.POINTER(DecodePlanStruct), i32, i32, i32, sz, vp, sz, sz, vp, vp]),
+                "zipnn_b200_decode_plan_dequant_fp8_select": (i32, [C.POINTER(DecodePlanStruct), sz, vp, sz, i32, i32, i32, i32,
+                                                                    C.POINTER(Fp8SelectItem), vp, sz, vp]),
                 "zipnn_b200_split": (i32, [vp, sz, i32, i32, vp, sz, vp]),
                 "zipnn_b200_regroup": (i32, [vp, sz, sz, i32, i32, vp, vp]),
                 "zipnn_b200_compress_host": (i32, [vp, sz, vp, sz, i32, i32, i32, sz, C.c_float, vp, sz, szp]),
@@ -161,7 +169,7 @@ EXPORTS = [
     "zipnn_b200_decode_plan_matmul_scratch_size", "zipnn_b200_decode_plan_matmul",
     "zipnn_b200_decode_plan_matvec_fp8_scratch_size", "zipnn_b200_decode_plan_matvec_fp8",
     "zipnn_b200_decode_plan_matmul_fp8_scratch_size", "zipnn_b200_decode_plan_matmul_fp8",
-    "zipnn_b200_decode_plan_dequant_fp8", "zipnn_b200_split", "zipnn_b200_regroup", "zipnn_b200_compress_host", "zipnn_b200_decompress_host",
+    "zipnn_b200_decode_plan_dequant_fp8", "zipnn_b200_decode_plan_dequant_fp8_select", "zipnn_b200_split", "zipnn_b200_regroup", "zipnn_b200_compress_host", "zipnn_b200_decompress_host",
     "zipnn_b200_timing_enable", "zipnn_b200_timing_kernel_count", "zipnn_b200_timing_kernel_name",
     "zipnn_b200_timing_collect",
 ]

@@ -59,6 +59,10 @@ struct ProductCfg {
   const float* scale;
   uint64_t srow, scol;
   uint32_t scols;
+  // the selected dequantize's per-slice grid (k_select_dequant_fp8, select.cuh): the tensor is `rows` slices of
+  // slice_rows rows, each with a grid of its own of slice_grid scales; slice s of row r is matvec_fp8_div(r, sslice)
+  uint64_t sslice;
+  uint32_t slice_rows, slice_grid;
 };
 
 // Elements of a block of a chunk with n elements: a quarter's vectors split over 8 warps, in whole 32-vector steps.
@@ -353,7 +357,10 @@ __device__ __forceinline__ uint4 fp8_dequant8(uint32_t a, uint32_t b, float sc) 
 // by multiply-highs (every element index is below 2^31: the host admits total <= INT32_MAX).  A lane converts its 16
 // bytes, multiplies each by the block's one scale (bk % 16 == 0, in % 16 == 0: the vector lies in one row and block)
 // and stores 32 bytes.
-template <int FMT, int ODT>
+// SLICED: the scale grid is one grid per slice [e] of a tensor [rows][slice_rows][in] (fp8 experts, whose slice rows
+// need not be a multiple of bn): the slice comes first, s = row / slice_rows, then the block of row - s * slice_rows
+// in the slice's grid at s * slice_grid.  The selected dequantize (select.cuh) only.
+template <int FMT, int ODT, bool SLICED = false>
 struct DequantEp {
   static_assert(ODT == kMvBf16 || ODT == kMvFp16, "bf16 or fp16 out");
   static constexpr bool on = true;
@@ -368,7 +375,13 @@ struct DequantEp {
       uint32_t r[4];
       ZB_FUSED_VECTOR(G, S, out_off, o, rot, r);
       const uint32_t e = e0 + o, row = matvec_fp8_div(e, rin), col = e - row * in;
-      const float sc = __ldg(m.scale + matvec_fp8_div(row, m.srow) * m.scols + matvec_fp8_div(col, m.scol));
+      float sc;
+      if constexpr (SLICED) {
+        const uint32_t s = matvec_fp8_div(row, m.sslice), r = row - s * m.slice_rows;
+        sc = __ldg(m.scale + s * m.slice_grid + matvec_fp8_div(r, m.srow) * m.scols + matvec_fp8_div(col, m.scol));
+      } else {
+        sc = __ldg(m.scale + matvec_fp8_div(row, m.srow) * m.scols + matvec_fp8_div(col, m.scol));
+      }
       const uint4 lo = fp8_dequant8<FMT, ODT>(r[0], r[1], sc), hi = fp8_dequant8<FMT, ODT>(r[2], r[3], sc);
       uint4* const dst = reinterpret_cast<uint4*>(m.y) + (e >> 3);
       dst[0] = lo;

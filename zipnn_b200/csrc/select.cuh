@@ -13,6 +13,7 @@
 //   k_select_regroup   regroup_tile over the selected tiles;
 //   k_select_overflow  decode_overflow_part over the selected overflow chunks, on the plan's overflow plane slots;
 //   (k_batch_errors    as after a plan run.)
+// k_select_dequant_fp8 (below) is k_select_sync for fp8 experts with k_dequant_fp8's dequantizing stores.
 // Grids come from bounds the host knows (ids, the most chunks a slice can touch, resident CTAs), never from the ids,
 // so the launch sequence is fixed and a selected run can be captured in a CUDA graph and replayed with new ids.
 // A chunk that straddles two slices is decoded whole; no byte of a chunk that meets no selected slice is written.
@@ -21,6 +22,7 @@
 #pragma once
 #include "decode_sync.cuh"
 #include "gather.cuh"
+#include "matvec.cuh"
 
 namespace zb {
 
@@ -158,6 +160,33 @@ __global__ void __launch_bounds__(kSyncThreads, 3) k_select_sync(BatchCfg B, Seg
     const uint64_t work = 4ull * e.y + (w & 3);
     __syncthreads();  // the previous unit's shared state is dead
     sync_process_any<false, kSyncReplay>(cfg, S, cv, work, X.seg + X.base[e.x] + work * kSyncThreads);
+  }
+}
+
+// ---- the selected fp8 dequantize (k_select_dequant_fp8) -----------------------------------------------------------
+// A selected run of a plan whose items are fp8 experts (every chunk fused, G = 1) with k_dequant_fp8's stores in place
+// of the run's: the bitstreams k_select_index picked are decoded by the replay decoder, and DequantEp (matvec.cuh, the
+// per-slice grid) writes each 16-byte vector dequantized to item t's d.m[t].y.  Fused items have no regroup tiles and
+// no overflow chunks, so only hsel matters; a call is k_select_index, this kernel and k_batch_errors.  The items'
+// ProductCfgs are a kernel parameter (no copy to the device per call): a graph replays with new ids and new scales.
+constexpr int kSelectFp8MaxItems = 4;
+struct SelectFp8Items {
+  ProductCfg m[kSelectFp8MaxItems];  // per plan item, in item order
+};
+
+template <int FMT, int ODT>
+__global__ void __launch_bounds__(kSyncThreads, 3) k_select_dequant_fp8(SelectCfg s, const __grid_constant__ SelectFp8Items d) {
+  extern __shared__ __align__(1024) unsigned char smem_raw[];
+  const SyncCarve cv = sync_carve(smem_raw);
+  SyncShared& S = *cv.S;
+  const uint64_t units = 4ull * *s.count;
+  for (uint64_t w = blockIdx.x; w < units; w += gridDim.x) {
+    const uint2 e = s.hsel[w >> 2];
+    const DequantEp<FMT, ODT, true> ep{d.m[e.x]};
+    const uint64_t work = 4ull * e.y + (w & 3);
+    __syncthreads();  // the previous unit's shared state is dead
+    sync_process<1, false, kSyncReplay, false, DequantEp<FMT, ODT, true>>(*ep.m.cfg, nullptr, S, cv.lut, cv.lut_s, work,
+                                                                         ep.m.seg + work * kSyncThreads, nullptr, &ep);
   }
 }
 

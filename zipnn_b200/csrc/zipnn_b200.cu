@@ -1404,6 +1404,38 @@ int select_items(const zipnn_b200_decode_plan* plan, size_t rows, PlanState& s, 
     if (rows == 0 || gi.orig % rows) return ZIPNN_B200_E_ARG;
   return ZIPNN_B200_OK;
 }
+// The host checks of the ids and the scratch that both selected calls make once the items passed: E_ARG or OK.
+int select_args_ok(const SelectLayout& L, const void* d_ids, size_t n_ids, int id_bytes, const void* d_scratch, size_t scratch_bytes) {
+  if (!d_ids || !d_scratch || ((uintptr_t)d_ids % (uintptr_t)id_bytes) || ((uintptr_t)d_scratch & 255)) return ZIPNN_B200_E_ARG;
+  if (n_ids > (1ull << 40)) return ZIPNN_B200_E_ARG;
+  return scratch_bytes < L.bytes ? ZIPNN_B200_E_ARG : ZIPNN_B200_OK;
+}
+SelectCfg select_cfg(const PlanState& s, const SelectLayout& L, uint8_t* ws, size_t rows, const void* d_ids, size_t n_ids, int id_bytes) {
+  SelectCfg sel;
+  sel.ids = d_ids;
+  sel.n = n_ids;
+  sel.id8 = id_bytes == 8;
+  sel.rows = rows;
+  sel.error = s.B.error_out;
+  sel.count = (uint32_t*)ws;
+  sel.ocfg = (DecodeCfg*)(ws + L.ocfg_off);
+  sel.octrl = (Ctrl*)(ws + L.octrl_off);
+  sel.hsel = (uint2*)(ws + L.hsel_off);
+  sel.tsel = (uint2*)(ws + L.tsel_off);
+  sel.osel = (uint32_t*)(ws + L.osel_off);
+  return sel;
+}
+// Grids from bounds of n alone: an item's touched chunks are at most min(n * span, K).  -> the bitstreams and regroup
+// tiles of every item's touched chunks, and the most touched chunks of one item.
+void select_bounds(const std::vector<GatherItem>& items, size_t rows, size_t n_ids, uint64_t& bitstreams, uint64_t& tiles, uint64_t& most) {
+  for (const GatherItem& gi : items) {
+    const uint64_t span = gather_span(gi.orig / rows, gi.chunk, gi.K);
+    const uint64_t m = n_ids > gi.K / span ? gi.K : std::min<uint64_t>(gi.K, n_ids * span);
+    bitstreams += 4ull * gi.G * m;
+    tiles += m * ((gi.chunk + kMergeTile - 1) / kMergeTile);
+    most = std::max(most, m);
+  }
+}
 }  // namespace
 
 int zipnn_b200_decode_plan_select_scratch_size(const zipnn_b200_decode_plan* plan, size_t rows, size_t* out) {
@@ -1426,33 +1458,15 @@ int zipnn_b200_decode_plan_run_select(const zipnn_b200_decode_plan* plan, size_t
     if (rc) return rc;
   }
   if (n_ids == 0) return ZIPNN_B200_OK;
-  if (!d_ids || !d_scratch || ((uintptr_t)d_ids % (uintptr_t)id_bytes) || ((uintptr_t)d_scratch & 255)) return ZIPNN_B200_E_ARG;
-  if (n_ids > (1ull << 40)) return ZIPNN_B200_E_ARG;
   const SelectLayout L = select_layout(s);
-  if (scratch_bytes < L.bytes) return ZIPNN_B200_E_ARG;
-  cudaStream_t st = (cudaStream_t)cuda_stream;
-  uint8_t* ws = (uint8_t*)d_scratch;
-  SelectCfg sel;
-  sel.ids = d_ids;
-  sel.n = n_ids;
-  sel.id8 = id_bytes == 8;
-  sel.rows = rows;
-  sel.error = s.B.error_out;
-  sel.count = (uint32_t*)ws;
-  sel.ocfg = (DecodeCfg*)(ws + L.ocfg_off);
-  sel.octrl = (Ctrl*)(ws + L.octrl_off);
-  sel.hsel = (uint2*)(ws + L.hsel_off);
-  sel.tsel = (uint2*)(ws + L.tsel_off);
-  sel.osel = (uint32_t*)(ws + L.osel_off);
-  // grids from bounds of n alone: an item's touched chunks are at most min(n * span, K)
-  uint64_t bitstreams = 0, tiles = 0, most = 0;
-  for (const GatherItem& gi : items) {
-    const uint64_t span = gather_span(gi.orig / rows, gi.chunk, gi.K);
-    const uint64_t m = n_ids > gi.K / span ? gi.K : std::min<uint64_t>(gi.K, n_ids * span);
-    bitstreams += 4ull * gi.G * m;
-    tiles += m * ((gi.chunk + kMergeTile - 1) / kMergeTile);
-    most = std::max(most, m);
+  {
+    const int rc = select_args_ok(L, d_ids, n_ids, id_bytes, d_scratch, scratch_bytes);
+    if (rc) return rc;
   }
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  const SelectCfg sel = select_cfg(s, L, (uint8_t*)d_scratch, rows, d_ids, n_ids, id_bytes);
+  uint64_t bitstreams = 0, tiles = 0, most = 0;
+  select_bounds(items, rows, n_ids, bitstreams, tiles, most);
   const unsigned sync_blocks = resident_grid(k_select_sync, kSyncSmemBytes, kSyncThreads, bitstreams);
   if (!sync_blocks) return ZIPNN_B200_E_CUDA;
   k_select_index<<<1, kGatherIndexThreads, 0, st>>>(s.B, sel);
@@ -1601,14 +1615,19 @@ struct Fp8Scale {
 bool fp8_args_ok(const Fp8Scale& f8) {
   return (f8.format == kFp8E4m3 || f8.format == kFp8E5m2) && f8.block_rows && f8.block_cols >= 16 && f8.block_cols % 16 == 0;
 }
-// ProductCfg's scale-grid fields.
-void fp8_grid(const Fp8Scale& f8, ProductCfg& m) {
+// ProductCfg's scale-grid fields.  slices > 1 (the selected dequantize): the weight is `slices` matrices of m.out / slices
+// rows, each with a grid of its own, back to back; the per-slice fields are set for any count (1: the whole matrix).
+void fp8_grid(const Fp8Scale& f8, ProductCfg& m, uint64_t slices = 1) {
+  const uint64_t out = m.out / slices;
   // a block at least as tall or wide as the matrix is the whole of it: clamped, bn and bk stay below 2^31
-  const uint64_t bn = std::min<uint64_t>(f8.block_rows, m.out), bk = std::min<uint64_t>(f8.block_cols, m.in);
+  const uint64_t bn = std::min<uint64_t>(f8.block_rows, out), bk = std::min<uint64_t>(f8.block_cols, m.in);
   m.scale = f8.d_scale;
   m.srow = matvec_fp8_recip(bn);
   m.scol = matvec_fp8_recip(bk);
   m.scols = (uint32_t)((m.in + bk - 1) / bk);
+  m.sslice = matvec_fp8_recip(out);
+  m.slice_rows = (uint32_t)out;
+  m.slice_grid = (uint32_t)((out + bn - 1) / bn * m.scols);
 }
 
 int product(ProductKind kind, const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, const void* d_x, size_t x_stride,
@@ -1731,6 +1750,55 @@ int zipnn_b200_decode_plan_dequant_fp8(const zipnn_b200_decode_plan* plan, int i
   const Fp8Scale f8{fp8_format, d_scale, block_rows, block_cols};
   if (!fp8_args_ok(f8)) return ZIPNN_B200_E_ARG;
   return dequant_fp8(plan, item, f8, out_dtype, in_features, d_out, (cudaStream_t)cuda_stream);
+}
+
+int zipnn_b200_decode_plan_dequant_fp8_select(const zipnn_b200_decode_plan* plan, size_t rows, const void* d_ids, size_t n_ids, int id_bytes,
+                                              int fp8_format, int out_dtype, int n_items, const zipnn_b200_fp8_select_item* items,
+                                              void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (id_bytes != 4 && id_bytes != 8) return ZIPNN_B200_E_ARG;
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  PlanState s;
+  std::vector<GatherItem> gis;
+  {
+    const int rc = select_items(plan, rows, s, gis);
+    if (rc) return rc;
+  }
+  if (!items || n_items <= 0 || (size_t)n_items != gis.size()) return ZIPNN_B200_E_ARG;
+  if (n_items > kSelectFp8MaxItems) return ZIPNN_B200_E_UNSUPPORTED;
+  SelectFp8Items d;
+  memset(&d, 0, sizeof(d));
+  for (int i = 0; i < n_items; i++) {
+    const zipnn_b200_fp8_select_item& it = items[i];
+    const Fp8Scale f8{fp8_format, it.d_scale, it.block_rows, it.block_cols};
+    if (!fp8_args_ok(f8)) return ZIPNN_B200_E_ARG;
+    ProductCfg& m = d.m[i];
+    const int rc = product_item(kMatvecFp8, plan, i, out_dtype, it.in_features, st, m);
+    if (rc) return rc;
+    if (m.out % rows) return ZIPNN_B200_E_ARG;  // a slice is whole rows
+    if (!it.d_out || ((uintptr_t)it.d_out & 15) || !it.d_scale || ((uintptr_t)it.d_scale & 3)) return ZIPNN_B200_E_ARG;
+    m.y = it.d_out;
+    fp8_grid(f8, m, rows);
+  }
+  if (n_ids == 0) return ZIPNN_B200_OK;
+  const SelectLayout L = select_layout(s);
+  {
+    const int rc = select_args_ok(L, d_ids, n_ids, id_bytes, d_scratch, scratch_bytes);
+    if (rc) return rc;
+  }
+  const SelectCfg sel = select_cfg(s, L, (uint8_t*)d_scratch, rows, d_ids, n_ids, id_bytes);
+  uint64_t bitstreams = 0, tiles = 0, most = 0;
+  select_bounds(gis, rows, n_ids, bitstreams, tiles, most);
+  const bool e4 = fp8_format == kFp8E4m3;
+  void (*const k)(SelectCfg, const SelectFp8Items) =
+      out_dtype == kMvBf16 ? (e4 ? &k_select_dequant_fp8<kFp8E4m3, kMvBf16> : &k_select_dequant_fp8<kFp8E5m2, kMvBf16>)
+                           : (e4 ? &k_select_dequant_fp8<kFp8E4m3, kMvFp16> : &k_select_dequant_fp8<kFp8E5m2, kMvFp16>);
+  const unsigned blocks = resident_grid(k, kSyncSmemBytes, kSyncThreads, bitstreams);
+  if (!blocks) return ZIPNN_B200_E_CUDA;
+  k_select_index<<<1, kGatherIndexThreads, 0, st>>>(s.B, sel);
+  ZB_LAUNCHED();
+  k<<<blocks, kSyncThreads, kSyncSmemBytes, st>>>(sel, d);
+  ZB_LAUNCHED();
+  return batch_errors(s.B, st);
 }
 
 int zipnn_b200_split(const void* d_in, size_t n, int num_buf, int bits_mode, void* d_planes, size_t stride,

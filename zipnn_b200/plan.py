@@ -33,6 +33,7 @@ MATMUL_MAX_TOKENS = _native.MATMUL_MAX_TOKENS
 _MATVEC_DTYPES = {torch.bfloat16: 0, torch.float16: 1, torch.float32: 2}   # ZIPNN_B200_MATVEC_*
 _MATMUL_DTYPES = (torch.bfloat16, torch.float16)
 _FP8_FORMATS = {torch.float8_e4m3fn: _native.FP8_E4M3, torch.float8_e5m2: _native.FP8_E5M2}   # ZIPNN_B200_FP8_*
+_SELECT_FP8_MAX_ITEMS = 4   # outputs of a plan dequant_fp8_select takes (kSelectFp8MaxItems)
 
 
 class _Product(NamedTuple):
@@ -485,21 +486,24 @@ class DecodePlan:
         overflow in D gives NaN or an infinity in that row, as F.linear of D does."""
         return self._product(_MATMUL_FP8, k, x, bias, out, scratch, scale=scale, block=block)
 
-    def _fp8_grid(self, name: str, in_features: int, scale, block, out_features: int) -> tuple:
-        """-> (bn, bk) after checking `scale` against the grid the block implies (for method `name`)."""
+    def _fp8_grid(self, name: str, in_features: int, scale, block, out_features: int, experts: int = 1) -> tuple:
+        """-> (bn, bk) after checking `scale` against the grid the block implies (for method `name`); `experts` > 1: a
+        weight [experts, out_features, in_features] with one grid per expert, back to back."""
         if not (isinstance(scale, torch.Tensor) and scale.is_cuda and scale.device == self.device and scale.dtype == torch.float32
                 and scale.is_contiguous()):
             raise ValueError(f"{name}'s scale must be a contiguous CUDA float32 tensor on the plan's device")
         if block is None:
-            if scale.numel() != 1:
-                raise ValueError(f"{name} takes block=None for a one-element scale only, not {scale.numel()} elements")
+            if scale.numel() != experts:
+                raise ValueError(f"{name} takes block=None for one scale per {'expert' if experts > 1 else 'tensor'} only, "
+                                 f"not {scale.numel()} elements")
             return out_features, in_features
         bn, bk = (int(b) for b in block)
         if bn < 1 or bk < 16 or bk % 16:
             raise ValueError(f"{name}'s block (bn, bk) needs bn >= 1 and bk a multiple of 16 of at least 16, not {(bn, bk)}")
-        grid = -(-out_features // bn) * -(-in_features // bk)
+        grid = experts * -(-out_features // bn) * -(-in_features // bk)
         if scale.numel() != grid:
-            raise ValueError(f"{name}'s scale for block {(bn, bk)} of a [{out_features}, {in_features}] weight has {grid} "
+            lead = f"{experts}, " if experts > 1 else ""
+            raise ValueError(f"{name}'s scale for block {(bn, bk)} of a [{lead}{out_features}, {in_features}] weight has {grid} "
                              f"elements, not {scale.numel()}")
         return bn, bk
 
@@ -535,6 +539,93 @@ class DecodePlan:
         if rc:
             _native.check(rc)
         return out
+
+    def dequant_fp8_select_ok(self, in_features) -> bool:
+        """Can `dequant_fp8_select` dequantize slices of this plan's outputs, output k seen as rows of `in_features[k]`
+        elements?  True when `select_ok` is, the plan has at most 4 outputs, all of one fp8 dtype, `matvec_fp8_ok(k,
+        in_features[k])` accepts each, and each slice [e] (along dim 0) is whole rows.  The first call for an output
+        synchronises (it reads the chunk modes); never raises."""
+        try:
+            inf = [int(i) for i in in_features]
+        except (TypeError, ValueError):
+            return False
+        if len(inf) != len(self._offs) or not 1 <= len(inf) <= _SELECT_FP8_MAX_ITEMS or not self.select_ok():
+            return False
+        if len({dt for _, _, dt, _ in self._offs}) != 1:
+            return False
+        for k, i in enumerate(inf):
+            _, _, dt, sh = self._offs[k]
+            if not self._ok(_MATVEC_FP8, k, i) or (math.prod(sh) // sh[0]) % i:
+                return False
+        return True
+
+    def dequant_fp8_select(self, ids: torch.Tensor, in_features, scales, blocks, dtype: torch.dtype = torch.bfloat16,
+                           outs=None, scratch: torch.Tensor = None) -> list:
+        """`dequant_fp8` of the slices [e] (along dim 0) that `ids` select, written straight from the coded streams of
+        the chunks that meet them (zipnn_b200_decode_plan_dequant_fp8_select): the routed experts of an fp8
+        mixture-of-experts layer, output k = an expert weight [E, out_k, in_k] with a scale grid per expert.  Every
+        element of a selected slice is bit for bit torch's `(W[e].to(torch.float32) * S[e]_expanded).to(dtype)`.  Each
+        chunk that meets a selected slice is written whole (a chunk that straddles slices writes its neighbours'
+        elements too, correctly); no other element of the outputs is written, so the slices that were not selected
+        hold whatever they held.  Three launches on the current CUDA stream, a fixed number, the ids never read on the
+        host: capturable in a CUDA graph and replayable with new ids and new scales.
+
+        ids:     CUDA int32 or int64 tensor of any shape on the plan's device; duplicates allowed; empty: nothing runs.
+        in_features: per output, in_k (its rows' elements).
+        scales:  per output, the contiguous CUDA float32 grid [E, ceil(out_k / bn), ceil(in_k / bk)] (any shape of that
+                 many elements), as transformers' `FP8Experts` holds it in `*_scale_inv`.
+        blocks:  per output, (bn, bk) as for `matvec_fp8`, or None: one scale per expert ([E, 1, 1]).
+        dtype:   bf16 or fp16.
+        outs:    optional list of contiguous 16-byte aligned tensors [E, out_k, in_k] of `dtype` on the plan's device.
+        scratch: as for `run_select` (at least `select_scratch_bytes()` bytes, not the plan's own scratch); default: a
+                 buffer kept by the plan.
+        -> the list of outputs.  An id outside [0, E) selects nothing and makes `check()` raise IndexError (sticky).
+        ValueError for a plan `dequant_fp8_select_ok` refuses, and for bad ids, scales, blocks, dtype or outs.  Works
+        without the plan's output buffer."""
+        name = "dequant_fp8_select"
+        self._check_ids(name, ids)
+        if dtype not in _MATMUL_DTYPES:
+            raise ValueError(f"{name} writes bf16 or fp16, not {dtype}")
+        inf = list(in_features) if isinstance(in_features, (list, tuple)) else None
+        if inf is None or not self.dequant_fp8_select_ok(inf):
+            raise ValueError(f"{name} cannot dequantize this plan's outputs with in_features {in_features} (see {name}_ok)")
+        inf = [int(i) for i in inf]
+        n_out = len(self._offs)
+        scales, blocks = list(scales), list(blocks)
+        if len(scales) != n_out or len(blocks) != n_out:
+            raise ValueError(f"{name} takes one scale and one block per output ({n_out})")
+        if outs is not None:
+            outs = list(outs)
+            if len(outs) != n_out:
+                raise ValueError(f"{name} takes one out per output ({n_out})")
+        E = self._offs[0][3][0]
+        arr = (_native.Fp8SelectItem * n_out)()
+        result = []
+        for k, (it, i) in enumerate(zip(arr, inf)):
+            wdt, total = self._product_item(k)
+            shape = (E, total // (E * i), i)
+            bn, bk = self._fp8_grid(name, i, scales[k], blocks[k], shape[1], experts=E)
+            out = None if outs is None else outs[k]
+            if out is None:
+                out = torch.empty(shape, dtype=dtype, device=self.device)
+            elif not (isinstance(out, torch.Tensor) and out.is_cuda and out.device == self.device and out.dtype == dtype
+                      and tuple(out.shape) == shape and out.is_contiguous() and out.data_ptr() % 16 == 0):
+                raise ValueError(f"{name}'s out {k} must be a contiguous 16-byte aligned {dtype} CUDA tensor of shape {shape} "
+                                 "on the plan's device")
+            it.in_features, it.d_scale, it.block_rows, it.block_cols, it.d_out = i, scales[k].data_ptr(), bn, bk, out.data_ptr()
+            result.append(out)
+        ids_c = ids.contiguous()
+        n = ids_c.numel()
+        if n == 0:
+            return result
+        scratch = self._scratch_for(name, scratch, self.select_scratch_bytes)
+        rc = _native.lib().zipnn_b200_decode_plan_dequant_fp8_select(self._ref, E, ids_c.data_ptr(), n, ids_c.element_size(),
+                                                                     _FP8_FORMATS[self._offs[0][2]], _MATVEC_DTYPES[dtype], n_out, arr,
+                                                                     scratch.data_ptr(), scratch.numel(),
+                                                                     torch.cuda.current_stream(self.device).cuda_stream)
+        if rc:
+            _native.check(rc)
+        return result
 
     def _product(self, kind: _Product, k: int, x, bias, out, scratch, scale=None, block=None) -> torch.Tensor:
         """matvec, matmul, matvec_fp8 and matmul_fp8: the checks and the call."""

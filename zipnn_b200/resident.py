@@ -31,6 +31,9 @@ Rules:
   * with `fp8=True` a selected fp8 linear layer (`fp8_linears`: transformers' `FP8Linear`) keeps its scales and bias
     dense and runs W8A16 from its stream at any number of rows: `DecodePlan.matvec_fp8` for at most `matvec` rows,
     `DecodePlan.dequant_fp8` + F.linear for more; it needs no downloaded kernel;
+  * with `fp8=True` and `experts=True` together, an fp8 experts module (`fp8_experts`: transformers' `FP8Experts`)
+    keeps its scales dense and runs W8A16: `DecodePlan.dequant_fp8_select` writes only its routed experts' weights,
+    dequantized to bf16 / fp16, and the bf16 experts implementation its config names runs on them;
   * with `experts=True` the experts module of a mixture-of-experts layer (`experts_module`: 3D weights [E, ...] called
     as experts(hidden_states, top_k_index, top_k_weights)) decodes only the slices [e] of the experts its router
     picked (`DecodePlan.run_select`); its own forward then runs unchanged and reads only those slices;
@@ -43,6 +46,8 @@ copy of the compressed weights on the GPU, and `save_module(model, file)` writes
 """
 from __future__ import annotations
 
+import inspect
+import math
 import os
 import traceback
 from typing import NamedTuple
@@ -136,7 +141,8 @@ class _Entry(NamedTuple):
     module: torch.nn.Module
     plan: DecodePlan
     names: list   # [(name, index into the plan's outputs)]
-    mode: str     # hooks: "decode", "prefetch", "experts"; a forward of its own: "matvec", "matmul", "fp8", "fp8_torch"
+    mode: str     # hooks: "decode", "prefetch", "experts"; a forward of its own: "matvec", "matmul", "fp8", "fp8_torch",
+                  # "fp8_experts", "fp8_experts_torch"
 
 
 class _Resident:
@@ -159,7 +165,7 @@ class _Resident:
         self.matvec_scratch_bytes = 0
         self.matmul_scratch = None     # the "matmul" modules' matmul scratch and what the largest needs of it
         self.matmul_scratch_bytes = 0
-        self.select_scratch = None     # the "experts" modules' run_select scratch, sized for the largest
+        self.select_scratch = None     # the "experts" and "fp8_experts" modules' selected-run scratch, sized for the largest
         self.fp8_scratch = None        # the "fp8" modules' matvec_fp8 scratch and what the largest needs of it
         self.fp8_scratch_bytes = 0
         self.fp8_matmul = 0            # fp8_matmul=N: the most input rows an "fp8" module multiplies by matmul_fp8
@@ -257,26 +263,59 @@ def fp8_linears(module: torch.nn.Module) -> bool:
     return tuple(scale.shape) == (-(-w.shape[0] // block[0]), -(-w.shape[1] // block[1]))
 
 
+def fp8_experts(module: torch.nn.Module) -> bool:
+    """Does `fp8=True, experts=True` run `module` from its compressed fp8 expert weights?  A module of the
+    `experts_module` convention (integer `num_experts` = E) with a `block_size` that is None or (bn, bk), at least one
+    float8_e4m3fn / float8_e5m2 parameter, each of them 3-D [E, out, in] with an fp32 `<name>_scale_inv` of the grid
+    the block implies, [E, ceil(out / bn), ceil(in / bk)] (None: [E, 1, 1]), and no bias parameter: transformers'
+    `FP8Experts` (gate_up_proj or up_proj, down_proj), found by these attributes."""
+    if not (experts_module(module) and hasattr(module, "block_size")):
+        return False
+    block, n = module.block_size, module.num_experts
+    if block is not None and not (isinstance(block, (tuple, list)) and len(block) == 2
+                                  and all(isinstance(b, int) and not isinstance(b, bool) and b >= 1 for b in block)):
+        return False
+    params = {name: p for name, p in module._parameters.items() if p is not None}
+    fp8 = [(name, p) for name, p in params.items() if p.dtype in _FP8]
+    if not fp8 or any("bias" in name for name in params):
+        return False
+    for name, w in fp8:
+        s = params.get(name + "_scale_inv")
+        if w.dim() != 3 or not (isinstance(s, torch.Tensor) and s.dtype == torch.float32):
+            return False
+        grid = (n, 1, 1) if block is None else (n, -(-w.shape[1] // block[0]), -(-w.shape[2] // block[1]))
+        if tuple(s.shape) != grid:
+            return False
+    return True
+
+
 def dequantize_fp8(weight: torch.Tensor, scale: torch.Tensor, block, dtype: torch.dtype) -> torch.Tensor:
-    """torch's dequantize of an fp8 weight [out, in]: (W.to(float32) * S_expanded).to(dtype), S expanded over its
-    (bn, bk) blocks (block None: one scale for the tensor).  `DecodePlan.dequant_fp8` gives the same bits."""
+    """torch's dequantize of an fp8 weight [..., out, in]: (W.to(float32) * S_expanded).to(dtype), S expanded over its
+    (bn, bk) blocks (block None: one scale per [out, in] matrix), one grid [ceil(out / bn), ceil(in / bk)] per leading
+    index (an experts weight [E, out, in] has one per expert).  `DecodePlan.dequant_fp8` and `dequant_fp8_select` give
+    the same bits."""
     w = weight.to(torch.float32)
+    lead = tuple(weight.shape[:-2])
     if block is None:
-        return (w * scale.reshape(())).to(dtype)
-    (out, inn), (bn, bk) = weight.shape, block
-    s = scale.reshape(-(-out // bn), -(-inn // bk)).repeat_interleave(bn, 0)[:out].repeat_interleave(bk, 1)[:, :inn]
+        return (w * scale.reshape(lead + (1, 1))).to(dtype)
+    (out, inn), (bn, bk) = weight.shape[-2:], block
+    s = scale.reshape(lead + (-(-out // bn), -(-inn // bk))).repeat_interleave(bn, -2)[..., :out, :]
+    s = s.repeat_interleave(bk, -1)[..., :inn]
     return (w * s).to(dtype)
 
 
-def dense_biases(groups, matvec: int, fp8: bool = False) -> list:
+def dense_biases(groups, matvec: int, fp8: bool = False, experts: bool = False) -> list:
     """`select`'s groups without the parameters that stay dense: under matvec=N the biases owned by `matvecs` modules
     only (the matvec adds them after the sum, so they must not need a decode); under fp8=True every parameter but the
-    weight of `fp8_linears` modules (scales, bias, activation scale: the products read them as they are)."""
+    weight of `fp8_linears` modules (scales, bias, activation scale: the products read them as they are); under
+    fp8=True and experts=True together every parameter but the fp8 ones of `fp8_experts` modules (scales, static
+    activation scales)."""
     if not (matvec or fp8):
         return groups
 
     def dense(o, n):
-        return (matvec and n == "bias" and matvecs(o)) or (fp8 and n != "weight" and fp8_linears(o))
+        return ((matvec and n == "bias" and matvecs(o)) or (fp8 and n != "weight" and fp8_linears(o))
+                or (fp8 and experts and o._parameters[n].dtype not in _FP8 and fp8_experts(o)))
     return [(p, owners) for p, owners in groups if not all(dense(o, n) for o, n in owners)]
 
 
@@ -334,6 +373,59 @@ def _fp8_forward(mod, state, plan, k, names, fast: bool):
                 y = F.linear(input, w)
             return y if mod.bias is None else (y + mod.bias).to(input.dtype)
         return decoded(input)
+    return forward
+
+
+def _experts_impl(mod):
+    """The experts function `mod.config._experts_implementation` names, for bf16 / fp16 weights: transformers'
+    `ALL_EXPERTS_FUNCTIONS` entry ("batched_mm", "grouped_mm"), else the class's own loop under the dispatcher that
+    transformers puts on `forward` (which would pick the fp8 functions)."""
+    name = getattr(getattr(mod, "config", None), "_experts_implementation", None)
+    if name not in (None, "eager"):
+        from transformers.integrations.moe import ALL_EXPERTS_FUNCTIONS
+        if name in ALL_EXPERTS_FUNCTIONS:
+            return ALL_EXPERTS_FUNCTIONS[name]
+    return inspect.unwrap(type(mod).forward)
+
+
+def _fp8_experts_forward(mod, state, plan, names, fast: bool):
+    """The forward of an fp8 experts module (W8A16: the activations are not quantized), called as experts(hidden_states,
+    top_k_index, top_k_weights), positional or by keyword.  For bf16 / fp16 hidden_states on the plan's device, outside
+    autocast, with CUDA int32 / int64 ids there: `plan.dequant_fp8_select` writes the routed experts' weights S * W in
+    the input's dtype into the shared output buffer, they are bound as the weights, and `_experts_impl` runs on them.
+    A module `fast` is False for (`dequant_fp8_select_ok` refuses it), and any other input, takes a selected run (the ids
+    as above; else the whole decode) and torch's dequantize into fresh tensors instead, with the same result."""
+    block = _fp8_block(mod)
+    shapes = [tuple(o.shape) for o in plan.outputs]
+    inf = [sh[-1] for sh in shapes]
+    blocks = [block] * len(names)
+    sizes = [2 * math.prod(sh) for sh in shapes]
+    offs = [0]
+    for n in sizes[:-1]:
+        offs.append(offs[-1] + (n + 15) // 16 * 16)
+    unbind = _unbind(names)
+
+    def forward(*args, **kwargs):
+        if torch.is_grad_enabled():
+            _grad_mode_error(mod, shared=True)
+        hidden = args[0] if args else kwargs.get("hidden_states")
+        ids = args[1] if len(args) > 1 else kwargs.get("top_k_index")
+        scales = [getattr(mod, name + "_scale_inv") for name, _ in names]
+        on_device = (isinstance(ids, torch.Tensor) and ids.is_cuda and ids.device == plan.device
+                     and ids.dtype in (torch.int32, torch.int64))
+        if (fast and on_device and isinstance(hidden, torch.Tensor) and hidden.dtype in (torch.bfloat16, torch.float16)
+                and hidden.device == plan.device and not torch.is_autocast_enabled(plan.device.type)):
+            outs = [plan._out[o: o + n].view(hidden.dtype).view(sh) for o, n, sh in zip(offs, sizes, shapes)]
+            ws = plan.dequant_fp8_select(ids, inf, scales, blocks, hidden.dtype, outs=outs, scratch=state.select_scratch)
+        else:
+            dt = hidden.dtype if isinstance(hidden, torch.Tensor) and hidden.dtype in (torch.bfloat16, torch.float16, torch.float32) else torch.bfloat16
+            coded = plan.run_select(ids, scratch=state.select_scratch) if on_device and plan.select_ok() else plan.run()
+            ws = [dequantize_fp8(coded[k], s, block, dt) for (_, k), s in zip(names, scales)]
+        _bind(mod, names, ws)
+        try:
+            return _experts_impl(mod)(mod, *args, **kwargs)
+        finally:
+            unbind(mod, args, None)
     return forward
 
 
@@ -417,7 +509,10 @@ def _resident_state(modules, groups, streams: dict, buffers: list, dev, opts: _O
     `DecodePlan.matmul_ok` accepts (matmul=N), "matvec" for one that only `DecodePlan.matvec_ok` accepts (matvec=N);
     "fp8" for an `fp8_linears` module whose one compressed parameter is its weight and which `DecodePlan.matvec_fp8_ok`
     accepts, "fp8_torch" for one it refuses (fp8=True; the shared output buffer holds at least twice such a weight's
-    bytes, its dequantized weight); "experts" for an `experts_module` whose plan passes `DecodePlan.select_ok`
+    bytes, its dequantized weight); "fp8_experts" for an `fp8_experts` module whose compressed parameters are its fp8
+    ones and whose plan `DecodePlan.select_ok` and `DecodePlan.dequant_fp8_select_ok` accept, "fp8_experts_torch" for
+    one they refuse (fp8=True and experts=True; the shared output buffer holds at least 2 bytes per fp8 element of such
+    a module, its dequantized weights); "experts" for an `experts_module` whose plan passes `DecodePlan.select_ok`
     (experts=True); else "prefetch" with prefetch=True, "decode" without."""
     where = {id(groups[i][0]): i for i in streams}
     per_module = []
@@ -429,7 +524,12 @@ def _resident_state(modules, groups, streams: dict, buffers: list, dev, opts: _O
     sizes = [DecodePlan.sizes([streams[i] for _, i in names]) for _, names in whole]
     own_sizes = [DecodePlan.sizes([streams[i]]) for i in own]
     fp8_mods = {id(m) for m, names in whole if opts.fp8 and fp8_linears(m) and [n for n, _ in names] == ["weight"]}
-    out_need = max([s[0] for s in sizes] + [2 * m.weight.numel() for m, _ in whole if id(m) in fp8_mods] + [1])
+    # fp8 experts whose fp8 parameters, and only those, are compressed; their dequantized weights go to the shared buffer
+    fp8_exp = {id(m) for m, names in whole if opts.fp8 and opts.experts and fp8_experts(m)
+               and sorted(n for n, _ in names) == sorted(n for n, p in _own_params(m) if p.dtype in _FP8)}
+    out_need = max([s[0] for s in sizes] + [2 * m.weight.numel() for m, _ in whole if id(m) in fp8_mods]
+                   + [sum((2 * groups[i][0].numel() + 15) // 16 * 16 for _, i in names) for m, names in whole if id(m) in fp8_exp]
+                   + [1])
     out = None if own else torch.empty(out_need, dtype=torch.uint8, device=dev)
     scratch = torch.empty(max([s[1] for s in sizes + own_sizes] + [1]), dtype=torch.uint8, device=dev)
     state = _Resident()
@@ -461,6 +561,10 @@ def _resident_state(modules, groups, streams: dict, buffers: list, dev, opts: _O
         elif id(m) in fp8_mods:
             block = _fp8_block(m)
             mode = "fp8" if plan.matvec_fp8_ok(0, m.in_features) and (block is None or block[1] % 16 == 0) else "fp8_torch"
+        elif id(m) in fp8_exp:
+            block = _fp8_block(m)
+            fast = plan.select_ok() and plan.dequant_fp8_select_ok([o.shape[-1] for o in plan.outputs])
+            mode = "fp8_experts" if fast and (block is None or block[1] % 16 == 0) else "fp8_experts_torch"
         elif opts.experts and experts_module(m, [n for n, _ in local]) and plan.select_ok():
             mode = "experts"
         else:
@@ -509,7 +613,7 @@ def _commit(module: torch.nn.Module, state: _Resident, opts: _Options) -> None:
     state.matvec = opts.matvec
     matvec = [e for e in state.entries if e.mode in ("matvec", "matmul")]
     matmul = [e for e in state.entries if e.mode == "matmul"]
-    experts = [e for e in state.entries if e.mode == "experts"]
+    experts = [e for e in state.entries if e.mode == "experts" or (e.mode.startswith("fp8_experts") and e.plan.select_ok())]
     fp8 = [e for e in state.entries if e.mode == "fp8"]
     if matvec and opts.matvec:
         state.matvec_scratch_bytes = max(e.plan.matvec_scratch_bytes(0, e.module.in_features, opts.matvec) for e in matvec)
@@ -518,7 +622,7 @@ def _commit(module: torch.nn.Module, state: _Resident, opts: _Options) -> None:
         state.matmul_scratch_bytes = max(e.plan.matmul_scratch_bytes(0, e.module.in_features, opts.matmul) for e in matmul)
         state.matmul_scratch = _plans_scratch_or_own(state, state.matmul_scratch_bytes)
     if experts:
-        # always a buffer of its own: run_select must not be given the plans' scratch
+        # always a buffer of its own: run_select and dequant_fp8_select must not be given the plans' scratch
         need = max(e.plan.select_scratch_bytes() for e in experts)
         state.select_scratch = torch.empty(need, dtype=torch.uint8, device=state.scratch.device)
     if fp8 and opts.matvec:
@@ -534,6 +638,8 @@ def _commit(module: torch.nn.Module, state: _Resident, opts: _Options) -> None:
                                                     opts.matmul if mode == "matmul" else 0)
         elif mode in ("fp8", "fp8_torch"):   # no hooks either: its forward multiplies from the stream, or decodes
             m.__dict__["forward"] = _fp8_forward(m, state, plan, 0, names, mode == "fp8")
+        elif mode in ("fp8_experts", "fp8_experts_torch"):   # its forward binds the dequantized weights itself
+            m.__dict__["forward"] = _fp8_experts_forward(m, state, plan, names, mode == "fp8_experts")
         else:
             if mode == "experts":
                 pre = m.register_forward_pre_hook(_pre_hook_experts(plan, names, state), with_kwargs=True)
@@ -615,6 +721,18 @@ def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = Fals
     The report gains "fp8_modules" and "fp8_scratch_bytes" (the matvec_fp8 scratch, the plans' one when it is large
     enough).  ValueError together with prefetch=True.
 
+    fp8=True and experts=True together (either alone changes nothing here): a selected `fp8_experts` module
+    (transformers' `FP8Experts`) compresses only its fp8 weights; the `*_scale_inv` grids and static activation scales
+    stay dense parameters.  Its forward takes bf16 / fp16 hidden_states on the weights' device, outside autocast, with
+    CUDA int32 / int64 `top_k_index` there: `DecodePlan.dequant_fp8_select` writes only the routed experts' weights,
+    dequantized to the input's dtype (bit for bit torch's dequantize), into the shared output buffer, and the experts
+    implementation `config._experts_implementation` names runs on them -- the class's own loop for "eager",
+    transformers' bf16 `batched_mm` / `grouped_mm` functions for those -- so it needs no downloaded kernel and does not
+    quantize the activations.  A module whose plan `dequant_fp8_select_ok` refuses, and any other input, takes a
+    selected run (or the whole decode) and torch's dequantize instead, with the same result.  The shared output buffer
+    holds at least 2 bytes per fp8 element of such a module; the selected-run scratch ("experts_scratch_bytes") serves
+    both kinds of experts modules.  The report of a model with such modules gains "fp8_experts_modules".
+
     fp8_matmul=N (0 .. MATMUL_MAX_TOKENS; 0, the default, changes nothing): with fp8=True, an fp8 module whose weight
     `DecodePlan.matvec_fp8_ok` accepts computes bf16 / fp16 inputs of more than `matvec` rows and at most N as
     `DecodePlan.matmul_fp8` (tensor cores, two launches, the weight neither dequantized into the shared buffer nor
@@ -626,7 +744,7 @@ def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = Fals
     if getattr(module, _ATTR, None) is not None:
         raise ValueError("compress_module: this module is already compressed")
     modules, groups = select(module, modules)
-    groups = dense_biases(groups, max(opts.matvec, opts.matmul), opts.fp8)
+    groups = dense_biases(groups, max(opts.matvec, opts.matmul), opts.fp8, opts.experts)
     params = [p for p, _ in groups]
     if not params:
         setattr(module, _ATTR, None)
@@ -664,6 +782,9 @@ def _with_prefetch(report: dict, state, opts: _Options) -> dict:
                       experts_scratch_bytes=0 if state.select_scratch is None else state.select_scratch.numel())
     if opts.fp8:
         report.update(fp8_modules=modes.count("fp8") + modes.count("fp8_torch"), fp8_scratch_bytes=state.fp8_scratch_bytes)
+    fp8_experts_modules = modes.count("fp8_experts") + modes.count("fp8_experts_torch")
+    if fp8_experts_modules:   # (only fp8=True with experts=True makes them; a model without one keeps its report)
+        report.update(fp8_experts_modules=fp8_experts_modules)
     if opts.fp8_matmul:
         report.update(fp8_matmul_modules=modes.count("fp8"), fp8_matmul_scratch_bytes=state.fp8_matmul_scratch_bytes)
     return report
@@ -688,7 +809,7 @@ def decompress_module(module: torch.nn.Module) -> None:
     for h in state.hooks:
         h.remove()
     for m, _, _, mode in state.entries:
-        if mode in ("matvec", "matmul", "fp8", "fp8_torch"):   # the modes whose forward _commit replaced
+        if mode in ("matvec", "matmul", "fp8", "fp8_torch", "fp8_experts", "fp8_experts_torch"):   # the modes whose forward _commit replaced
             m.__dict__.pop("forward", None)
     for m, _, _, _ in state.gathers:
         m.__dict__.pop("forward", None)
@@ -796,7 +917,7 @@ def _files(filenames) -> list:
     return [os.fspath(f) for f in filenames]
 
 
-def plan_load(module: torch.nn.Module, filenames, modules=None, matvec: int = 0, fp8: bool = False) -> LoadPlan:
+def plan_load(module: torch.nn.Module, filenames, modules=None, matvec: int = 0, fp8: bool = False, experts: bool = False) -> LoadPlan:
     """The checks and choices of `load_module`, from the files' headers: ValueError naming the keys for a missing or
     unexpected key, a dtype or shape that differs, a non-persistent buffer on the meta device, and for a module that
     is already compressed."""
@@ -804,7 +925,7 @@ def plan_load(module: torch.nn.Module, filenames, modules=None, matvec: int = 0,
         raise ValueError("load_module: this module is already compressed")
     found = file_entries(_files(filenames))
     modules, groups = select(module, modules)
-    groups = dense_biases(groups, matvec, fp8)   # (matvec=N, fp8=True: the parameters that stay dense are read so)
+    groups = dense_biases(groups, matvec, fp8, experts)   # (matvec=N, fp8=True: the parameters that stay dense are read so)
     plan = LoadPlan(modules, groups)
     group_of = {id(p): gi for gi, (p, _) in enumerate(groups)}
     by_key = {}
@@ -986,7 +1107,7 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None,
         raise ValueError(f"load_module: {device!r} is not a CUDA device")
     if dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
-    plan = plan_load(module, filenames, modules, max(opts.matvec, opts.matmul), opts.fp8)
+    plan = plan_load(module, filenames, modules, max(opts.matvec, opts.matmul), opts.fp8, opts.experts)
     try:
         state, report, dense, stayed, moved = _load_device(plan, dev, opts)
     except BaseException as e:
