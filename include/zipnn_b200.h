@@ -405,6 +405,37 @@ int zipnn_b200_decode_plan_dequant_fp8_select(const zipnn_b200_decode_plan* plan
                                               const zipnn_b200_fp8_select_item* items, void* d_scratch,
                                               size_t scratch_bytes, void* cuda_stream);
 
+/* _experts_matvec_fp8: the routed experts of one item of an fp8 mixture-of-experts plan times x, from the coded
+ * bitstreams of the chunks they meet; no weight is written.  The plan is one _dequant_fp8_select takes (every item
+ * `rows` = E slices along dim 0); item `item` is seen as E experts [out][in_features], out = its rows / E, with the
+ * per-expert scale grid d_scale [E][ceil(out / bn)][ceil(in / bk)] and blocks as for _dequant_fp8_select.  d_ids holds
+ * n_ids = T * top_k expert ids (id_bytes 4 or 8), pair p = t * top_k + j; T <= ZIPNN_B200_EXPERTS_MATVEC_MAX_TOKENS (4:
+ * a lane holds one fp32 sum per pair slot, and 8 slots do not fit the decoder's 80 registers without spills).  For every
+ * pair p with an id in [0, E):
+ *   d_y[p * y_stride + o] = x_dtype(sum_i x_p[i] * (float(W[ids[p]][o][i]) * S[ids[p]][o / bn][i / bk]))
+ * with x_p row p / top_k of d_x (x_per_pair == 0: one row per token) or row p (x_per_pair != 0: one row per pair), rows
+ * x_stride elements apart, of x_dtype (ZIPNN_B200_MATVEC_BF16 or _FP16).  Bit for bit _matvec_fp8 of the item seen as
+ * [E * out][in] with x = x_p, rows ids[p] * out + o: the same products, sums in the same order, one rounding.  Pairs
+ * with an invalid id write nothing.
+ * Five launches whatever the id values are (the index kernel of _run_select on this item, the pair tables, the product,
+ * the reduce, the plan run's error pass; none for n_ids == 0), no copy and no host read but the first call's read of
+ * the item's chunk modes: capturable in a CUDA graph, replayable with new ids, x and scales.  An id outside [0, E), or
+ * an expert routed more than T rounded up to a power of two times (a token that repeats an expert), raises E_INDEX.
+ * _experts_matvec_fp8_scratch_size: the scratch bytes for (rows, in_features, n_ids, top_k): the select scratch, the
+ * pair tables and _matvec_fp8's partial sums.  The scratch holds nothing between calls.
+ * Host-side rejections launch and write nothing: E_ARG as _dequant_fp8_select refuses the plan, rows, ids, scratch,
+ * fp8_format, the blocks and d_scale, as _matvec_fp8 refuses x_dtype, in_features, d_x, d_y and their strides, for
+ * an item out of range, top_k == 0, n_ids not a multiple of top_k, T over the limit, an item whose slices are not whole
+ * rows, x rows spanning more than 2^32 elements and a scratch under the stated size. */
+#define ZIPNN_B200_EXPERTS_MATVEC_MAX_TOKENS 4
+int zipnn_b200_decode_plan_experts_matvec_fp8_scratch_size(const zipnn_b200_decode_plan* plan, int item, size_t rows,
+                                                           size_t in_features, size_t n_ids, size_t top_k, size_t* out);
+int zipnn_b200_decode_plan_experts_matvec_fp8(const zipnn_b200_decode_plan* plan, int item, size_t rows, const void* d_ids,
+                                              size_t n_ids, int id_bytes, size_t top_k, int fp8_format, int x_dtype,
+                                              size_t in_features, const void* d_x, size_t x_stride, int x_per_pair,
+                                              const float* d_scale, size_t block_rows, size_t block_cols, void* d_y,
+                                              size_t y_stride, void* d_scratch, size_t scratch_bytes, void* cuda_stream);
+
 /* ---- stage 1 alone ------------------------------------------------------------ */
 /* d_planes: num_buf planes of `stride` bytes each; plane g receives byte g of every element
  * of the (optionally rotated) input.  Lengths as in the reference: n/num_buf, the first

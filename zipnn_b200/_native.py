@@ -20,6 +20,7 @@ NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "
 
 OK, E_ARG, E_CAPACITY, E_CORRUPT, E_CUDA, E_UNSUPPORTED, E_INDEX = 0, 1, 2, 3, 4, 5, 6
 MATVEC_MAX_TOKENS = 8   # ZIPNN_B200_MATVEC_MAX_TOKENS
+EXPERTS_MATVEC_MAX_TOKENS = 4   # ZIPNN_B200_EXPERTS_MATVEC_MAX_TOKENS
 MATMUL_MAX_TOKENS = 64  # ZIPNN_B200_MATMUL_MAX_TOKENS
 FP8_E4M3, FP8_E5M2 = 0, 1   # ZIPNN_B200_FP8_E4M3 / _E5M2
 
@@ -140,6 +141,9 @@ def lib() -> C.CDLL:
                 "zipnn_b200_decode_plan_dequant_fp8": (i32, [C.POINTER(DecodePlanStruct), i32, i32, i32, sz, vp, sz, sz, vp, vp]),
                 "zipnn_b200_decode_plan_dequant_fp8_select": (i32, [C.POINTER(DecodePlanStruct), sz, vp, sz, i32, i32, i32, i32,
                                                                     C.POINTER(Fp8SelectItem), vp, sz, vp]),
+                "zipnn_b200_decode_plan_experts_matvec_fp8_scratch_size": (i32, [C.POINTER(DecodePlanStruct), i32, sz, sz, sz, sz, szp]),
+                "zipnn_b200_decode_plan_experts_matvec_fp8": (i32, [C.POINTER(DecodePlanStruct), i32, sz, vp, sz, i32, sz, i32, i32, sz,
+                                                                    vp, sz, i32, vp, sz, sz, vp, sz, vp, sz, vp]),
                 "zipnn_b200_split": (i32, [vp, sz, i32, i32, vp, sz, vp]),
                 "zipnn_b200_regroup": (i32, [vp, sz, sz, i32, i32, vp, vp]),
                 "zipnn_b200_compress_host": (i32, [vp, sz, vp, sz, i32, i32, i32, sz, C.c_float, vp, sz, szp]),
@@ -169,7 +173,8 @@ EXPORTS = [
     "zipnn_b200_decode_plan_matmul_scratch_size", "zipnn_b200_decode_plan_matmul",
     "zipnn_b200_decode_plan_matvec_fp8_scratch_size", "zipnn_b200_decode_plan_matvec_fp8",
     "zipnn_b200_decode_plan_matmul_fp8_scratch_size", "zipnn_b200_decode_plan_matmul_fp8",
-    "zipnn_b200_decode_plan_dequant_fp8", "zipnn_b200_decode_plan_dequant_fp8_select", "zipnn_b200_split", "zipnn_b200_regroup", "zipnn_b200_compress_host", "zipnn_b200_decompress_host",
+    "zipnn_b200_decode_plan_dequant_fp8", "zipnn_b200_decode_plan_dequant_fp8_select",
+    "zipnn_b200_decode_plan_experts_matvec_fp8_scratch_size", "zipnn_b200_decode_plan_experts_matvec_fp8", "zipnn_b200_split", "zipnn_b200_regroup", "zipnn_b200_compress_host", "zipnn_b200_decompress_host",
     "zipnn_b200_timing_enable", "zipnn_b200_timing_kernel_count", "zipnn_b200_timing_kernel_name",
     "zipnn_b200_timing_collect",
 ]

@@ -31,6 +31,8 @@
 #include <cuda_fp16.h>
 #include <cuda_fp8.h>
 
+#include <type_traits>
+
 #include "decode_sync.cuh"
 
 namespace zb {
@@ -63,6 +65,18 @@ struct ProductCfg {
   // slice_rows rows, each with a grid of its own of slice_grid scales; slice s of row r is matvec_fp8_div(r, sslice)
   uint64_t sslice;
   uint32_t slice_rows, slice_grid;
+};
+
+// The selected experts matvec's arguments (k_select_matvec_fp8, select.cuh): the item [E][out][in] as one matrix of
+// E * out rows with the per-slice scale grid (sslice, slice_rows, slice_grid), nt = the pair slots per expert, and
+// k_select_pairs' tables.  Slot t of expert e multiplies x row tab[e * nt + t] / k (one x row per token) or
+// tab[e * nt + t] (one x row per pair), taken by a multiply-high by xdiv = matvec_fp8_recip(k or 1).  A type of its own
+// rather than new ProductCfg fields, so that ProductCfg, and every kernel that takes it, stays as it was.
+struct ExpertsCfg : ProductCfg {
+  uint32_t* cnt;  // [E] pairs routed to expert e (at most nt)
+  uint32_t* tab;  // [E][nt] their pair numbers, ascending
+  uint32_t* pos;  // [pairs] pair p's slot in its expert's list
+  uint64_t xdiv;
 };
 
 // Elements of a block of a chunk with n elements: a quarter's vectors split over 8 warps, in whole 32-vector steps.
@@ -144,20 +158,37 @@ __device__ __forceinline__ void fp8_floats(uint32_t a, uint32_t b, float (&f)[8]
 // NT: the accumulators a lane holds, n_tokens rounded up to a power of two.  Tokens past n_tokens repeat the last one
 // and are not stored: 3 and 5 to 7 tokens pay for 4 and 8.  A uniform `t < n_tokens` exit from the token loop was
 // measured instead: it keeps the loads of the tokens from being issued together, and 8 tokens took 1.3 to 1.5 times as long.
-template <int DT, int NT, int FMT = -1>
+//
+// EXPERTS (fp8 only; k_select_matvec_fp8): m is an ExpertsCfg, and the matrix is E experts of slice_rows rows.  A row's
+// expert is matvec_fp8_div(row, sslice), its scale the expert's own grid (DequantEp's SLICED lookup), and token slot t
+// of the row is the t-th pair routed to that expert: its x row comes from the pair table.  A lane reads the table again
+// only when the expert of its row changes (a warp's rows almost always share one).  Slots past the expert's pair count
+// repeat its last pair (row 0 of x for an expert with none) and are not stored: the flush writes slot t only for
+// t < cnt[expert], so the rows of an unrouted expert in a chunk that straddles experts write nothing.
+template <int DT, int NT, int FMT = -1, bool EXPERTS = false>
 struct MatvecEp {
   static_assert(FMT < 0 || DT != kMvFp32, "fp8 weights: x of bf16 or fp16");
+  static_assert(!EXPERTS || FMT >= 0, "the experts form is fp8's");
   static constexpr bool on = true;
   static constexpr int EPV = FMT < 0 ? 16 / matvec_esize(DT) : 16;
-  ProductCfg m;
+  std::conditional_t<EXPERTS, ExpertsCfg, ProductCfg> m;
 
-  __device__ __forceinline__ void flush(float (&acc)[NT], float* slot, int lane) const {
+  // The slots of `row` that are stored.
+  __device__ __forceinline__ uint32_t stored(uint64_t row) const {
+    if constexpr (EXPERTS) {
+      return __ldg(m.cnt + matvec_fp8_div((uint32_t)row, m.sslice));
+    } else {
+      return m.nt;
+    }
+  }
+
+  __device__ __forceinline__ void flush(float (&acc)[NT], float* slot, int lane, uint32_t ns) const {
 #pragma unroll
     for (int t = 0; t < NT; t++) {
       float v = acc[t];
 #pragma unroll
       for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-      if (lane == t && (uint32_t)t < m.nt) slot[t] = v;
+      if (lane == t && (uint32_t)t < ns) slot[t] = v;
       acc[t] = 0.f;
     }
   }
@@ -180,6 +211,8 @@ struct MatvecEp {
     float acc[NT];
 #pragma unroll
     for (int t = 0; t < NT; t++) acc[t] = 0.f;
+    [[maybe_unused]] uint32_t xo[NT];       // EXPERTS: the element offset of slot t's x row, for expert xe
+    [[maybe_unused]] uint32_t xe = ~0u;
     uint64_t cur = row0;
     for (uint32_t v = v0; v < v1; v += 32) {
       const uint32_t nvalid = min(32u, v1 - v);
@@ -221,7 +254,22 @@ struct MatvecEp {
         uint32_t r[4];
         const uint32_t o = (v + (uint32_t)lane) * 16u;
         ZB_FUSED_VECTOR(G, S, out_off, o, rot, r);
-        const float sc = __ldg(m.scale + matvec_fp8_div((uint32_t)lrow, m.srow) * m.scols + matvec_fp8_div((uint32_t)lcol, m.scol));
+        float sc;
+        if constexpr (EXPERTS) {
+          const uint32_t e = matvec_fp8_div((uint32_t)lrow, m.sslice), er = (uint32_t)lrow - e * m.slice_rows;
+          sc = __ldg(m.scale + e * m.slice_grid + matvec_fp8_div(er, m.srow) * m.scols + matvec_fp8_div((uint32_t)lcol, m.scol));
+          if (e != xe) {
+            xe = e;
+            const uint32_t n = __ldg(m.cnt + e);
+#pragma unroll
+            for (int t = 0; t < NT; t++) {
+              const uint32_t p = n ? __ldg(m.tab + e * NT + min((uint32_t)t, n - 1u)) : 0u;
+              xo[t] = matvec_fp8_div(p, m.xdiv) * (uint32_t)m.xs;
+            }
+          }
+        } else {
+          sc = __ldg(m.scale + matvec_fp8_div((uint32_t)lrow, m.srow) * m.scols + matvec_fp8_div((uint32_t)lcol, m.scol));
+        }
         // in two halves of 8 columns, every token's sum carried from the first to the second (the order of each sum
         // is the same), the half loop not unrolled: only 16 bytes of x per token are in flight at once.  Unrolled, the
         // compiler issues all 32 bytes of every token together and NT = 8 spills at 80 registers.
@@ -231,8 +279,13 @@ struct MatvecEp {
           fp8_floats<FMT>(h ? r[2] : r[0], h ? r[3] : r[1], w);
 #pragma unroll
           for (int t = 0; t < NT; t++) {
-            const uint64_t tt = min((uint32_t)t, m.nt - 1u);
-            const uint4 xv = __ldg(reinterpret_cast<const uint4*>(xb + (tt * m.xs + lcol) * 2) + h);
+            uint64_t xrow;
+            if constexpr (EXPERTS) {
+              xrow = xo[t];
+            } else {
+              xrow = min((uint32_t)t, m.nt - 1u) * m.xs;
+            }
+            const uint4 xv = __ldg(reinterpret_cast<const uint4*>(xb + (xrow + lcol) * 2) + h);
             const uint32_t xr[4] = {xv.x, xv.y, xv.z, xv.w};
             float xf[8];
             matvec_floats<DT, 8>(xr, xf);
@@ -245,7 +298,7 @@ struct MatvecEp {
       }
       for (uint64_t rr = row0; rr <= last; rr++) {
         if (rr != cur) {
-          flush(acc, slots + (cur - first) * m.nt, lane);
+          flush(acc, slots + (cur - first) * m.nt, lane, stored(cur));
           cur = rr;
         }
         if (lrow == rr) {
@@ -260,7 +313,7 @@ struct MatvecEp {
         row0++;
       }
     }
-    flush(acc, slots + (cur - first) * m.nt, lane);
+    flush(acc, slots + (cur - first) * m.nt, lane, stored(cur));
   }
 };
 

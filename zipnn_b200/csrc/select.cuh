@@ -190,6 +190,91 @@ __global__ void __launch_bounds__(kSyncThreads, 3) k_select_dequant_fp8(SelectCf
   }
 }
 
+// ---- the selected experts matvec (k_select_matvec_fp8) --------------------------------------------------------------
+// y[p][o] = XDT(sum_i x_p[i] * (float(W[ids[p]][o][i]) * S[ids[p]][o / bn][i / bk])) for every pair p = t * k + j of
+// ids [T][k], x_p = x[p / k] (one x row per token) or x[p] (one per pair), on one item [E][out][in] of fp8 experts
+// (ExpertsCfg, matvec.cuh).  A call is five launches, whatever the ids: k_select_index on the one item, k_select_pairs,
+// k_select_matvec_fp8, k_select_matvec_reduce, k_batch_errors.  The product kernel is k_select_dequant_fp8's loop over
+// the selected bitstreams with MatvecEp's experts form: a warp's partial sums take the matvec's slots ([32 K blocks]
+// [rs][nt] of the whole item), where slot t of a row is the t-th pair routed to the row's expert.  Only the slots of
+// routed experts' rows in selected chunks are written, and the reduce reads only those, so the sums of a pair are
+// matvec_fp8's for the expert's rows: the same products, the same order, the same rounding.
+
+// (one CTA) The pair tables of the n = T * k ids over s.rows = E experts: cnt[e] pairs routed to e, tab[e][0..nt) their
+// numbers in ascending p, pos[p] p's slot in its expert's list.  Each pair counts the equal ids before and after it
+// (n is at most 4 * k), so nothing depends on thread order and there are no atomics but the error.  An id outside
+// [0, E) marks nothing (k_select_index raises kErrIndex for it); an expert given more than nt pairs (a token that
+// repeats an expert) raises kErrIndex, and its count stops at nt.  The counts are zeroed here: a call needs no memset.
+__global__ void __launch_bounds__(kGatherIndexThreads) k_select_pairs(SelectCfg s, ExpertsCfg m) {
+  for (uint64_t e = threadIdx.x; e < s.rows; e += blockDim.x) m.cnt[e] = 0;
+  __syncthreads();
+  for (uint64_t p = threadIdx.x; p < s.n; p += blockDim.x) {
+    const int64_t id = select_id(s, p);
+    if (id < 0 || (uint64_t)id >= s.rows) continue;
+    uint32_t before = 0, after = 0;
+    for (uint64_t q = 0; q < s.n; q++) {
+      if (select_id(s, q) == id) {
+        before += q < p;
+        after += q > p;
+      }
+    }
+    m.pos[p] = before;
+    if (before < m.nt) {
+      m.tab[(uint64_t)id * m.nt + before] = (uint32_t)p;
+    } else {
+      atomicOr(s.error, kErrIndex);
+    }
+    if (after == 0) m.cnt[id] = min(before + 1u, m.nt);
+  }
+}
+
+// Pair slots per expert: 1, 2 or 4 (T rounded up to a power of two).  With 8, a lane's sums and x row offsets need more
+// than the 80 registers of three CTAs per SM, and ptxas spills.
+constexpr int kExpertsMaxTokens = 4;
+
+template <int FMT, int XDT, int NT>
+__global__ void __launch_bounds__(kSyncThreads, 3) k_select_matvec_fp8(SelectCfg s, ExpertsCfg m) {
+  extern __shared__ __align__(1024) unsigned char smem_raw[];
+  const SyncCarve cv = sync_carve(smem_raw);
+  SyncShared& S = *cv.S;
+  static_assert(NT <= kExpertsMaxTokens, "no spills");
+  using Ep = MatvecEp<XDT, NT, FMT, true>;
+  const Ep ep{m};
+  const uint64_t units = 4ull * *s.count;
+  for (uint64_t w = blockIdx.x; w < units; w += gridDim.x) {
+    const uint64_t work = 4ull * s.hsel[w >> 2].y + (w & 3);  // (one item: the piece is 0)
+    __syncthreads();  // the previous unit's shared state is dead
+    sync_process<1, false, kSyncReplay, false, Ep>(*m.cfg, nullptr, S, cv.lut, cv.lut_s, work, m.seg + work * kSyncThreads, nullptr, &ep);
+  }
+}
+
+// One thread per (pair p, output o): R = ids[p] * out + o.  R's partial sums at slot pos[p], added in ascending element
+// order from +0 as k_matvec_reduce adds them, rounded once to XDT and stored at y[p * ys + o].  A pair with an invalid
+// id, or past its expert's slots, writes nothing.
+template <int XDT>
+__global__ void __launch_bounds__(256) k_select_matvec_reduce(SelectCfg s, ExpertsCfg m) {
+  const uint64_t out = m.slice_rows;
+  const uint64_t idx = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (idx >= s.n * out) return;
+  const uint64_t p = idx / out, o = idx - p * out;
+  const int64_t id = select_id(s, p);
+  if (id < 0 || (uint64_t)id >= s.rows) return;
+  const uint32_t slot = m.pos[p];
+  if (slot >= m.nt) return;
+  const uint64_t R = (uint64_t)id * out + o;
+  float sum = 0.f;
+  for (uint64_t e = R * m.in; e < (R + 1) * m.in;) {
+    const MatvecBlock b = matvec_block_of(m, e);
+    sum += m.part[((b.id * m.rs) + R - b.start / m.in) * m.nt + slot];
+    e = b.end;
+  }
+  if constexpr (XDT == kMvBf16) {
+    reinterpret_cast<__nv_bfloat16*>(m.y)[p * m.ys + o] = __float2bfloat16_rn(sum);
+  } else {
+    reinterpret_cast<__half*>(m.y)[p * m.ys + o] = __float2half_rn(sum);
+  }
+}
+
 // The selected regroup tiles (k_regroup_batch's tile numbering within a piece).
 __global__ void __launch_bounds__(kMergeThreads) k_select_regroup(BatchCfg B, SelectCfg s) {
   __shared__ PlaneSrc src[4];

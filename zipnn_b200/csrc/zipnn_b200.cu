@@ -1688,7 +1688,8 @@ int dequant_fp8(const zipnn_b200_decode_plan* plan, int item, const Fp8Scale& f8
 
 static_assert(kMatvecMaxTokens == ZIPNN_B200_MATVEC_MAX_TOKENS && kMvBf16 == ZIPNN_B200_MATVEC_BF16 && kMvFp16 == ZIPNN_B200_MATVEC_FP16 &&
                   kMvFp32 == ZIPNN_B200_MATVEC_FP32 && kMatmulMaxTokens == ZIPNN_B200_MATMUL_MAX_TOKENS &&
-                  kFp8E4m3 == ZIPNN_B200_FP8_E4M3 && kFp8E5m2 == ZIPNN_B200_FP8_E5M2,
+                  kFp8E4m3 == ZIPNN_B200_FP8_E4M3 && kFp8E5m2 == ZIPNN_B200_FP8_E5M2 &&
+                  kExpertsMaxTokens == ZIPNN_B200_EXPERTS_MATVEC_MAX_TOKENS,
               "the header's constants are the kernels'");
 
 int zipnn_b200_decode_plan_matvec_scratch_size(const zipnn_b200_decode_plan* plan, int item, int dtype, size_t in_features, size_t n_tokens,
@@ -1797,6 +1798,138 @@ int zipnn_b200_decode_plan_dequant_fp8_select(const zipnn_b200_decode_plan* plan
   k_select_index<<<1, kGatherIndexThreads, 0, st>>>(s.B, sel);
   ZB_LAUNCHED();
   k<<<blocks, kSyncThreads, kSyncSmemBytes, st>>>(sel, d);
+  ZB_LAUNCHED();
+  return batch_errors(s.B, st);
+}
+
+// ---- the selected experts matvec (select.cuh): x times the routed experts of one item, from its coded bitstreams ----
+// Scratch: [the select scratch][cnt u32 E][tab u32 E * nt][pos u32 n_ids][the matvec's partial sums with nt tokens],
+// nt = T = n_ids / top_k rounded up to a power of two.
+namespace {
+struct ExpertsLayout {
+  size_t cnt_off, tab_off, pos_off, part_off, bytes;
+};
+uint32_t experts_slots(size_t tokens) { return tokens <= 1 ? 1u : tokens <= 2 ? 2u : 4u; }
+ExpertsLayout experts_layout(const PlanState& s, const ProductCfg& m, size_t rows, size_t n_ids, uint32_t nt) {
+  ExpertsLayout L;
+  L.cnt_off = select_layout(s).bytes;
+  L.tab_off = round_up(L.cnt_off + sizeof(uint32_t) * rows, 256);
+  L.pos_off = round_up(L.tab_off + sizeof(uint32_t) * rows * nt, 256);
+  L.part_off = round_up(L.pos_off + sizeof(uint32_t) * n_ids, 256);
+  L.bytes = L.part_off + product_scratch_bytes(kMatvecFp8, m, nt);
+  return L;
+}
+// The checks both calls make: the plan and item (select_items, product_item), whole rows per slice, and the pairs.
+// -> the item's records, m with its fields of the item and the shapes, and T.
+int experts_item(const zipnn_b200_decode_plan* plan, int item, size_t rows, int x_dtype, size_t in_features, size_t n_ids,
+                 size_t top_k, cudaStream_t st, PlanState& s, std::vector<GatherItem>& gis, ExpertsCfg& m, size_t& tokens) {
+  {
+    const int rc = select_items(plan, rows, s, gis);
+    if (rc) return rc;
+  }
+  if (item < 0 || (size_t)item >= gis.size()) return ZIPNN_B200_E_ARG;
+  memset(&m, 0, sizeof(m));
+  {
+    const int rc = product_item(kMatvecFp8, plan, item, x_dtype, in_features, st, m);
+    if (rc) return rc;
+  }
+  if (m.out % rows) return ZIPNN_B200_E_ARG;  // a slice is whole rows
+  if (top_k == 0 || n_ids % top_k) return ZIPNN_B200_E_ARG;
+  tokens = n_ids / top_k;
+  if (tokens > (size_t)kExpertsMaxTokens) return ZIPNN_B200_E_ARG;
+  return ZIPNN_B200_OK;
+}
+}  // namespace
+
+int zipnn_b200_decode_plan_experts_matvec_fp8_scratch_size(const zipnn_b200_decode_plan* plan, int item, size_t rows, size_t in_features,
+                                                           size_t n_ids, size_t top_k, size_t* out) {
+  if (!out) return ZIPNN_B200_E_ARG;
+  PlanState s;
+  std::vector<GatherItem> gis;
+  ExpertsCfg m;
+  size_t tokens = 0;
+  const int rc = experts_item(plan, item, rows, kMvBf16, in_features, n_ids, top_k, nullptr, s, gis, m, tokens);
+  if (rc) return rc;
+  *out = experts_layout(s, m, rows, n_ids, experts_slots(tokens)).bytes;
+  return ZIPNN_B200_OK;
+}
+
+int zipnn_b200_decode_plan_experts_matvec_fp8(const zipnn_b200_decode_plan* plan, int item, size_t rows, const void* d_ids, size_t n_ids,
+                                              int id_bytes, size_t top_k, int fp8_format, int x_dtype, size_t in_features, const void* d_x,
+                                              size_t x_stride, int x_per_pair, const float* d_scale, size_t block_rows, size_t block_cols,
+                                              void* d_y, size_t y_stride, void* d_scratch, size_t scratch_bytes, void* cuda_stream) {
+  if (id_bytes != 4 && id_bytes != 8) return ZIPNN_B200_E_ARG;
+  const Fp8Scale f8{fp8_format, d_scale, block_rows, block_cols};
+  if (!fp8_args_ok(f8)) return ZIPNN_B200_E_ARG;
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  PlanState s;
+  std::vector<GatherItem> gis;
+  ExpertsCfg m;
+  size_t tokens = 0;
+  {
+    const int rc = experts_item(plan, item, rows, x_dtype, in_features, n_ids, top_k, st, s, gis, m, tokens);
+    if (rc) return rc;
+  }
+  if (n_ids == 0) return ZIPNN_B200_OK;
+  const uint32_t nt = experts_slots(tokens);
+  const ExpertsLayout L = experts_layout(s, m, rows, n_ids, nt);
+  {
+    const int rc = select_args_ok(select_layout(s), d_ids, n_ids, id_bytes, d_scratch, scratch_bytes);
+    if (rc) return rc;
+  }
+  const uint64_t out = m.out / rows, xrows = x_per_pair ? n_ids : tokens;
+  const uint32_t xes = (uint32_t)matvec_esize(x_dtype);
+  if (!d_x || !d_y || ((uintptr_t)d_x & 15) || ((uintptr_t)d_y % xes) || !d_scale || ((uintptr_t)d_scale & 3)) return ZIPNN_B200_E_ARG;
+  if (xrows > 1 && ((x_stride * xes) % 16 || x_stride < m.in)) return ZIPNN_B200_E_ARG;
+  if (n_ids > 1 && y_stride < out) return ZIPNN_B200_E_ARG;
+  if (xrows * std::max<uint64_t>(x_stride, m.in) > UINT32_MAX) return ZIPNN_B200_E_ARG;  // the x row offsets are 32-bit
+  if (scratch_bytes < L.bytes) return ZIPNN_B200_E_ARG;
+  uint8_t* const ws = (uint8_t*)d_scratch;
+  m.x = d_x;
+  m.y = d_y;
+  m.part = (float*)(ws + L.part_off);
+  m.xs = x_stride;
+  m.ys = y_stride;
+  m.nt = nt;
+  fp8_grid(f8, m, rows);
+  m.cnt = (uint32_t*)(ws + L.cnt_off);
+  m.tab = (uint32_t*)(ws + L.tab_off);
+  m.pos = (uint32_t*)(ws + L.pos_off);
+  m.xdiv = matvec_fp8_recip(x_per_pair ? 1 : top_k);
+  // k_select_index on a one-item view of the plan's batch: its hsel holds the item's selected bitstreams (piece 0)
+  BatchCfg one = s.B;
+  one.cfgs += item;
+  one.chunk_start += item;
+  one.n = 1;
+  const SelectCfg sel = select_cfg(s, select_layout(s), ws, rows, d_ids, n_ids, id_bytes);
+  uint64_t bitstreams = 0, tiles = 0, most = 0;
+  select_bounds(std::vector<GatherItem>{gis[(size_t)item]}, rows, n_ids, bitstreams, tiles, most);
+  const bool e4 = fp8_format == kFp8E4m3;
+  void (*k)(SelectCfg, ExpertsCfg) = nullptr;
+  void (*reduce)(SelectCfg, ExpertsCfg) = nullptr;
+  auto pick = [&](auto xdt) {
+    constexpr int XDT = decltype(xdt)::value;
+    reduce = &k_select_matvec_reduce<XDT>;
+    if (e4) {
+      k = nt == 1 ? &k_select_matvec_fp8<kFp8E4m3, XDT, 1> : nt == 2 ? &k_select_matvec_fp8<kFp8E4m3, XDT, 2> : &k_select_matvec_fp8<kFp8E4m3, XDT, 4>;
+    } else {
+      k = nt == 1 ? &k_select_matvec_fp8<kFp8E5m2, XDT, 1> : nt == 2 ? &k_select_matvec_fp8<kFp8E5m2, XDT, 2> : &k_select_matvec_fp8<kFp8E5m2, XDT, 4>;
+    }
+  };
+  if (x_dtype == kMvBf16) {
+    pick(std::integral_constant<int, kMvBf16>());
+  } else {
+    pick(std::integral_constant<int, kMvFp16>());
+  }
+  const unsigned blocks = resident_grid(k, kSyncSmemBytes, kSyncThreads, bitstreams);
+  if (!blocks) return ZIPNN_B200_E_CUDA;
+  k_select_index<<<1, kGatherIndexThreads, 0, st>>>(one, sel);
+  ZB_LAUNCHED();
+  k_select_pairs<<<1, kGatherIndexThreads, 0, st>>>(sel, m);
+  ZB_LAUNCHED();
+  k<<<blocks, kSyncThreads, kSyncSmemBytes, st>>>(sel, m);
+  ZB_LAUNCHED();
+  reduce<<<(unsigned)((n_ids * out + 255) / 256), 256, 0, st>>>(sel, m);
   ZB_LAUNCHED();
   return batch_errors(s.B, st);
 }

@@ -30,6 +30,7 @@ _ALIGN = 16
 GATHER_SLOTS = 64   # chunk slots of gather's default scratch: 16 MiB for 256 KiB chunks
 MATVEC_MAX_TOKENS = _native.MATVEC_MAX_TOKENS
 MATMUL_MAX_TOKENS = _native.MATMUL_MAX_TOKENS
+EXPERTS_MATVEC_MAX_TOKENS = _native.EXPERTS_MATVEC_MAX_TOKENS
 _MATVEC_DTYPES = {torch.bfloat16: 0, torch.float16: 1, torch.float32: 2}   # ZIPNN_B200_MATVEC_*
 _MATMUL_DTYPES = (torch.bfloat16, torch.float16)
 _FP8_FORMATS = {torch.float8_e4m3fn: _native.FP8_E4M3, torch.float8_e5m2: _native.FP8_E5M2}   # ZIPNN_B200_FP8_*
@@ -626,6 +627,100 @@ class DecodePlan:
         if rc:
             _native.check(rc)
         return result
+
+    def experts_matvec_fp8_ok(self, k: int, in_features: int) -> bool:
+        """Can `experts_matvec_fp8` multiply by the experts of output `k`, seen as [E, out, in_features] (E = shape[0])?
+        True when `select_ok` is, `matvec_fp8_ok(k, in_features)` accepts the output and each expert is whole rows.
+        The first call for an output synchronises (it reads the chunk modes); never raises."""
+        try:
+            k, i = int(k), int(in_features)
+        except (TypeError, ValueError):
+            return False
+        if not 0 <= k < len(self._offs) or i <= 0 or not self.select_ok():
+            return False
+        _, _, dt, sh = self._offs[k]
+        return dt in _FP8_FORMATS and self._ok(_MATVEC_FP8, k, i) and (math.prod(sh) // sh[0]) % i == 0
+
+    def experts_matvec_fp8_scratch_bytes(self, k: int, in_features: int, top_k: int, n_tokens: int = EXPERTS_MATVEC_MAX_TOKENS) -> int:
+        """Bytes of an `experts_matvec_fp8` scratch for output `k`, rows of `in_features` elements, `top_k` experts per
+        token and `n_tokens` tokens: the select scratch, the pair tables and the matvec's partial sums."""
+        out = C.c_size_t(0)
+        with torch.cuda.device(self.device):
+            rc = _native.lib().zipnn_b200_decode_plan_experts_matvec_fp8_scratch_size(self._ref, int(k), self._offs[0][3][0], int(in_features),
+                                                                                       int(n_tokens) * int(top_k), int(top_k), C.byref(out))
+        _native.check(rc)
+        return out.value
+
+    def experts_matvec_fp8(self, k: int, ids: torch.Tensor, x: torch.Tensor, scale: torch.Tensor, block: tuple = None,
+                           out: torch.Tensor = None, scratch: torch.Tensor = None) -> torch.Tensor:
+        """The routed experts of output `k` times x, from the coded streams of the chunks they meet
+        (zipnn_b200_decode_plan_experts_matvec_fp8): output k is an fp8 expert weight [E, out, in] with a scale grid
+        per expert, and for every pair (t, j) of `ids`, y[t, j] = x_tj @ (S[e] * W[e]).T with e = ids[t, j].  No weight
+        is written.  Each result is bit for bit `matvec_fp8` of the output seen as [E * out, in] with x = x_tj, rows
+        e * out ... (e + 1) * out - 1.  Five launches on the current CUDA stream, a fixed number, the ids never read on
+        the host: capturable in a CUDA graph and replayable with new ids, x and scales.
+
+        ids:     CUDA int32 or int64 tensor [T, top_k] on the plan's device, T <= EXPERTS_MATVEC_MAX_TOKENS.  Empty: nothing
+                 runs.
+        x:       CUDA bf16 or fp16 tensor [T, in] (pair (t, j) multiplies x[t]: the first projection) or [T, top_k, in]
+                 (it multiplies x[t, j]: the down projection); rows that are not 16-byte aligned are copied first.
+        scale, block: as for `dequant_fp8_select` (a grid per expert, [E, ceil(out / bn), ceil(in / bk)], or block=None
+                 for one scale per expert).
+        out:     optional [T, top_k, out] tensor of x's dtype with contiguous, equally spaced rows.
+        scratch: optional 256-byte aligned CUDA uint8 buffer of at least `experts_matvec_fp8_scratch_bytes(k, in,
+                 top_k, T)` bytes, not the plan's own scratch; it holds nothing between calls.  Default: a buffer kept
+                 by the plan.
+        -> out.  An id outside [0, E), or an expert routed more than once by one token, makes `check()` raise
+        IndexError (sticky).  ValueError for an output `experts_matvec_fp8_ok` refuses, and for bad ids, x, scale, block,
+        out or scratch.  Works without the plan's output buffer."""
+        name = "experts_matvec_fp8"
+        self._check_ids(name, ids)
+        if ids.dim() != 2:
+            raise ValueError(f"{name} takes ids [T, top_k], not {tuple(ids.shape)}")
+        T, top_k = ids.shape
+        if T > EXPERTS_MATVEC_MAX_TOKENS:
+            raise ValueError(f"{name} takes at most {EXPERTS_MATVEC_MAX_TOKENS} tokens, not {T}")
+        if not (isinstance(x, torch.Tensor) and x.is_cuda and x.device == self.device and x.dtype in _MATMUL_DTYPES
+                and tuple(x.shape[:-1]) in ((T,), (T, top_k))):
+            raise ValueError(f"{name} takes a CUDA bf16 or fp16 x [T, in] or [T, top_k, in] on the plan's device, T, top_k = {T}, {top_k}")
+        per_pair = x.dim() == 3
+        in_features = x.shape[-1]
+        if not self.experts_matvec_fp8_ok(k, in_features):
+            raise ValueError(f"{name} cannot multiply by output {k} with in_features {in_features} (see {name}_ok)")
+        wdt, total = self._product_item(k)
+        E = self._offs[0][3][0]
+        rows = total // (E * in_features)
+        bn, bk = self._fp8_grid(name, in_features, scale, block, rows, experts=E)
+        shape = (T, top_k, rows)
+        if out is None:
+            out = torch.empty(shape, dtype=x.dtype, device=self.device)
+        elif not (isinstance(out, torch.Tensor) and out.is_cuda and out.device == self.device and out.dtype == x.dtype
+                  and tuple(out.shape) == shape):
+            raise ValueError(f"{name}'s out must be a {x.dtype} CUDA tensor of shape {shape} on the plan's device")
+        n = T * top_k
+        if n == 0:
+            return out
+        try:
+            y2 = out.view(n, rows)
+        except RuntimeError:
+            y2 = None
+        if y2 is None or y2.stride(1) != 1:
+            raise ValueError(f"{name}'s out must have contiguous rows, equally spaced")
+        xr = n if per_pair else T
+        x2 = x.reshape(xr, in_features)
+        if x2.stride(1) != 1 or x2.data_ptr() % 16 or (xr > 1 and (x2.stride(0) * x.element_size()) % 16):
+            x2 = x2.contiguous()
+            if x2.data_ptr() % 16:
+                x2 = x2.clone()
+        ids_c = ids.contiguous()
+        scratch = self._scratch_for(name, scratch, lambda: self.experts_matvec_fp8_scratch_bytes(k, in_features, top_k, T))
+        rc = _native.lib().zipnn_b200_decode_plan_experts_matvec_fp8(
+            self._ref, k, E, ids_c.data_ptr(), n, ids_c.element_size(), top_k, _FP8_FORMATS[wdt], _MATVEC_DTYPES[x.dtype],
+            in_features, x2.data_ptr(), x2.stride(0), int(per_pair), scale.data_ptr(), bn, bk, y2.data_ptr(), y2.stride(0),
+            scratch.data_ptr(), scratch.numel(), torch.cuda.current_stream(self.device).cuda_stream)
+        if rc:
+            _native.check(rc)
+        return out
 
     def _product(self, kind: _Product, k: int, x, bias, out, scratch, scale=None, block=None) -> torch.Tensor:
         """matvec, matmul, matvec_fp8 and matmul_fp8: the checks and the call."""

@@ -56,7 +56,7 @@ import torch
 import torch.nn.functional as F
 
 from . import prefetch as _prefetch
-from .plan import _HEAD, MATMUL_MAX_TOKENS, MATVEC_MAX_TOKENS, DecodePlan, _Stream
+from .plan import _HEAD, EXPERTS_MATVEC_MAX_TOKENS, MATMUL_MAX_TOKENS, MATVEC_MAX_TOKENS, DecodePlan, _Stream
 from .safetensors_io import _FileRange, _cuda_device, compress_groups, file_entries, save_coded
 from .util_safetensors import COMPRESSION_METHOD
 from .zipnn import DecodePipe, ZipNN
@@ -115,11 +115,13 @@ class _Options(NamedTuple):
     experts: bool
     fp8: bool
     fp8_matmul: int  # the most input rows an "fp8" module multiplies on tensor cores without dequantizing (0: none)
+    experts_matvec: int  # the most tokens an "fp8_experts_matvec" module multiplies from its streams (0: none)
 
 
-def _options(prefetch=False, gather=False, matvec=0, matmul=0, experts=False, fp8=False, fp8_matmul=0) -> _Options:
-    """ValueError for a row count out of range, for fp8_matmul without fp8=True and for a mode that does not combine
-    with prefetch=True."""
+def _options(prefetch=False, gather=False, matvec=0, matmul=0, experts=False, fp8=False, fp8_matmul=0,
+             experts_matvec=0) -> _Options:
+    """ValueError for a row count out of range, for fp8_matmul without fp8=True, for experts_matvec without fp8=True
+    and experts=True, and for a mode that does not combine with prefetch=True."""
     for name, n, limit in (("matvec", matvec, MATVEC_MAX_TOKENS), ("matmul", matmul, MATMUL_MAX_TOKENS),
                            ("fp8_matmul", fp8_matmul, MATMUL_MAX_TOKENS)):
         if not (isinstance(n, int) and 0 <= n <= limit):
@@ -133,7 +135,12 @@ def _options(prefetch=False, gather=False, matvec=0, matmul=0, experts=False, fp
         raise ValueError("fp8=True and prefetch=True do not combine yet: the prefetch schedule decodes every module")
     if fp8_matmul and not fp8:
         raise ValueError("fp8_matmul applies to the fp8 modules of fp8=True: pass fp8=True with it")
-    return _Options(bool(prefetch), bool(gather), matvec, matmul, bool(experts), bool(fp8), fp8_matmul)
+    if not (isinstance(experts_matvec, int) and not isinstance(experts_matvec, bool) and 0 <= experts_matvec <= EXPERTS_MATVEC_MAX_TOKENS):
+        raise ValueError(f"experts_matvec must be an integer from 0 to {EXPERTS_MATVEC_MAX_TOKENS}, not {experts_matvec!r}")
+    if experts_matvec and not (fp8 and experts):
+        raise ValueError("experts_matvec applies to the fp8 experts modules of fp8=True with experts=True: pass fp8=True and "
+                         "experts=True with it")
+    return _Options(bool(prefetch), bool(gather), matvec, matmul, bool(experts), bool(fp8), fp8_matmul, experts_matvec)
 
 
 class _Entry(NamedTuple):
@@ -142,7 +149,7 @@ class _Entry(NamedTuple):
     plan: DecodePlan
     names: list   # [(name, index into the plan's outputs)]
     mode: str     # hooks: "decode", "prefetch", "experts"; a forward of its own: "matvec", "matmul", "fp8", "fp8_torch",
-                  # "fp8_experts", "fp8_experts_torch"
+                  # "fp8_experts", "fp8_experts_torch", "fp8_experts_matvec"
 
 
 class _Resident:
@@ -171,6 +178,9 @@ class _Resident:
         self.fp8_matmul = 0            # fp8_matmul=N: the most input rows an "fp8" module multiplies by matmul_fp8
         self.fp8_matmul_scratch = None  # the "fp8" modules' matmul_fp8 scratch and what the largest needs of it
         self.fp8_matmul_scratch_bytes = 0
+        self.experts_matvec = 0        # experts_matvec=N: the most tokens an "fp8_experts_matvec" module multiplies from its streams
+        self.experts_matvec_scratch = None  # their experts_matvec_fp8 scratch and what the largest needs of it
+        self.experts_matvec_scratch_bytes = 0
 
 
 def _grad_mode_error(mod, shared: bool = False):
@@ -287,6 +297,26 @@ def fp8_experts(module: torch.nn.Module) -> bool:
         if tuple(s.shape) != grid:
             return False
     return True
+
+
+def experts_matvec_layout(module: torch.nn.Module):
+    """The projections of an `fp8_experts` module in one of transformers' `FP8Experts` layouts, which experts_matvec=N
+    multiplies from the streams: -> (first, "down_proj"), first = "gate_up_proj" [E, 2I, H], gated by the module's
+    `_apply_gate`, or "up_proj" [E, I, H] (an FP8Experts built with has_gate=False), activated by its `act_fn`, and
+    down_proj [E, H, I]; None for any other module.  The parameters decide, not the `has_gate` attribute: transformers
+    sets it True whatever the constructor was given."""
+    if not fp8_experts(module):
+        return None
+    params = {name: p for name, p in module._parameters.items() if p is not None and p.dtype in _FP8}
+    gate = "gate_up_proj" in params
+    first = "gate_up_proj" if gate else "up_proj"
+    if sorted(params) != sorted([first, "down_proj"]) or not callable(getattr(module, "_apply_gate" if gate else "act_fn", None)):
+        return None
+    f, d = params[first].shape, params["down_proj"].shape
+    inter = f[1] // 2 if gate else f[1]
+    if (gate and f[1] % 2) or f[0] != d[0] or d[1] != f[2] or d[2] != inter:
+        return None
+    return first, "down_proj"
 
 
 def dequantize_fp8(weight: torch.Tensor, scale: torch.Tensor, block, dtype: torch.dtype) -> torch.Tensor:
@@ -429,6 +459,41 @@ def _fp8_experts_forward(mod, state, plan, names, fast: bool):
     return forward
 
 
+def _fp8_experts_matvec_forward(mod, state, plan, names):
+    """The forward of an "fp8_experts_matvec" module: the inputs the fast path of `_fp8_experts_forward` takes, with at
+    most `state.experts_matvec` rows of hidden_states [T, H] and ids [T, k], are multiplied by the routed experts
+    straight from the streams, nothing bound and the shared output buffer untouched: h = experts_matvec_fp8 of the first
+    projection with x [T, H]; the gate (`_apply_gate`) or the activation; d = experts_matvec_fp8 of down_proj with x
+    [T, k, I]; then FP8Experts.forward's combine, d times the routing weights in d's dtype, in fp32 summed over the k
+    slots in ascending order, back to the input's dtype.  Every other input goes to `_fp8_experts_forward` as before."""
+    fallback = _fp8_experts_forward(mod, state, plan, names, True)
+    block = _fp8_block(mod)
+    first, down = experts_matvec_layout(mod)
+    where = dict(names)
+    kf, kd = where[first], where[down]
+
+    def forward(*args, **kwargs):
+        hidden = args[0] if args else kwargs.get("hidden_states")
+        ids = args[1] if len(args) > 1 else kwargs.get("top_k_index")
+        weights = args[2] if len(args) > 2 else kwargs.get("top_k_weights")
+        if not (not torch.is_grad_enabled() and isinstance(ids, torch.Tensor) and ids.is_cuda and ids.device == plan.device
+                and ids.dtype in (torch.int32, torch.int64) and ids.dim() == 2 and isinstance(hidden, torch.Tensor)
+                and hidden.dtype in (torch.bfloat16, torch.float16) and hidden.device == plan.device and hidden.dim() == 2
+                and hidden.shape[0] == ids.shape[0] <= state.experts_matvec and isinstance(weights, torch.Tensor)
+                and not torch.is_autocast_enabled(plan.device.type)):
+            return fallback(*args, **kwargs)
+        scratch = state.experts_matvec_scratch
+        h = plan.experts_matvec_fp8(kf, ids, hidden, getattr(mod, first + "_scale_inv"), block, scratch=scratch)
+        a = mod._apply_gate(h) if first == "gate_up_proj" else mod.act_fn(h)
+        d = plan.experts_matvec_fp8(kd, ids, a, getattr(mod, down + "_scale_inv"), block, scratch=scratch)
+        wd = (d * weights.to(d.dtype)[..., None]).to(torch.float32)
+        acc = torch.zeros(wd.shape[0], wd.shape[2], dtype=torch.float32, device=wd.device)
+        for j in range(wd.shape[1]):
+            acc += wd[:, j]
+        return acc.to(hidden.dtype)
+    return forward
+
+
 def _matvec_forward(mod, state, plan, k, names, dtype, device, matmul: int = 0):
     """The forward of a matvec module: an input of at most `state.matvec` rows (a host-side test of its shape) that has
     the weight's `dtype` and `device`, outside autocast, goes to `plan.matvec`; one of more rows and at most `matmul`
@@ -565,6 +630,9 @@ def _resident_state(modules, groups, streams: dict, buffers: list, dev, opts: _O
             block = _fp8_block(m)
             fast = plan.select_ok() and plan.dequant_fp8_select_ok([o.shape[-1] for o in plan.outputs])
             mode = "fp8_experts" if fast and (block is None or block[1] % 16 == 0) else "fp8_experts_torch"
+            if mode == "fp8_experts" and opts.experts_matvec and experts_matvec_layout(m) is not None and all(
+                    plan.experts_matvec_fp8_ok(k, plan.outputs[k].shape[-1]) for _, k in local):
+                mode = "fp8_experts_matvec"
         elif opts.experts and experts_module(m, [n for n, _ in local]) and plan.select_ok():
             mode = "experts"
         else:
@@ -632,6 +700,13 @@ def _commit(module: torch.nn.Module, state: _Resident, opts: _Options) -> None:
     if fp8 and opts.fp8_matmul:
         state.fp8_matmul_scratch_bytes = max(e.plan.matmul_fp8_scratch_bytes(0, e.module.in_features, opts.fp8_matmul) for e in fp8)
         state.fp8_matmul_scratch = _plans_scratch_or_own(state, state.fp8_matmul_scratch_bytes)
+    state.experts_matvec = opts.experts_matvec
+    em = [e for e in state.entries if e.mode == "fp8_experts_matvec"]
+    if em:   # (top_k = E bounds the pair tables of any routing)
+        state.experts_matvec_scratch_bytes = max(e.plan.experts_matvec_fp8_scratch_bytes(k, e.plan.outputs[k].shape[-1], e.module.num_experts,
+                                                                                           opts.experts_matvec)
+                                                 for e in em for _, k in e.names)
+        state.experts_matvec_scratch = _plans_scratch_or_own(state, state.experts_matvec_scratch_bytes)
     for key, (m, plan, names, mode) in enumerate(state.entries):
         if mode in ("matvec", "matmul"):   # no hooks: its forward decides per input whether anything is decoded
             m.__dict__["forward"] = _matvec_forward(m, state, plan, 0, names, plan.outputs[0].dtype, plan.device,
@@ -640,6 +715,8 @@ def _commit(module: torch.nn.Module, state: _Resident, opts: _Options) -> None:
             m.__dict__["forward"] = _fp8_forward(m, state, plan, 0, names, mode == "fp8")
         elif mode in ("fp8_experts", "fp8_experts_torch"):   # its forward binds the dequantized weights itself
             m.__dict__["forward"] = _fp8_experts_forward(m, state, plan, names, mode == "fp8_experts")
+        elif mode == "fp8_experts_matvec":   # no binding at all for a few tokens; more take the "fp8_experts" forward
+            m.__dict__["forward"] = _fp8_experts_matvec_forward(m, state, plan, names)
         else:
             if mode == "experts":
                 pre = m.register_forward_pre_hook(_pre_hook_experts(plan, names, state), with_kwargs=True)
@@ -657,7 +734,7 @@ def _commit(module: torch.nn.Module, state: _Resident, opts: _Options) -> None:
 
 
 def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = False, gather: bool = False, matvec: int = 0,
-                    matmul: int = 0, experts: bool = False, fp8: bool = False, fp8_matmul: int = 0) -> dict:
+                    matmul: int = 0, experts: bool = False, fp8: bool = False, fp8_matmul: int = 0, experts_matvec: int = 0) -> dict:
     """Compress the weights of `modules` (default: every submodule that directly owns bf16 / fp16 / fp32 / fp8
     parameters) into streams kept in HBM, decoded just before each module's forward.  All parameters are compressed
     in one `compress_batch` call and must be on one CUDA device.
@@ -739,8 +816,16 @@ def compress_module(module: torch.nn.Module, modules=None, prefetch: bool = Fals
     read back): F.linear of the same dequantized weight, with the fp32 sums in another order.  Inputs of at most
     `matvec` rows still take matvec_fp8, larger ones dequant_fp8 + F.linear.  The report gains "fp8_matmul_modules" and
     "fp8_matmul_scratch_bytes" (one scratch for all of them, the plans' one when it is large enough).  ValueError
-    without fp8=True and together with prefetch=True."""
-    opts = _options(prefetch, gather, matvec, matmul, experts, fp8, fp8_matmul)
+    without fp8=True and together with prefetch=True.
+
+    experts_matvec=N (0 .. EXPERTS_MATVEC_MAX_TOKENS; 0, the default, changes nothing): with fp8=True and experts=True,
+    an "fp8_experts" module in one of transformers' `FP8Experts` layouts (`experts_matvec_layout`) whose plan
+    `DecodePlan.experts_matvec_fp8_ok` accepts for both projections runs as "fp8_experts_matvec": bf16 / fp16 inputs of
+    at most N tokens are multiplied by the routed experts straight from the streams (`DecodePlan.experts_matvec_fp8`,
+    no weight written or bound), then gated and combined as FP8Experts.forward does; larger inputs take the
+    "fp8_experts" forward.  The report gains "experts_matvec_modules" and "experts_matvec_scratch_bytes" (one scratch
+    for all of them, the plans' one when it is large enough).  ValueError without both fp8=True and experts=True."""
+    opts = _options(prefetch, gather, matvec, matmul, experts, fp8, fp8_matmul, experts_matvec)
     if getattr(module, _ATTR, None) is not None:
         raise ValueError("compress_module: this module is already compressed")
     modules, groups = select(module, modules)
@@ -782,11 +867,14 @@ def _with_prefetch(report: dict, state, opts: _Options) -> dict:
                       experts_scratch_bytes=0 if state.select_scratch is None else state.select_scratch.numel())
     if opts.fp8:
         report.update(fp8_modules=modes.count("fp8") + modes.count("fp8_torch"), fp8_scratch_bytes=state.fp8_scratch_bytes)
-    fp8_experts_modules = modes.count("fp8_experts") + modes.count("fp8_experts_torch")
+    fp8_experts_modules = modes.count("fp8_experts") + modes.count("fp8_experts_torch") + modes.count("fp8_experts_matvec")
     if fp8_experts_modules:   # (only fp8=True with experts=True makes them; a model without one keeps its report)
         report.update(fp8_experts_modules=fp8_experts_modules)
     if opts.fp8_matmul:
         report.update(fp8_matmul_modules=modes.count("fp8"), fp8_matmul_scratch_bytes=state.fp8_matmul_scratch_bytes)
+    if opts.experts_matvec:
+        report.update(experts_matvec_modules=modes.count("fp8_experts_matvec"),
+                      experts_matvec_scratch_bytes=state.experts_matvec_scratch_bytes)
     return report
 
 
@@ -809,7 +897,7 @@ def decompress_module(module: torch.nn.Module) -> None:
     for h in state.hooks:
         h.remove()
     for m, _, _, mode in state.entries:
-        if mode in ("matvec", "matmul", "fp8", "fp8_torch", "fp8_experts", "fp8_experts_torch"):   # the modes whose forward _commit replaced
+        if mode in ("matvec", "matmul", "fp8", "fp8_torch", "fp8_experts", "fp8_experts_torch", "fp8_experts_matvec"):   # the modes whose forward _commit replaced
             m.__dict__.pop("forward", None)
     for m, _, _, _ in state.gathers:
         m.__dict__.pop("forward", None)
@@ -1063,7 +1151,7 @@ def _load_device(plan: LoadPlan, dev, opts: _Options) -> tuple:
 
 def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None, prefetch: bool = False,
                 gather: bool = False, matvec: int = 0, matmul: int = 0, experts: bool = False, fp8: bool = False,
-                fp8_matmul: int = 0) -> dict:
+                fp8_matmul: int = 0, experts_matvec: int = 0) -> dict:
     """Load a checkpoint into `module` with the weights of `modules` kept compressed on `device`: the state
     `compress_module` leaves (same selection rules, hooks, plans and report), reached without a dense copy of those
     weights on the GPU.
@@ -1098,10 +1186,10 @@ def load_module(module: torch.nn.Module, filenames, device="cuda", modules=None,
     and the batched decode's workspace; plain entries add one group at a time: its input, its streams' bound and the
     compress workspace.  A model loaded from .znn files never has its compressed weights dense on the device.
 
-    prefetch, gather, matvec, matmul, experts, fp8, fp8_matmul: as for `compress_module`.
+    prefetch, gather, matvec, matmul, experts, fp8, fp8_matmul, experts_matvec: as for `compress_module`.
 
     -> the report of `compress_module`."""
-    opts = _options(prefetch, gather, matvec, matmul, experts, fp8, fp8_matmul)
+    opts = _options(prefetch, gather, matvec, matmul, experts, fp8, fp8_matmul, experts_matvec)
     dev = _cuda_device(device)
     if dev is None:
         raise ValueError(f"load_module: {device!r} is not a CUDA device")
