@@ -144,8 +144,12 @@ def _quantized(fmt, out, inn, seed):
     return (w / full).to(F.TORCH[fmt]), scale
 
 
-def _check64(y, x, wq, scale, bias, what):
-    wd = wq.double() * scale.double().repeat_interleave(128, 0)[: wq.shape[0]].repeat_interleave(128, 1)[:, : wq.shape[1]]
+def _check64(y, x, wq, scale, bias, what, block=(128, 128)):
+    """y against fp64 x (S W)^T (+ bias), S the grid of (bn, bk) blocks (a block larger than W is the whole of it)."""
+    out, inn = wq.shape
+    bn, bk = min(block[0], out), min(block[1], inn)
+    s = scale.double().reshape(-(-out // bn), -(-inn // bk))
+    wd = wq.double() * s.repeat_interleave(bn, 0)[:out].repeat_interleave(bk, 1)[:, :inn]
     x64 = x.double().reshape(-1, x.shape[-1])
     ref, mag = x64 @ wd.T, x64.abs() @ wd.abs().T
     if bias is not None:
